@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of the RPBCAC training hot path (BASELINE.json metric: agent-updates/sec).
 
-  python bench.py --gpus 1 --steps K --warmup W              our arm (B200 kernels)
+  python bench.py --gpus 1 --steps K --warmup W              our arm (sm_90a kernels)
+  python bench.py ... --dump-outputs DIR                     also write what the last timed step computed, DIR/<name>.npy
   python bench.py --impl reference --gpus N --steps K ...    CPU arm: the oracle port of the reference on host cores
   torchrun ... bench.py --gpus N ...                         one rank per GPU, env batch sharded (weak scaling)
 
@@ -12,7 +13,7 @@ agent-updates per step = n_agents * n_envs * max_ep_len * n_ep_fixed (SURVEY 8d)
 
 Workload (config.workload = "C2"): BASELINE.json configs[1] -- 5x5 grid, 4 cooperative + 1 malicious agent,
 H = 1, 4096 parallel environments per GPU, reference hyper-parameters (main.py:31-40, slow_lr 0.002).
-Inputs are larger than L2 (steady-state buffer 1.47 GB >> 126 MB), so no explicit L2 flush is needed.
+Inputs are larger than L2 (steady-state buffer 1.47 GB >> 50 MB), so no explicit L2 flush is needed.
 """
 import argparse
 import json
@@ -69,7 +70,7 @@ def workload(name, n_envs):
 
 # --------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampled DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled DURING the timed region: the SM clock the numbers were taken at, and any throttling."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -116,24 +117,11 @@ class ClockSampler:
         return out
 
 
-def grad_traffic(workload_name):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one full-batch gradient launch from the committed `ncu --set full`
-    capture (profiles/r02_grad_traffic.json); only valid for the workload it was captured on."""
-    if workload_name != "C2":
-        return None
-    for name in ("r02_grad_traffic.json", "r01_grad_traffic.json"):
-        try:
-            return json.load(open(os.path.join(ROOT, "profiles", name)))["traffic_bytes"]
-        except Exception:
-            continue
-    return None
-
-
 def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, sm_max_mhz=1965.0), "fallback"
+        return dict(hbm_gbs=3350.0, bf16_tflops=989.0, sm_max_mhz=1980.0), "H100 SXM data sheet"
 
 
 # --------------------------------------------------------------------------------------------- CPU arm
@@ -213,6 +201,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-consensus", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -278,8 +268,10 @@ def main():
     tr.rollout_block()
     tr.rollout_block()
 
+    last = {}
+
     def step():
-        tr.rollout_block()
+        last["est"], last["ret"] = tr.rollout_block()
         tr.update_round()
 
     for _ in range(args.warmup):
@@ -301,6 +293,8 @@ def main():
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms = float(ms.item())
     clk = clocks.stop() if rank == 0 else {}
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, tr, last)
     launches = tr.launches - l0
     # every rank must hold bit-identical replicated parameters after the timed region (weak scaling means nothing if the
     # replicas drifted apart): all-gather the packed parameters and compare with rank 0's
@@ -330,13 +324,10 @@ def main():
         # SURVEY 8(d): MAC per buffer row of one fused forward + backward: critic 1 660, team reward 1 860 at 5 agents
         mac_net = lambda d: (d * 20 + 400 + 20) + (d * 20 + 840)
         d_c, d_t = 2 * NA, 3 * NA
-        try:
-            fp32_peak = json.load(open(os.path.join(ROOT, "profiles", "r01_fp32_peak.json")))["fp32_tflops"]
-            fp32_src = ("builder-measured on this pool (FFMA2 issue-rate loop, profiles/r01_peak_rates.md); nominal "
-                        "2*128*148*1.965 GHz = 74.4; MEASURED_PEAKS.json has no fp32 entry")
-        except Exception:
-            fp32_peak = 2 * 128 * 148 * (peaks.get("sm_max_mhz", 1965.0) * 1e6) / 1e12
-            fp32_src = "nominal 2*128 lanes*148 SMs*max SM clock"
+        n_sm = torch.cuda.get_device_properties(local_rank).multi_processor_count
+        sm_mhz = clk.get("sm_max_mhz") or peaks.get("sm_max_mhz", 1980.0)
+        fp32_peak = 2 * 128 * n_sm * (sm_mhz * 1e6) / 1e12
+        fp32_src = f"nominal 2*128 lanes*{n_sm} SMs*{sm_mhz:.0f} MHz max SM clock"
         # regime 1: the full-batch local fits (rcmarl_grad over the whole buffer, 2 nets per cooperative agent)
         alg_bytes = 20 * NA * rows_fit                       # SURVEY 8(d): 20*n_agents B per row per lock-step GD step
         flops_fit = 2.0 * n_coop * (mac_net(d_c) + mac_net(d_t)) * rows_fit
@@ -361,14 +352,12 @@ def main():
             t_tot += float(np.sum(prof["minibatch_sgd"]))
             f_tot += flops_call * len(prof["minibatch_sgd"])
         tf_w = f_tot / (t_tot * 1e-3) / 1e12
-        kname = ("grad_kernel_ws + mb_persist_ws_kernel (warp-specialised tcgen05 3xTF32 + FFMA2 fused MLP forward/backward; "
-                 "rcmarl_grad + rcmarl_minibatch_fit)") if tr.NA == 5 else \
-            f"grad_kernel<{tr.NA},MSE> (FFMA2 fused MLP forward/backward; rcmarl_grad + rcmarl_minibatch_fit)"
+        kname = (f"grad_kernel<{tr.NA},MSE> + mb_persist_kernel<{tr.NA}> (FFMA fused MLP forward/backward; "
+                 "rcmarl_grad + rcmarl_minibatch_fit)")
         roof = dict(kernel=kname,
                     bound="fp32", achieved=tf_w, peak=fp32_peak, unit="TFLOP/s", frac=tf_w / fp32_peak,
                     frac_is="time-weighted over both regimes of the kernel (full-batch fits + mini-batch chains)",
-                    share_of_step=t_tot / ms, traffic=grad_traffic(args.workload),
-                    traffic_note="DRAM bytes of ONE full-batch launch (ncu --set full); compare with hbm_view.algorithmic_bytes_per_launch",
+                    share_of_step=t_tot / ms,
                     peak_source=fp32_src, regimes=regimes,
                     hbm_view=dict(achieved=alg_bytes / (fit_ms * 1e-3) / 1e9, peak=peaks["hbm_gbs"], unit="GB/s",
                                   frac=alg_bytes / (fit_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
@@ -382,7 +371,7 @@ def main():
     if rank == 0 and not args.no_consensus:
         g = torch.Generator(device="cuda")
         g.manual_seed(0)
-        # three rotating inputs of 272 MB each: every launch reads data that the 126 MB L2 cannot still hold
+        # three rotating inputs of 272 MB each: every launch reads data that the 50 MB L2 cannot still hold
         Xs = [torch.randn(64, 1 << 20, device="cuda", generator=g) for _ in range(3)]
         out = torch.empty(1 << 20, device="cuda")
         cons = {}
@@ -433,6 +422,18 @@ def main():
     if world > 1:
         dist.destroy_process_group()
     return 0
+
+
+def dump_outputs(out_dir, tr, last):
+    """What a caller of the timed path holds after its last step: the per-episode means that rollout_block returned
+    (estimated and true discounted returns, [n_ep, n_agents]) and the packed parameters update_round left behind
+    ([n_agents, n_params] per net).  The parameters are what every later step computes from."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = dict(rollout_est_returns=last["est"], rollout_true_returns=last["ret"], actor=tr.actor, critic=tr.critic,
+                  team_reward=tr.tr, critic_local=tr.critic_local)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def e2e_arm(cfg, args, rank, world, tr):

@@ -1,4 +1,4 @@
-/* rcmarl.h -- C ABI of librcmarl.so: the sm_100a kernels behind the RPBCAC
+/* rcmarl.h -- C ABI of librcmarl.so: the sm_90a kernels behind the RPBCAC
  * training hot path (reference: mfigura/Resilient-consensus-based-MARL).
  *
  * The reference has no FFI layer: its boundary is the duck-typed Python Agent

@@ -1,5 +1,5 @@
 """Adversarial agents with the reference's API (agents/adversarial_CAC_agents.py of
-mfigura/Resilient-consensus-based-MARL) on the sm_100a kernels of librcmarl.so.
+mfigura/Resilient-consensus-based-MARL) on the sm_90a kernels of librcmarl.so.
 
   Faulty_CAC_agent     :5-72    transmits fixed critic / TR parameters, trains only its actor
   Malicious_CAC_agent  :74-182  private local critic + compromised critic / TR trained on -r_coop and transmitted

@@ -1,5 +1,5 @@
 """RPBCAC_agent with the reference's API (agents/resilient_CAC_agents.py:5-223 of
-mfigura/Resilient-consensus-based-MARL), executed by the sm_100a kernels of librcmarl.so.
+mfigura/Resilient-consensus-based-MARL), executed by the sm_90a kernels of librcmarl.so.
 
 Same constructor and method names, argument meaning and mutation conventions as the reference (SURVEY.md 8b):
   *_update_local            return (message copy, loss) and leave the agent's own networks untouched (:113,120)

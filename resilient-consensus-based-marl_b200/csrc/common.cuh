@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the RPBCAC sm_100a kernels.
+// common.cuh -- shared device helpers for the RPBCAC sm_90a kernels.
 // Network layout and math follow main.py:60-82 (Dense 20 / LeakyReLU(0.1)), see include/rcmarl.h.
 #pragma once
 #include <cuda_runtime.h>
@@ -169,33 +169,20 @@ __device__ __forceinline__ float clip_mean_small(const float (&v)[MAXN], int n, 
     return s / (float)n;
 }
 
-// Blackwell packed fp32 FMA (fma.rn.f32x2 -> SASS FFMA2): two IEEE fp32 FMAs per issue slot.
-typedef unsigned long long f2;
-__device__ __forceinline__ f2 pack2(float lo, float hi) {
-    f2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
+// A pair of fp32 values (two adjacent hidden units, or two accumulators) updated together.  Hopper has no packed fp32
+// FMA, so a pair operation is two IEEE fp32 FMAs (FFMA); the values are the same as one packed operation would give.
+typedef float2 f2;
+__device__ __forceinline__ f2 pack2(float lo, float hi) { return make_float2(lo, hi); }
 __device__ __forceinline__ void unpack2(f2 v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+    lo = v.x;
+    hi = v.y;
 }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-    f2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-
-// in-place form: the accumulator is tied to one register pair ("+l"), so ptxas cannot route a loop-carried accumulator through
-// a freshly loaded operand register and copy it back (17 MOVs per 40 FFMA2 in the consumer loop of grad_kernel_ws otherwise)
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ void fma2_acc(f2& acc, f2 a, f2 b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
+    acc.x = fmaf(a.x, b.x, acc.x);
+    acc.y = fmaf(a.y, b.y, acc.y);
 }
-
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-    f2 d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // Where a kernel reads the packed network parameters from: the CTA's staged copy in shared memory (uniform LDS.128,
 // 2 shared-memory wavefronts per quad).  The accessor keeps the dense-layer code independent of the source; a constant-
@@ -210,7 +197,7 @@ struct SmemW {
 #define RCMARL_LRELU_MAX 1
 #endif
 // LeakyReLU of a packed pair.  slope in (0, 1) => lrelu(z) == max(z, slope * z) bit for bit (z > 0: slope*z < z;
-// z < 0: slope*z > z; +-0 and NaN map to themselves), which is FMUL2 + 2 FMNMX instead of 2 x (FMUL, FSETP, FSEL).
+// z < 0: slope*z > z; +-0 and NaN map to themselves), which is 2 x (FMUL, FMNMX) instead of 2 x (FMUL, FSETP, FSEL).
 __device__ __forceinline__ void lrelu_pair(f2 z, float& a, float& b) {
     float za, zb;
     unpack2(z, za, zb);
@@ -225,7 +212,7 @@ __device__ __forceinline__ void lrelu_pair(f2 z, float& a, float& b) {
 #endif
 }
 
-// z[r][:] = b + x[r] W for R rows at once: every weight quad feeds 2*R FFMA2; outputs are packed as pairs of adjacent
+// z[r][:] = b + x[r] W for R rows at once: every weight quad feeds 4*R FFMA; outputs are packed as pairs of adjacent
 // hidden units.  `w` is the parameter source (SmemW), offW / offb the offsets of W [K][20] and b [20] in it.
 template <int K, int R, class WS>
 __device__ __forceinline__ void dense20_rows(const WS& w, int offW, int offb, const float (&x)[R][K],

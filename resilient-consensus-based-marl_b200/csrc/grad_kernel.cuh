@@ -2,9 +2,9 @@
 // (rcmarl_grad, include/rcmarl.h; replaces the fwd/bwd inside critic.fit / TR.fit / actor.train_on_batch,
 // agents/resilient_CAC_agents.py:99,118,136 and adversarial:41,116,133,150,163).
 //
-// The kernel is FP32-FMA work fed from shared memory, and on B200 the shared-memory pipe (one wavefront per
-// clock per SM) is the first limit: measured with ncu (profiles/r01_grad_kernel_ncu.md) a warp-uniform LDS.128 costs
-// 2 wavefronts and any other LDS.128 costs 4, while the four FMA pipes retire 4 warp-FFMAs per clock.  Balance
+// The kernel is FP32-FMA work fed from shared memory, and the shared-memory pipe (one wavefront per clock per SM) is
+// the first limit: a warp-uniform LDS.128 costs 2 wavefronts and any other LDS.128 costs 4, while the four FMA pipes
+// retire 4 warp-FFMAs per clock.  Balance
 // therefore needs >= 4 FFMA per wavefront everywhere:
 //   phase 1 (forward + backward-data): every lane carries R = 2 buffer rows, so each broadcast weight quad
 //            (uniform LDS.128, 2 wavefronts) feeds 8 FFMA;
@@ -139,14 +139,13 @@ struct GradParams {
 };
 
 // 1: the constant columns of the tile rows ([.., 1, 0 pad], zero pads of the deltas) are written once per kernel instead of
-//    once per chunk (3-4 of 22 STS.128 per row).  Measured on B200 together with RCMARL_LRELU_MAX: 10.53 -> 10.30 ms per
-//    full-batch launch, results bit-identical (tools/ab_grad.py).
+//    once per chunk (3-4 of 22 STS.128 per row).  Results bit-identical (tools/ab_grad.py).
 #ifndef RCMARL_PAD_HOIST
 #define RCMARL_PAD_HOIST 1
 #endif
 // 1: the CTA signals its programmatic dependents (the reduce kernel of the same mini-batch step, launched with the PDL
 //    attribute) once its row loop is done, so the reduce grid is already queued when the last CTA exits; the reduce kernel
-//    waits for this grid with griddepcontrol.wait.  Measured on B200 (C2): 1192.9 -> 1175.1 ms per update round.
+//    waits for this grid with griddepcontrol.wait.
 // 1: warp-major assignment of 64-row chunks to (CTA, warp), see grad_body (not yet measured on the GPU: added after the
 //    round-1 GPU budget was spent; 0 restores the measured CTA-major order)
 #ifndef RCMARL_CHUNK_WARP_MAJOR

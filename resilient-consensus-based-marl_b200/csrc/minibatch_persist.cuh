@@ -20,12 +20,6 @@
 #pragma once
 #include "grad_kernel.cuh"
 #include "comm.cuh"
-#ifndef RCMARL_GRAD_WS
-#define RCMARL_GRAD_WS 1
-#endif
-#if RCMARL_GRAD_WS
-#include "grad_kernel_ws.cuh"
-#endif
 
 namespace rcmarl {
 
@@ -152,178 +146,5 @@ mb_persist_kernel(const __grid_constant__ MbParams P) {
     if (ch.kind == RCMARL_IN_SA) mb_body<NA, 3 * NA, NW>(P, ch, j, smem, y, gy);
     else mb_body<NA, 2 * NA, NW>(P, ch, j, smem, y, gy);
 }
-
-#if RCMARL_GRAD_WS
-// =====================================================================================================================
-// The same persistent fit on the warp-specialised tensor-core core (grad_kernel_ws.cuh), n_agents = 5.  Both roles run the
-// same step loop with the role branch inside the step; every CTA-wide barrier sits behind that branch (one program location).
-// =====================================================================================================================
-struct MbStepCtx {
-    uint2* my1;                 // this CTA's level-1 cells
-    const uint2* chain1;        // level-1 cells of the chain's first CTA
-    const CommDev* comm;
-    int64_t off2;               // the chain's block in the level-2 cells
-    int32_t gy, stride, sl_begin, sl_end, S, sgroup, e_local, e_per_warp;
-    float loss_coef;
-};
-
-// sums of this step -> level-1 cells -> slice owner's CTA-ordered sum -> level-2 cells -> SGD step on the shared-memory copy
-template <int DIN>
-__device__ __forceinline__ void mb_step_tail(const WsShared& S, const MbStepCtx& c, uint32_t s1, uint32_t s2, float coef,
-                                             bool first_epoch, float& loss_acc, bool mb_tl_on = false, int mb_tl_step = 0) {
-    constexpr int NP = param_count(DIN, 1);
-    const int warp = threadIdx.x >> 5;
-    uint2* my1 = c.my1;
-    ws_cta_sums<DIN>(S, [my1, s1](int i, float v) { st_cell(my1 + i, v, s1); });
-    MB_TICK(5);
-    for (int base = c.sl_begin + warp * c.e_per_warp; base < c.sl_end; base += WS_WARPS * c.e_per_warp) {
-        const int i = base + c.e_local;
-        float s = 0.f;
-        if (i < c.sl_end) {
-            for (int yy = c.sgroup; yy < c.gy; yy += c.S)
-                s += __uint_as_float(poll_cell(c.chain1 + (int64_t)yy * c.stride + i, s1, c.comm->error).x);
-        }
-        for (int o = 1; o < c.S; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (i < c.sl_end && c.sgroup == 0) comm_push(*c.comm, c.off2 + i, s, s2);
-    }
-    MB_TICK(6);
-    for (int i = threadIdx.x; i <= NP; i += WS_THREADS) {
-        const float tot = comm_wait_total(*c.comm, c.off2 + i, s2);
-        if (i < NP) S.sw[i] = S.sw[i] - coef * tot;
-        else if (first_epoch) loss_acc += c.loss_coef * tot;
-    }
-    MB_TICK(7);
-}
-
-template <int NA, int DIN>
-__device__ __forceinline__ void mb_body_ws(const MbParams& P, const MbChain& ch, int j, float* smem, int y, int gy) {
-    constexpr int NP = param_count(DIN, 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const WsShared S = ws_carve(smem);
-    ws_init(S);
-    pdl_wait();
-    stage_weights(S.sw, ch.w, NP);
-    __syncthreads();
-
-    rcmarl_grad_job gj;
-    gj.w = ch.w; gj.target = ch.target; gj.sums = nullptr; gj.time_idx = nullptr;
-    gj.target_stride = ch.target_stride; gj.kind = ch.kind; gj.action_agent = 0;
-    rcmarl_rows Rw = P.rows;
-
-    MbStepCtx c;
-    c.my1 = P.cells1 + (int64_t)blockIdx.x * P.stride;
-    c.chain1 = P.cells1 + (int64_t)P.cta_first[j] * P.stride;
-    c.comm = &P.comm;
-    c.off2 = (int64_t)j * P.stride;
-    c.gy = gy; c.stride = P.stride;
-    const int per = (NP + 1 + gy - 1) / gy;
-    c.sl_begin = y * per < NP + 1 ? y * per : NP + 1;
-    c.sl_end = c.sl_begin + per < NP + 1 ? c.sl_begin + per : NP + 1;
-    int Sl = 1;
-    while (Sl < gy && Sl < 32) Sl <<= 1;
-    c.S = Sl; c.sgroup = lane & (Sl - 1); c.e_local = lane / Sl; c.e_per_warp = 32 / Sl;
-    c.loss_coef = ch.loss_coef;
-    const int nb = (P.n_times + P.mb_times - 1) / P.mb_times;
-    const float world = (float)P.comm.world;
-    uint32_t seq1 = P.seq1, seq2 = P.comm.seq, nbase = 0;      // nbase: this stream's tiles so far (ring bookkeeping)
-    float loss_acc = 0.f;
-
-    // One step loop for both roles: the role branch sits INSIDE the step, every CTA-wide barrier behind it at one program
-    // location (nothing role-specific is live there: both roles have parked their sums by then).
-    const bool producer = warp < 4 * WS_GROUPS;
-    const int cw = warp - 4 * WS_GROUPS;
-    const int group = warp >> 2, prow = (warp & 3) * 32 + lane;      // producer group, row of the tile
-    uint32_t mph = 0;
-#if RCMARL_WS_TIMELINE
-    const bool mb_tl_on = blockIdx.x == 0 && threadIdx.x == 0;       // ticks 0 .. 9: first producer thread
-    int mb_tl_step = -1;
-#else
-    constexpr bool mb_tl_on = false;
-    constexpr int mb_tl_step = 0;
-#endif
-    // rows of step (e, b): a mini-batch is mb_times time rows x all environments of this rank
-    auto step_rows = [&](int e, int b, rcmarl_rows& R) {
-        const int cnt = P.n_times - b * P.mb_times < P.mb_times ? P.n_times - b * P.mb_times : P.mb_times;
-        R.n_rows = (int64_t)cnt * R.n_envs;
-        R.time_idx = ch.time_idx + (int64_t)e * P.n_times + (int64_t)b * P.mb_times;
-    };
-    WsFirst<DIN> nf;                                                  // first tile of the NEXT sweep, fetched one step ahead
-    nf.tgt = 0.f; nf.live = false;
-#pragma unroll
-    for (int k = 0; k < DIN; ++k) nf.x[k] = 0.f;
-    step_rows(0, 0, Rw);
-    if (producer && group < ws_tile_count(Rw.n_rows, y, gy)) ws_fetch<NA, DIN>(Rw, gj, y, gy, group, prow, nf.x, nf.tgt, nf.live);
-    for (int e = 0; e < P.epochs; ++e) {
-        for (int b = 0; b < nb; ++b, ++seq1, ++seq2) {
-#if RCMARL_WS_TIMELINE
-            ++mb_tl_step;
-#endif
-            MB_TICK(0);
-            ws_build_operands<DIN>(S);
-            __syncthreads();
-            MB_TICK(1);
-            tmem_fence_after_sync();
-            step_rows(e, b, Rw);
-            const int nq = ws_tile_count(Rw.n_rows, y, gy);
-            const float n_rows_f = (float)Rw.n_rows;
-            if (producer) {
-                float g3[HID + 1];
-#pragma unroll
-                for (int k = 0; k <= HID; ++k) g3[k] = 0.f;
-                float loss = 0.f;
-                ws_produce<NA, DIN, WS_SHADOW_STEP, true>(S, Rw, gj, y, gy, nq, nbase, mph, g3, loss, &nf);
-                {   // the next step's first rows: in flight during this step's reduction, exchange and SGD
-                    const int bn = b + 1 < nb ? b + 1 : 0, en = b + 1 < nb ? e : e + 1;
-                    if (en < P.epochs) {
-                        rcmarl_rows Rn = Rw;
-                        step_rows(en, bn, Rn);
-                        if (group < ws_tile_count(Rn.n_rows, y, gy)) ws_fetch<NA, DIN>(Rn, gj, y, gy, group, prow, nf.x, nf.tgt, nf.live);
-                    }
-                }
-                MB_TICK(2);
-                ws_park_producer(S, g3, loss);
-                MB_TICK(3);
-            } else {
-#if RCMARL_WS_TIMELINE
-                const bool mb_tl_on = blockIdx.x == 0 && threadIdx.x == 32 * 4 * WS_GROUPS;   // first consumer thread: ticks 10 .. 12
-#endif
-                f2 acc[WS_ACC];
-#pragma unroll
-                for (int k = 0; k < WS_ACC; ++k) acc[k] = pack2(0.f, 0.f);
-                ws_consume(S, cw, nq, nbase, acc);
-                MB_TICK(10);
-                named_barrier(WS_BAR_CONS, 32 * WS_CONS);             // every tile consumed
-                MB_TICK(11);
-                ws_park_consumer(S, cw, acc);
-                MB_TICK(12);
-            }
-            __syncthreads();                                          // scratch complete
-            MB_TICK(4);
-            mb_step_tail<DIN>(S, c, seq1, seq2, ch.lr * 2.0f / (n_rows_f * world), e == 0, loss_acc, mb_tl_on, mb_tl_step);
-            __syncthreads();                                          // new parameters visible; scratch reusable
-            MB_TICK(8);
-        }
-    }
-    if (y == 0) {
-        for (int i = threadIdx.x; i < NP; i += WS_THREADS) ch.w[i] = S.sw[i];
-        if (threadIdx.x == (NP % WS_THREADS) && ch.loss_out) *ch.loss_out = ch.loss_accumulate ? *ch.loss_out + loss_acc : loss_acc;
-    }
-    tmem_fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc_all(*S.tslot);
-}
-
-__global__ void __launch_bounds__(WS_THREADS, 1) mb_persist_ws_kernel(const __grid_constant__ MbParams P) {
-    extern __shared__ __align__(16) float smem[];
-    pdl_launch_dependents();
-    int j = 0;
-    while (j + 1 < P.n_chains && (int)blockIdx.x >= P.cta_first[j + 1]) ++j;
-    const MbChain& ch = P.chains[j];
-    const int y = (int)blockIdx.x - P.cta_first[j], gy = P.cta_first[j + 1] - P.cta_first[j];
-    if (ch.kind == RCMARL_IN_SA) mb_body_ws<5, 15>(P, ch, j, smem, y, gy);
-    else mb_body_ws<5, 10>(P, ch, j, smem, y, gy);
-}
-
-#endif  // RCMARL_GRAD_WS
 
 }  // namespace rcmarl

@@ -48,8 +48,8 @@ struct Track {
         large[H] = fmaxf(large[H], c);
     }
     // Two values at once for H == 1: sort the pair, then the two smallest of {small[0] <= small[1], lo <= hi} are
-    // min(small[0], lo) and min3(small[1], hi, max(small[0], lo)); likewise the two largest.  8 min / max per pair (three-input
-    // FMNMX3 for the second order statistic) instead of 12, same values and the same summation order as two push() calls.
+    // min(small[0], lo) and min3(small[1], hi, max(small[0], lo)); likewise the two largest.  10 min / max per pair instead
+    // of 12, same values and the same summation order as two push() calls.
     __device__ __forceinline__ void push2(float a, float b) {
         static_assert(H == 1, "pair update is written for H == 1");
         sum += a;
@@ -57,10 +57,10 @@ struct Track {
         const float lo = fminf(a, b), hi = fmaxf(a, b);
         const float m = fmaxf(small[0], lo);
         small[0] = fminf(small[0], lo);
-        asm("min.f32 %0, %0, %1, %2;" : "+f"(small[1]) : "f"(hi), "f"(m));
+        small[1] = fminf(fminf(small[1], hi), m);
         const float w = fminf(large[0], hi);
         large[0] = fmaxf(large[0], hi);
-        asm("max.f32 %0, %0, %1, %2;" : "+f"(large[1]) : "f"(lo), "f"(w));
+        large[1] = fmaxf(fmaxf(large[1], lo), w);
     }
     __device__ __forceinline__ void window(float own, float& lo, float& hi) const {
         lo = fminf(small[H], own);
@@ -469,7 +469,7 @@ using namespace rcmarl;
 
 extern "C" {
 
-const char* rcmarl_version(void) { return "rcmarl-b200 0.1 (sm_100a, fp32)"; }
+const char* rcmarl_version(void) { return "rcmarl-h100 0.1 (sm_90a, fp32)"; }
 
 const char* rcmarl_status_string(int s) {
     switch (s) {

@@ -1,4 +1,4 @@
-// train_kernels.cu -- update-round kernels of the RPBCAC hot path (sm_100a, fp32 FFMA).
+// train_kernels.cu -- update-round kernels of the RPBCAC hot path (sm_90a, fp32 FFMA).
 //
 //   values_kernel   K1/K3  batched forward values / TD targets / TD errors / actor probabilities
 //   grad_kernel     K2/K7/K9  fused forward + backward of the 20-wide MLPs over a row set (grad_kernel.cuh):
@@ -18,14 +18,6 @@
 #define RC_GRAD_KERNEL grad_kernel
 #define RC_GRAD_WARPS grad_warps
 #define RC_GRAD_SMEM grad_smem_floats
-// RCMARL_GRAD_WS (default 1): mean-squared-error jobs at n_agents = 5 run on the warp-specialised tensor-core kernel
-// (grad_kernel_ws.cuh); -DRCMARL_GRAD_WS=0 (make variant_ffma) keeps them on the FFMA2 kernel of round 1 (grad_kernel.cuh)
-#ifndef RCMARL_GRAD_WS
-#define RCMARL_GRAD_WS 1
-#endif
-#if RCMARL_GRAD_WS
-#include "grad_kernel_ws.cuh"
-#endif
 #include "comm.cuh"
 #include "minibatch_persist.cuh"
 
@@ -43,7 +35,7 @@ int sm_count_cached() {
             cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0)
             n = v;
         else
-            return 148;  // B200; not cached so that a later call with a device re-queries
+            return 132;  // H100 SXM; not cached so that a later call with a device re-queries
     }
     return n;
 }
@@ -262,7 +254,7 @@ struct TeamParams {
     int32_t stride;
     // jobs of THIS launch (blockIdx.x -> job index).  rcmarl_team launches the team-reward nets (15 inputs) and the critics
     // (10 inputs) separately: the loop body of one instantiation is ~24 KB of SASS, two of them resident on an SM overflow the
-    // 32 KB instruction cache (28 % of the stall samples were "no instruction", profiles/r02_ncu_other_kernels.md)
+    // instruction cache
     int32_t job_list[RCMARL_MAX_JOBS];
 };
 constexpr int TEAM_N = HID + 2;  // 20 weights + bias numerators + diagnostic loss
@@ -488,19 +480,6 @@ static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st
         cfg.blockDim = dim3(32 * NWC);
         cfg.dynamicSmemBytes = smem_ce;
         RC_CUDA(cudaLaunchKernelEx(&cfg, RC_GRAD_KERNEL<NA, RCMARL_LOSS_CE>, P));
-#if RCMARL_GRAD_WS
-    } else if (NA == 5) {
-        constexpr size_t smem_ws = sizeof(float) * ws_smem_floats();
-        static_assert(smem_ws <= 227 * 1024, "grad_kernel_ws exceeds the shared-memory limit");
-        static bool attr_ws = false;
-        if (!attr_ws) {
-            if (set_smem(grad_kernel_ws, smem_ws)) return RCMARL_ERR_CUDA;
-            attr_ws = true;
-        }
-        cfg.blockDim = dim3(WS_THREADS);
-        cfg.dynamicSmemBytes = smem_ws;
-        RC_CUDA(cudaLaunchKernelEx(&cfg, grad_kernel_ws, P));
-#endif
     } else {
         if (!attr_mse) {
             if (set_smem(RC_GRAD_KERNEL<NA, RCMARL_LOSS_MSE>, smem_mse)) return RCMARL_ERR_CUDA;
@@ -517,9 +496,6 @@ static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st
 // chunks (64 rows) one CTA of this configuration consumes per sweep
 template <int NA>
 static int grad_chunks_per_cta(int loss_mode) {
-#if RCMARL_GRAD_WS
-    if (NA == 5 && loss_mode == RCMARL_LOSS_MSE) return 2;      // one 128-row tile (= two 64-row chunks) at a time
-#endif
     return loss_mode == RCMARL_LOSS_CE ? RC_GRAD_WARPS<NA, RCMARL_LOSS_CE>() : RC_GRAD_WARPS<NA, RCMARL_LOSS_MSE>();
 }
 
@@ -566,14 +542,8 @@ static int grid_y_for(int64_t work_items, int n_jobs, int ctas_per_sm) {
 // Shares of the one-wave, 1-D grid of grad_kernel: job j owns the CTAs [cta_first[j], cta_first[j + 1]).
 // Default: equal shares, floor(SMs / n_jobs) CTAs per job (all jobs then sweep the rows in lock-step, which keeps the
 // buffer rows they share in L2).  RCMARL_BALANCED_GRID=1 in the environment sizes the shares by cost instead: a job's
-// cost per row depends on its network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks, so with 148 SMs
-// 4 team-reward + 4 critic jobs get 19 + 18 CTAs each instead of 18 + 18, and the 3 chains of a malicious agent
-// 48 / 52 / 48 instead of 49 each (the team-reward job then needs 5 rounds instead of 6); greedy: the job that currently
-// finishes last gets the next CTA.  Measured on B200 (profiles/r01_late_variants.md, run 3): -1.2 % / -2.2 % on isolated
-// full-batch / mini-batch launches but +1.5 % on the C2 update round, so it stays opt-in until that is understood.
-#ifndef RCMARL_MB_EQUAL_SHARES
-#define RCMARL_MB_EQUAL_SHARES 0
-#endif
+// cost per row depends on its network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks, greedy: the job that
+// currently finishes last gets the next CTA.  It stays opt-in: it has not been measured faster on the update round.
 #ifndef RCMARL_BALANCED_GRID_DEFAULT
 #define RCMARL_BALANCED_GRID_DEFAULT 0
 #endif
@@ -635,32 +605,6 @@ static int grad_job_cost(int na, int kind, int loss_mode) {
     return grad_row_cost(kind == RCMARL_IN_SA ? 3 * na : 2 * na, 1);
 }
 
-#if RCMARL_GRAD_WS
-static int launch_mb_persist_ws(const MbParams& P, int n_ctas, cudaStream_t st) {
-    constexpr size_t smem = sizeof(float) * ws_smem_floats();
-    static int resident = -1;
-    if (resident < 0) {
-        if (set_smem(mb_persist_ws_kernel, smem)) return RCMARL_ERR_CUDA;
-        int per_sm = 0;
-        RC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mb_persist_ws_kernel, WS_THREADS, smem));
-        resident = per_sm * sm_count_cached();
-    }
-    if (n_ctas > resident) return RCMARL_ERR_ARG;
-    cudaLaunchAttribute pdl;
-    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pdl.val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_ctas);
-    cfg.blockDim = dim3(WS_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cfg.attrs = &pdl;
-    cfg.numAttrs = 1;
-    RC_CUDA(cudaLaunchKernelEx(&cfg, mb_persist_ws_kernel, P));
-    RC_CUDA(cudaGetLastError());
-    return 0;
-}
-#endif
 
 
 template <int NA>
@@ -892,21 +836,14 @@ int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, 
         c.w = sjobs[j].dst; c.target = q.target; c.time_idx = q.time_idx; c.loss_out = sjobs[j].loss_out;
         c.target_stride = q.target_stride; c.lr = sjobs[j].coef > 0.f ? sjobs[j].coef : lr;
         c.loss_coef = sjobs[j].loss_coef; c.kind = q.kind; c.loss_accumulate = sjobs[j].loss_accumulate;
-#if RCMARL_GRAD_WS && RCMARL_MB_EQUAL_SHARES
-        // experiment (off): equal shares on the tensor-core core (50 / 49 / 49 CTAs at C2 instead of the cost model's 48 / 52 / 48).
-        // Measured slower, 41.0 vs 40.1 us per step: the team-reward chain (15 inputs to load per row) is the slower one per tile
-        // and wants its 20-tile share (profiles/r02_kernel_experiments.md)
-        cost[j] = NA == 5 ? 1 : grad_job_cost(NA, q.kind, RCMARL_LOSS_MSE);
-#else
         cost[j] = grad_job_cost(NA, q.kind, RCMARL_LOSS_MSE);
-#endif
         if (n + 1 > maxn) maxn = n + 1;
     }
     const int cpc = NA == 5 ? grad_chunks_per_cta<5>(RCMARL_LOSS_MSE) : grad_chunks_per_cta<16>(RCMARL_LOSS_MSE);
     const int64_t n_rows_mb = (int64_t)(n_times < mb_times ? n_times : mb_times) * rows->n_envs;
     // CTA shares by cost (the chains do not share rows in L2 the way the lock-step full-batch jobs do).  A mapping with every
-    // CTA serving every chain in turn (reduction of a chain hidden behind the other chains' turns) measured 70 instead of 46 us
-    // per step and was removed (profiles/r02_kernel_experiments.md).
+    // CTA serving every chain in turn (reduction of a chain hidden behind the other chains' turns) was measured
+    // slower and removed.
     int n_ctas = 0;
     {
         int g[RCMARL_MAX_JOBS];
@@ -932,26 +869,8 @@ int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, 
         P.comm.rank = 0; P.comm.world = 1; P.comm.seq = seq_first;
     }
     cudaStream_t st = (cudaStream_t)stream;
-#if RCMARL_GRAD_WS
-    if (NA == 5) return launch_mb_persist_ws(P, n_ctas, st);
-#endif
     return NA == 5 ? launch_mb_persist<5>(P, n_ctas, st) : launch_mb_persist<16>(P, n_ctas, st);
 }
-
-#if RCMARL_GRAD_WS && RCMARL_WS_TIMELINE
-/* debug builds only (csrc/Makefile variant_tl): stage timestamps of the first producer thread, [64 tiles][16 ticks] */
-int rcmarl_debug_timeline(long long* out_host, int n) {
-    if (!out_host || n < 1 || n > 64 * 16) return RCMARL_ERR_ARG;
-    RC_CUDA(cudaMemcpyFromSymbol(out_host, g_ws_timeline, sizeof(long long) * n));
-    return RCMARL_OK;
-}
-/* same for the persistent mini-batch kernel: [64 steps][16 ticks] of CTA 0 / thread 0 */
-int rcmarl_debug_timeline_mb(long long* out_host, int n) {
-    if (!out_host || n < 1 || n > 64 * 16) return RCMARL_ERR_ARG;
-    RC_CUDA(cudaMemcpyFromSymbol(out_host, g_mb_timeline, sizeof(long long) * n));
-    return RCMARL_OK;
-}
-#endif
 
 int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs, void* ws, int64_t ws_bytes,
                 void* stream) {

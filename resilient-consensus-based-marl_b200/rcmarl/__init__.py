@@ -1,4 +1,4 @@
-"""rcmarl -- host side of the B200-native RPBCAC hot path (see DESIGN.md).
+"""rcmarl -- host side of the H100-native RPBCAC hot path (see DESIGN.md).
 
 `rcmarl._lib` binds librcmarl.so (C ABI, include/rcmarl.h); `rcmarl.ops` wraps
 its entry points for torch CUDA tensors; `rcmarl.trainer` is the batched

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Launch the UNMODIFIED reference driver (main.py of mfigura/Resilient-consensus-based-MARL) on the B200 packages.
+"""Launch the UNMODIFIED reference driver (main.py of mfigura/Resilient-consensus-based-MARL) on the drop-in packages.
 
     RCMARL_N_ENVS=4096 python resilient-consensus-based-marl_b200/run_main.py /path/to/reference/main.py --H=1 --slow_lr=0.002
 

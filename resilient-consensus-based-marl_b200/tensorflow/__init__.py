@@ -1,7 +1,7 @@
 """Architecture-descriptor facade for the TensorFlow names the reference driver uses (main.py:7-9,47,60-86).
 
 This is NOT TensorFlow: `keras.Sequential([...])` records the (fixed) RPBCAC network shape and owns a packed
-float32 parameter vector in device memory; every forward / backward pass is executed by the sm_100a kernels of
+float32 parameter vector in device memory; every forward / backward pass is executed by the sm_90a kernels of
 librcmarl.so through rcmarl.ops.  Unsupported Keras functionality raises NotImplementedError."""
 import sys
 import types

@@ -145,7 +145,7 @@ class Sequential(Model):
               all(isinstance(d.activation, LeakyReLU) and abs(d.activation.alpha - 0.1) < 1e-12 for d in dense[:2]) and
               dense[2].activation in (None, 'softmax') and isinstance(layer_list[1], Flatten))
         if not ok:
-            raise NotImplementedError("the sm_100a kernels implement the reference architecture only: "
+            raise NotImplementedError("the sm_90a kernels implement the reference architecture only: "
                                       "Flatten, Dense(20, LeakyReLU(0.1)) x2, Dense(n_out[, softmax]) (main.py:60-82)")
         self.n_agents, self.n_feat = spec.shape
         self.d_in = self.n_agents * self.n_feat
@@ -231,7 +231,7 @@ class Sequential(Model):
 
     def fit(self, *a, **k):
         raise NotImplementedError("use the agent methods (critic_update_local, ...) or rcmarl.trainer: training runs "
-                                  "in the fused sm_100a kernels, not through a generic Keras fit loop")
+                                  "in the fused sm_90a kernels, not through a generic Keras fit loop")
 
     train_on_batch = fit
 

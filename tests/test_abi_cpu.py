@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == bound, (set(declared) ^ set(bound))
     for name in declared:
         assert hasattr(lib, name)
-    assert b"sm_100a" in lib.rcmarl_version()
+    assert b"sm_90a" in lib.rcmarl_version()
     assert lib.rcmarl_status_string(-2) == b"workspace too small"
 
 
@@ -37,7 +37,7 @@ def test_param_counts_and_workspace_query():
     assert lib.rcmarl_param_count(15, 1) == 761
     assert lib.rcmarl_param_count(10, 5) == 745
     assert lib.rcmarl_param_count(32, 1) == 1101 and lib.rcmarl_param_count(48, 1) == 1421   # C3
-    assert lib.rcmarl_workspace_bytes(8, 761) >= 296 * 8 * 762 * 4 // 8
+    assert lib.rcmarl_workspace_bytes(8, 761) >= 264 * 8 * 762 * 4 // 8         # two CTAs per SM on 132 SMs
 
 
 def test_bad_arguments_are_rejected_without_a_device():

@@ -131,3 +131,14 @@ def test_grad_grid_plan_equal_and_balanced_shares():
                 assert min(g) >= 1 and sum(g) <= max(148, n), (kinds, rows, na, bal, g)
     with pytest.raises(L.RcmarlError):
         _grid_plan([7], 10, False)
+
+
+def test_grad_grid_plan_on_132_sms():
+    """The plans the launchers build on an H100 SXM (132 SMs) for the C2 jobs: the full-batch fit and a mini-batch step of the
+    malicious agent, equal and cost-balanced shares."""
+    from rcmarl import _lib as L
+    SA, S = L.IN_SA, L.IN_S
+    assert _grid_plan([SA, S] * 4, 12288000, False, sms=132) == [16] * 8
+    assert _grid_plan([SA, S] * 4, 12288000, True, sms=132) == [17, 16] * 4
+    assert _grid_plan([S, SA, S], 131072, False, sms=132) == [44, 44, 44]
+    assert _grid_plan([S, SA, S], 131072, True, sms=132) == [43, 46, 43]

@@ -1,12 +1,12 @@
 #!/bin/bash
 # One-call A/B on a GPU box.  Candidates are library build variants (csrc/Makefile `variants`: librcmarl_<name>.so,
 # selected with RCMARL_LIB) and / or environment switches of the default library.
-#   AB_LIBS="ffma r1"                      variants to compare with the default library
+#   AB_LIBS="v0 p0"                        variants to compare with the default library
 #   AB_ENVS="RCMARL_BALANCED_GRID=1"     switches to compare with the default settings
-#   AB_TEST_LIBS="r1"                    variants to run the kernel + trainer GPU tests with
+#   AB_TEST_LIBS="v0"                    variants to run the kernel + trainer GPU tests with
 # For every candidate: gradient sums of fixed seeded inputs compared with the default's bit for bit (tools/ab_grad.py),
 # CUDA-event timings of rcmarl_grad at the C2 shapes, and a short C2 bench.  Then the full GPU suite with the defaults.
-cd "${GRAFT_REPO_ROOT:-/root/repo}"
+cd "$(dirname "$0")/.."
 P=$PWD/resilient-consensus-based-marl_b200/rcmarl
 mkdir -p gpurun_out
 bench_line() {

@@ -1,6 +1,6 @@
-"""NumPy emulation of the 3xTF32 split used by csrc/grad_kernel_ws.cuh (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo; weights B: hi = value
+"""NumPy emulation of the 3xTF32 split of the tensor-core fit design in DESIGN.md §7, which no shipped kernel uses (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo; weights B: hi = value
 rounded to tf32 with round-to-nearest-away; activations A: hi either rounded (three ops per element) or TRUNCATED to tf32 (two
-ops, the shipped form); lo = value - hi, truncated to tf32 by the tensor core; fp32 accumulation): error of one hidden layer of
+ops, the measured form); lo = value - hi, truncated to tf32 by the tensor core; fp32 accumulation): error of one hidden layer of
 the RPBCAC nets against fp64, max and mean signed (bias), next to plain fp32 and single-pass TF32.  CPU only.
     python tools/experiments/tf32x3_error.py
 """
