@@ -78,9 +78,9 @@ int64_t rcmarl_param_count(int d_in, int n_out); /* packed length of one network
 /* Scratch needed by the *_grad entry points for `n_jobs` jobs of at most `max_params` parameters. */
 int64_t rcmarl_workspace_bytes(int n_jobs, int max_params);
 
-/* How rcmarl_grad / rcmarl_minibatch_sgd would split a one-wave grid of `sm_count` CTAs over `n_jobs` jobs that sweep
- * `n_rows` buffer rows: ctas_host[j] = CTAs of job j (kinds_host[j] = RCMARL_IN_*).  balanced = 0: equal shares (the
- * default of the launchers); 1: shares sized by each job's cost per row (environment switch RCMARL_BALANCED_GRID=1).
+/* How a one-wave grid of `sm_count` CTAs is split over `n_jobs` jobs that sweep `n_rows` buffer rows:
+ * ctas_host[j] = CTAs of job j (kinds_host[j] = RCMARL_IN_*).  balanced = 0: equal shares, the plan of rcmarl_grad;
+ * 1: shares sized by each job's cost per row, the plan of rcmarl_minibatch_fit (with n_rows = one mini-batch).
  * Host arithmetic only (no device needed); exposed for tests and for sizing experiments. */
 int rcmarl_grad_grid_plan(int n_agents, const int32_t* kinds_host, int n_jobs, int loss_mode, int64_t n_rows, int balanced,
                           int sm_count, int32_t* ctas_host);
@@ -173,26 +173,21 @@ typedef struct {
 } rcmarl_sgd_job;
 int rcmarl_sgd_apply(const rcmarl_sgd_job* jobs_host, int n_jobs, void* stream);
 
-/* K9.  Mini-batch SGD epochs for several networks in lock-step (Keras fit(batch_size=32, epochs=10, shuffle=True),
- * agents/adversarial_CAC_agents.py:133,150,163,239,251): for e < epochs, for each batch b of `mb_times`
- * time rows: rows = { time_idx_j[e*n_times + b*mb_times + i]*n_envs + env }, gradient (rcmarl_grad, MSE), then
- * theta_j -= lr*2/(rows in batch, summed over ranks) * g in place.  Reduction of the CTA partials, the cross-GPU
- * exchange (when an exchange context is bound, see rcmarl_comm_*) and the SGD apply are ONE kernel; the grad kernel
- * of the next step starts its prologue under it (programmatic dependent launch).
- * gjobs[j].time_idx must point at that network's [epochs][n_times] permutation table; sjobs[j].dst == src == gjobs[j].w;
- * sjobs[j].loss_out (optional) accumulates sum(e^2)*loss_coef over epoch 0 only (history['loss'][0]).
- * rows->n_rows / time_idx are ignored.  Without a bound exchange context a data-parallel caller loops over
- * rcmarl_grad / all-reduce / rcmarl_sgd_apply instead. */
-int rcmarl_minibatch_sgd(const rcmarl_rows* rows_host, const rcmarl_grad_job* gjobs_host,
-                         const rcmarl_sgd_job* sjobs_host, int n_jobs, int epochs, int n_times, int mb_times,
-                         float lr, void* ws, int64_t ws_bytes, void* stream);
-
-/* The same fit as ONE persistent kernel (csrc/minibatch_persist.cuh): the CTAs stay resident for all epochs x
- * mini-batches, every chain's parameters live in the shared memory of its CTAs, and the per-step reduction over CTAs
- * (and, with a bound exchange context, over ranks through NVLink peer memory) runs through {value, sequence} cells
- * instead of kernel boundaries -- no launches, no grid barrier, no atomics; results are bitwise reproducible and
- * identical on every rank.  Arguments as rcmarl_minibatch_sgd, except:
- *   sjobs[j].coef > 0 overrides `lr` for chain j (per-agent fast_lr, agents/resilient_CAC_agents.py:36);
+/* K9.  Mini-batch SGD epochs for several networks (chains) in lock-step (Keras fit(batch_size=32, epochs=10,
+ * shuffle=True), agents/adversarial_CAC_agents.py:133,150,163,239,251): for e < epochs, for each batch b of `mb_times`
+ * time rows: rows = { time_idx_j[e*n_times + b*mb_times + i]*n_envs + env }, MSE gradient g over them (as rcmarl_grad),
+ * then theta_j -= lr_j*2/(rows in batch, summed over ranks) * g in place.
+ * ONE persistent kernel (csrc/minibatch_persist.cuh): the CTAs stay resident for all epochs x mini-batches, every chain's
+ * parameters live in the shared memory of its CTAs, and the per-step reduction over CTAs (and, with a bound exchange
+ * context, over ranks through NVLink peer memory) runs through {value, sequence} cells instead of kernel boundaries --
+ * no launches, no grid barrier, no atomics; results are bitwise reproducible and identical on every rank.  Without a
+ * bound exchange context a data-parallel caller loops over rcmarl_grad / all-reduce / rcmarl_sgd_apply instead.
+ *   gjobs[j].time_idx: that chain's [epochs][n_times] permutation table; rows->n_rows / time_idx are ignored;
+ *   sjobs[j].dst == src == gjobs[j].w, sjobs[j].n = its parameter count, sjobs[j].first = 0;
+ *   sjobs[j].coef > 0 is chain j's learning rate lr_j (per-agent fast_lr, agents/resilient_CAC_agents.py:36),
+ *     otherwise lr_j = `lr`;
+ *   sjobs[j].loss_out (optional) receives loss_coef * sum(e^2) over epoch 0 only (history['loss'][0]), added to it
+ *     when loss_accumulate;
  *   cells / cells_bytes: caller-owned scratch of rcmarl_minibatch_cells_bytes() bytes that must be ZERO before the
  *     first call and is otherwise only touched by this entry point;
  *   seq_first >= 1: first of the `rcmarl_minibatch_steps()` consecutive sequence numbers this call consumes; the
@@ -252,9 +247,9 @@ int rcmarl_reward_mix(const float* r, int64_t n_rows, int n_agents, const int32_
 
 /* ---------------------------------------------------------------------------
  * Data parallelism over environment shards (SURVEY 8e): one process per GPU of ONE node.  A bound exchange context
- * makes rcmarl_grad / rcmarl_team / rcmarl_minibatch_sgd return (and apply) sums over ALL ranks: the per-CTA partials
+ * makes rcmarl_grad / rcmarl_team return, and rcmarl_minibatch_fit apply, sums over ALL ranks: the per-CTA partials
  * are reduced, exchanged through NVLink peer memory (CUDA IPC buffers, one-shot all-reduce, rank-ordered summation =>
- * bitwise identical results on every rank) and, for the mini-batch path, applied -- all inside ONE kernel
+ * bitwise identical results on every rank) and, for the mini-batch fit, applied -- all inside ONE kernel
  * (csrc/comm.cuh).  Every rank must issue the same sequence of those calls.  Without a bound context the caller
  * all-reduces `sums` itself (e.g. NCCL) between rcmarl_grad and the apply.
  *   create(rank, world <= 8, capacity) -> export a 64-byte IPC handle -> exchange handles out of band (e.g.

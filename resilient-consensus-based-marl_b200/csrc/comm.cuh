@@ -30,9 +30,8 @@ struct CommDev {
     uint32_t seq;
 };
 
-#ifndef RCMARL_CELL_POLL_NS
-#define RCMARL_CELL_POLL_NS 40                               // back-off between polls of a cell that has not arrived yet
-#endif
+constexpr int CELL_POLL_NS = 40;                           // back-off between polls of a cell that has not arrived yet
+
 __device__ __forceinline__ void st_cell(uint2* p, float v, uint32_t seq) {
     asm volatile("st.volatile.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(__float_as_uint(v)), "r"(seq) : "memory");
 }
@@ -72,7 +71,7 @@ __device__ __forceinline__ float comm_wait_total(const CommDev& c, int64_t offse
                     __threadfence_system();
                     __trap();                            // surfaces as a CUDA error at the next synchronisation
                 }
-                __nanosleep(RCMARL_CELL_POLL_NS);
+                __nanosleep(CELL_POLL_NS);
                 x = ld_cell(cell);
             }
             v[p] = __uint_as_float(x.x);

@@ -178,49 +178,27 @@ __device__ __forceinline__ void unpack2(f2 v, float& lo, float& hi) {
     hi = v.y;
 }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-__device__ __forceinline__ void fma2_acc(f2& acc, f2 a, f2 b) {
-    acc.x = fmaf(a.x, b.x, acc.x);
-    acc.y = fmaf(a.y, b.y, acc.y);
-}
 __device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
-// Where a kernel reads the packed network parameters from: the CTA's staged copy in shared memory (uniform LDS.128,
-// 2 shared-memory wavefronts per quad).  The accessor keeps the dense-layer code independent of the source; a constant-
-// bank source was measured in round 1 and rejected (DESIGN.md section 7).
-struct SmemW {
-    const float* p;
-    __device__ __forceinline__ float4 q(int off) const { return *reinterpret_cast<const float4*>(p + off); }
-    __device__ __forceinline__ float s(int off) const { return p[off]; }
-};
-
-#ifndef RCMARL_LRELU_MAX
-#define RCMARL_LRELU_MAX 1
-#endif
 // LeakyReLU of a packed pair.  slope in (0, 1) => lrelu(z) == max(z, slope * z) bit for bit (z > 0: slope*z < z;
 // z < 0: slope*z > z; +-0 and NaN map to themselves), which is 2 x (FMUL, FMNMX) instead of 2 x (FMUL, FSETP, FSEL).
 __device__ __forceinline__ void lrelu_pair(f2 z, float& a, float& b) {
-    float za, zb;
+    float za, zb, ta, tb;
     unpack2(z, za, zb);
-#if RCMARL_LRELU_MAX
-    float ta, tb;
     unpack2(mul2(z, pack2(SLOPE, SLOPE)), ta, tb);
     a = fmaxf(za, ta);
     b = fmaxf(zb, tb);
-#else
-    a = lrelu(za);
-    b = lrelu(zb);
-#endif
 }
 
-// z[r][:] = b + x[r] W for R rows at once: every weight quad feeds 4*R FFMA; outputs are packed as pairs of adjacent
-// hidden units.  `w` is the parameter source (SmemW), offW / offb the offsets of W [K][20] and b [20] in it.
-template <int K, int R, class WS>
-__device__ __forceinline__ void dense20_rows(const WS& w, int offW, int offb, const float (&x)[R][K],
-                                             float (&h)[R][HID]) {
+// z[r][:] = b + x[r] W for R rows at once (W row-major [K][20] and b [20] in shared memory, broadcast float4 reads):
+// every weight quad feeds 4*R FFMA; outputs are packed as pairs of adjacent hidden units.
+template <int K, int R>
+__device__ __forceinline__ void dense20_rows(const float* __restrict__ sW, const float* __restrict__ sb,
+                                             const float (&x)[R][K], float (&h)[R][HID]) {
     f2 hp[R][HID / 2];
 #pragma unroll
     for (int q = 0; q < HID / 4; ++q) {
-        const float4 v = w.q(offb + 4 * q);
+        const float4 v = reinterpret_cast<const float4*>(sb)[q];
 #pragma unroll
         for (int r = 0; r < R; ++r) { hp[r][2 * q] = pack2(v.x, v.y); hp[r][2 * q + 1] = pack2(v.z, v.w); }
     }
@@ -229,9 +207,10 @@ __device__ __forceinline__ void dense20_rows(const WS& w, int offW, int offb, co
         f2 xk[R];
 #pragma unroll
         for (int r = 0; r < R; ++r) xk[r] = pack2(x[r][k], x[r][k]);
+        const float4* w = reinterpret_cast<const float4*>(sW + k * HID);
 #pragma unroll
         for (int q = 0; q < HID / 4; ++q) {
-            const float4 v = w.q(offW + k * HID + 4 * q);
+            const float4 v = w[q];
             const f2 w0 = pack2(v.x, v.y), w1 = pack2(v.z, v.w);
 #pragma unroll
             for (int r = 0; r < R; ++r) {
@@ -244,30 +223,6 @@ __device__ __forceinline__ void dense20_rows(const WS& w, int offW, int offb, co
     for (int r = 0; r < R; ++r)
 #pragma unroll
         for (int j = 0; j < HID / 2; ++j) lrelu_pair(hp[r][j], h[r][2 * j], h[r][2 * j + 1]);
-}
-// shared-memory form used by values_kernel / team_kernel: W and b are pointers into the staged network
-template <int K, int R>
-__device__ __forceinline__ void dense20_rows(const float* __restrict__ sW, const float* __restrict__ sb,
-                                             const float (&x)[R][K], float (&h)[R][HID]) {
-    dense20_rows<K, R>(SmemW{sW}, 0, (int)(sb - sW), x, h);
-}
-
-template <int DIN, class WS>
-__device__ __forceinline__ float head1_w(const WS& w, const float (&h2)[HID]) {
-    float out = w.s(off_b3(DIN, 1));
-#pragma unroll
-    for (int j = 0; j < HID; ++j) out = fmaf(h2[j], w.s(off_W3(DIN) + j), out);
-    return out;
-}
-
-template <int DIN, class WS>
-__device__ __forceinline__ void head5_w(const WS& w, const float (&h2)[HID], float (&logit)[NACT]) {
-#pragma unroll
-    for (int o = 0; o < NACT; ++o) logit[o] = w.s(off_b3(DIN, NACT) + o);
-#pragma unroll
-    for (int j = 0; j < HID; ++j)
-#pragma unroll
-        for (int o = 0; o < NACT; ++o) logit[o] = fmaf(h2[j], w.s(off_W3(DIN) + j * NACT + o), logit[o]);
 }
 
 // hidden features of R rows at once (critic_features / TR_features, agents/resilient_CAC_agents.py:39-40)

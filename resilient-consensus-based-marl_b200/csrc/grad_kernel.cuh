@@ -80,11 +80,7 @@ __host__ __device__ constexpr int stage_floats_per_row(int din, bool is_sa_net) 
 // warps per CTA: as many 64-row tiles as fit next to the staged weights, at most 8
 // Bulk-copy input staging costs 64 x 3*NA x 4 bytes of shared memory per warp.  At n_agents = 5 (3.8 KB per warp) it fits
 // next to 8 tiles; at n_agents = 16 it would cut the CTA from 6 to 4 warps, so those instantiations keep per-lane loads.
-#ifndef RCMARL_NO_TMA
 __host__ __device__ constexpr bool grad_use_tma(int na) { return na <= 5; }
-#else
-__host__ __device__ constexpr bool grad_use_tma(int na) { return false; }
-#endif
 
 template <int DIN, int NOUT, bool SA_NET>
 constexpr int grad_warps_for() {
@@ -138,23 +134,6 @@ struct GradParams {
     int16_t cta_first[RCMARL_MAX_JOBS + 1];
 };
 
-// 1: the constant columns of the tile rows ([.., 1, 0 pad], zero pads of the deltas) are written once per kernel instead of
-//    once per chunk (3-4 of 22 STS.128 per row).  Results bit-identical (tools/ab_grad.py).
-#ifndef RCMARL_PAD_HOIST
-#define RCMARL_PAD_HOIST 1
-#endif
-// 1: the CTA signals its programmatic dependents (the reduce kernel of the same mini-batch step, launched with the PDL
-//    attribute) once its row loop is done, so the reduce grid is already queued when the last CTA exits; the reduce kernel
-//    waits for this grid with griddepcontrol.wait.
-// 1: warp-major assignment of 64-row chunks to (CTA, warp), see grad_body (not yet measured on the GPU: added after the
-//    round-1 GPU budget was spent; 0 restores the measured CTA-major order)
-#ifndef RCMARL_CHUNK_WARP_MAJOR
-#define RCMARL_CHUNK_WARP_MAJOR 1
-#endif
-#ifndef RCMARL_PDL_REDUCE
-#define RCMARL_PDL_REDUCE 1
-#endif
-
 __device__ __forceinline__ void st4(float* p, float a, float b, float c, float d) {
     *reinterpret_cast<float4*>(p) = make_float4(a, b, c, d);
 }
@@ -170,7 +149,6 @@ struct GradCore {
     static constexpr int R = 2;
     static constexpr int SROW = 3 * NA;                                     // staged row = one sa row (ns rows are shorter)
     static constexpr int SWARP = grad_use_tma(NA) ? L::ROWS * SROW : 0;      // staging floats per warp
-    static constexpr bool kPadHoist = RCMARL_PAD_HOIST != 0;
 
     float* sw;          // staged network parameters (shared)
     float* tiles;       // [GRAD_WARPS][ROWS][RS]
@@ -206,22 +184,21 @@ struct GradCore {
     }
 
     // the constant columns of this lane's two tile rows ([.., 1, 0 pad] of the activations, zero pad of the deltas)
-    // never change: write them once instead of once per chunk.  Must be repeated after cta_reduce (which reuses the tiles).
+    // never change: write them once instead of once per chunk (saves 3-4 of 22 STS.128 per row).  Must be repeated after
+    // cta_reduce (which reuses the tiles).
     __device__ __forceinline__ void write_pads() {
-        if constexpr (kPadHoist) {
 #pragma unroll
-            for (int r = 0; r < R; ++r) {
-                float* rowp = wt + (lane + 32 * r) * L::RS;
+        for (int r = 0; r < R; ++r) {
+            float* rowp = wt + (lane + 32 * r) * L::RS;
 #pragma unroll
-                for (int q = 0; q < L::LA1 / 4; ++q)
-                    if (4 * q >= DIN) st4(rowp + L::OA1 + 4 * q, 4 * q == DIN ? 1.f : 0.f, 0.f, 0.f, 0.f);
-                st4(rowp + L::OA2 + 20, 1.f, 0.f, 0.f, 0.f);
-                if constexpr (L::L3T) st4(rowp + L::OA3 + 20, 1.f, 0.f, 0.f, 0.f);
-                st4(rowp + L::OD1 + 20, 0.f, 0.f, 0.f, 0.f);
-                st4(rowp + L::OD2 + 20, 0.f, 0.f, 0.f, 0.f);
-            }
-            __syncwarp();
+            for (int q = 0; q < L::LA1 / 4; ++q)
+                if (4 * q >= DIN) st4(rowp + L::OA1 + 4 * q, 4 * q == DIN ? 1.f : 0.f, 0.f, 0.f, 0.f);
+            st4(rowp + L::OA2 + 20, 1.f, 0.f, 0.f, 0.f);
+            if constexpr (L::L3T) st4(rowp + L::OA3 + 20, 1.f, 0.f, 0.f, 0.f);
+            st4(rowp + L::OD1 + 20, 0.f, 0.f, 0.f, 0.f);
+            st4(rowp + L::OD2 + 20, 0.f, 0.f, 0.f, 0.f);
         }
+        __syncwarp();
     }
 
     __device__ __forceinline__ void zero_acc() {
@@ -235,7 +212,6 @@ struct GradCore {
     // Sweep the rows of `Rw` that belong to CTA y of gy (64-row chunks, see below); weights are read from `sw`.
     // Accumulates into acc / g3 / loss.
     __device__ __forceinline__ void sweep(const rcmarl_rows& Rw, const rcmarl_grad_job& job, int y, int gy) {
-    const SmemW W{sw};
     // Input staging by the TMA engine: the 64 rows of a chunk are one contiguous, 16-byte aligned span of sa / ns whenever
     // the chunk is full and (contiguous row mode, or gathered mode with n_envs % 64 == 0); lane 0 issues one 1-D bulk copy
     // per chunk, completion is tracked by the warp's mbarrier; other chunks fall back to per-lane loads.
@@ -249,17 +225,12 @@ struct GradCore {
         return (reinterpret_cast<uintptr_t>(src) & 15) == 0;
     };
     bool staged = false;
-    // Chunk c of the job goes to (CTA y, warp w) with c = k * cstep + w * gy + y (RCMARL_CHUNK_WARP_MAJOR, default) or
-    // c = k * cstep + y * GRAD_WARPS + w.  Both cover every chunk exactly once; they differ in who runs the last, partial
-    // round: warp-major leaves one or two busy warps on every SM (on different schedulers, so they run faster alone),
-    // CTA-major leaves a few SMs with all warps busy and the others idle -- at the C2 mini-batch shape (2048 chunks per
-    // job on 49 x 8 warps = 5.22 rounds) the whole launch then waits for a full sixth round on 11 SMs.
+    // Chunk c of the job goes to (CTA y, warp w) with c = k * cstep + w * gy + y: warp-major, so that the last, partial
+    // round leaves one or two busy warps on every SM (on different schedulers, so they run faster alone).  A CTA-major
+    // order (c = k * cstep + y * GRAD_WARPS + w) would leave a few SMs with all warps busy and the others idle, and the
+    // whole launch would wait for a full extra round on those SMs.
     const int64_t cstep = (int64_t)gy * GRAD_WARPS;
-#if RCMARL_CHUNK_WARP_MAJOR
     const int64_t cfirst = (int64_t)warp * gy + y;
-#else
-    const int64_t cfirst = (int64_t)y * GRAD_WARPS + warp;
-#endif
     {
         const int64_t c0 = cfirst;
         const float* src = nullptr;
@@ -308,13 +279,13 @@ struct GradCore {
                         bulk_load(stage, src, (uint32_t)(L::ROWS * rowf * sizeof(float)), bar);
                     }
                 }
-                dense20_rows<DIN, R>(W, 0, off_b1(DIN), x, h1);
+                dense20_rows<DIN, R>(sw, sw + off_b1(DIN), x, h1);
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
                     float* a1 = wt + (lane + 32 * r) * L::RS + L::OA1;
 #pragma unroll
                     for (int q = 0; q < L::LA1 / 4; ++q) {
-                        if (kPadHoist && 4 * q >= DIN) continue;
+                        if (4 * q >= DIN) continue;                       // constant columns: write_pads()
                         float v[4];
 #pragma unroll
                         for (int u = 0; u < 4; ++u) {
@@ -325,29 +296,28 @@ struct GradCore {
                     }
                 }
             }
-            dense20_rows<HID, R>(W, off_W2(DIN), off_b2(DIN), h1, h2);
+            dense20_rows<HID, R>(sw + off_W2(DIN), sw + off_b2(DIN), h1, h2);
             float d2[R][HID];
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 float* rowp = wt + (lane + 32 * r) * L::RS;
 #pragma unroll
                 for (int q = 0; q < 5; ++q) st4(rowp + L::OA2 + 4 * q, h1[r][4 * q], h1[r][4 * q + 1], h1[r][4 * q + 2], h1[r][4 * q + 3]);
-                if constexpr (!kPadHoist) st4(rowp + L::OA2 + 20, 1.f, 0.f, 0.f, 0.f);
                 const float tgt = live[r] ? __ldg(job.target + row[r] * job.target_stride) : 0.f;
                 if constexpr (NOUT == 1) {
                     // Keras MSE (Appendix A.2): dLoss/dout = 2 (out - y) / B; the 2/B is applied by the caller
-                    const float e = live[r] ? head1_w<DIN>(W, h2[r]) - tgt : 0.f;
+                    const float e = live[r] ? head1<DIN>(sw, h2[r]) - tgt : 0.f;
                     loss = fmaf(e, e, loss);
 #pragma unroll
                     for (int j = 0; j < HID; ++j) {
                         g3[j] = fmaf(h2[r][j], e, g3[j]);
-                        d2[r][j] = W.s(off_W3(DIN) + j) * e * lrelu_grad_from_out(h2[r][j]);
+                        d2[r][j] = sw[off_W3(DIN) + j] * e * lrelu_grad_from_out(h2[r][j]);
                     }
                     g3[HID] += e;
                 } else {
                     // weighted sparse categorical cross-entropy on the logits (Appendix A.5)
                     float p[NACT], mx, lse, g[NACT];
-                    head5_w<DIN>(W, h2[r], p);
+                    head5<DIN>(sw, h2[r], p);
                     const int a = (int)__ldg(Rw.sa + row[r] * (3 * NA) + 3 * job.action_agent + 2);
                     float la = 0.f;
 #pragma unroll
@@ -358,20 +328,18 @@ struct GradCore {
                     for (int o = 0; o < NACT; ++o) g[o] = (p[o] - (o == a ? 1.f : 0.f)) * tgt;
 #pragma unroll
                     for (int q = 0; q < 5; ++q) st4(rowp + L::OA3 + 4 * q, h2[r][4 * q], h2[r][4 * q + 1], h2[r][4 * q + 2], h2[r][4 * q + 3]);
-                    if constexpr (!kPadHoist) st4(rowp + L::OA3 + 20, 1.f, 0.f, 0.f, 0.f);
                     st4(rowp + L::OD3, g[0], g[1], g[2], g[3]);
                     st4(rowp + L::OD3 + 4, g[4], 0.f, 0.f, 0.f);
 #pragma unroll
                     for (int j = 0; j < HID; ++j) {
                         float s = 0.f;
 #pragma unroll
-                        for (int o = 0; o < NACT; ++o) s = fmaf(W.s(off_W3(DIN) + j * NACT + o), g[o], s);
+                        for (int o = 0; o < NACT; ++o) s = fmaf(sw[off_W3(DIN) + j * NACT + o], g[o], s);
                         d2[r][j] = s * lrelu_grad_from_out(h2[r][j]);
                     }
                 }
 #pragma unroll
                 for (int q = 0; q < 5; ++q) st4(rowp + L::OD2 + 4 * q, d2[r][4 * q], d2[r][4 * q + 1], d2[r][4 * q + 2], d2[r][4 * q + 3]);
-                if constexpr (!kPadHoist) st4(rowp + L::OD2 + 20, 0.f, 0.f, 0.f, 0.f);
             }
             // delta1[i] = (W2[i][:] . delta2) * lrelu'(z1[i]) for both rows; each W2 quad feeds 8 FFMA
             f2 d2p[R][HID / 2];
@@ -390,7 +358,7 @@ struct GradCore {
                     for (int r = 0; r < R; ++r) s[r] = pack2(0.f, 0.f);
 #pragma unroll
                     for (int qq = 0; qq < 5; ++qq) {
-                        const float4 v = W.q(off_W2(DIN) + i * HID + 4 * qq);
+                        const float4 v = *reinterpret_cast<const float4*>(sw + off_W2(DIN) + i * HID + 4 * qq);
                         const f2 w0 = pack2(v.x, v.y), w1 = pack2(v.z, v.w);
 #pragma unroll
                         for (int r = 0; r < R; ++r) {
@@ -409,16 +377,10 @@ struct GradCore {
                 for (int r = 0; r < R; ++r)
                     st4(wt + (lane + 32 * r) * L::RS + L::OD1 + 4 * q, d1[r][0], d1[r][1], d1[r][2], d1[r][3]);
             }
-#pragma unroll
-            for (int r = 0; r < R; ++r)
-                if constexpr (!kPadHoist) st4(wt + (lane + 32 * r) * L::RS + L::OD1 + 20, 0.f, 0.f, 0.f, 0.f);
         }
         __syncwarp();
         // ---------------- phase 2: 8x8 register tile per lane, NG rows per step ----------------
-#ifndef RCMARL_PH2_UNROLL
-#define RCMARL_PH2_UNROLL 4
-#endif
-        constexpr int kPh2Unroll = RCMARL_PH2_UNROLL;
+        constexpr int kPh2Unroll = 4;
 #pragma unroll kPh2Unroll
         for (int it = 0; it < L::ROWS / L::NG; ++it) {
             const float* rp = wt + (it * L::NG + grp) * L::RS;
@@ -507,9 +469,9 @@ __device__ __forceinline__ void grad_body(const GradParams& P, const rcmarl_grad
     core.write_pads();
     core.zero_acc();
     core.sweep(Rw, job, y, gy);
-#if RCMARL_PDL_REDUCE
+    // a reduce kernel launched as a programmatic dependent (launch_reduce_comm, train_kernels.cu) is queued once every CTA is
+    // past its row loop, i.e. before the last CTA exits; it waits for this grid with griddepcontrol.wait
     pdl_launch_dependents();
-#endif
     float* out = P.partial + (int64_t)blockIdx.x * P.stride;
     core.cta_reduce([out](int i, float v) { out[i] = v; });
 }

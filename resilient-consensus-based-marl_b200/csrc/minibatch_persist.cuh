@@ -1,8 +1,8 @@
-// minibatch_persist.cuh -- the adversaries' mini-batch fits as ONE persistent kernel per rcmarl_minibatch_sgd call
+// minibatch_persist.cuh -- the adversaries' mini-batch fits as ONE persistent kernel per rcmarl_minibatch_fit call
 // (replaces critic.fit / TR.fit(batch_size=32, epochs=10) of agents/adversarial_CAC_agents.py:133,150,163,239,251).
 //
-// Round 1 ran every SGD step as two launches (grad_kernel + fused reduce / apply): 9 400 sequential steps per update
-// round at ~17 us of launch gaps, prologues and a separate reduce grid each.  Here the CTAs stay resident for all
+// As two launches per SGD step (grad_kernel + reduce / apply), a fit costs 9 400 sequential steps per update round at
+// ~17 us of launch gaps, prologues and a separate reduce grid each.  Here the CTAs stay resident for all
 // epochs x mini-batches of a call, each chain's parameters live in the shared memory of its CTAs, and a step is
 //   1. sweep this CTA's 64-row chunks of the mini-batch (GradCore, register accumulators),
 //   2. fixed-order CTA reduction; the CTA's sums go out as level-1 cells {value, seq} (8-byte stores),
@@ -53,7 +53,7 @@ __device__ __forceinline__ uint2 poll_cell(const uint2* cell, uint32_t seq, uint
                 __threadfence_system();
                 __trap();
             }
-            __nanosleep(RCMARL_CELL_POLL_NS);           // spinning CTAs must not crowd the writers out of the L2 queues
+            __nanosleep(CELL_POLL_NS);         // spinning CTAs must not crowd the writers out of the L2 queues
             x = ld_cell(cell);
         } while (x.y != seq);
     }

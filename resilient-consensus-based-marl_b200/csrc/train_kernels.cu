@@ -12,12 +12,8 @@
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
 // training/train_agents.py:86-163 (cited per entry point in include/rcmarl.h).
-#include <stdlib.h>
 #include "common.cuh"
 #include "grad_kernel.cuh"
-#define RC_GRAD_KERNEL grad_kernel
-#define RC_GRAD_WARPS grad_warps
-#define RC_GRAD_SMEM grad_smem_floats
 #include "comm.cuh"
 #include "minibatch_persist.cuh"
 
@@ -163,50 +159,21 @@ __global__ void __launch_bounds__(256) reduce_kernel(const __grid_constant__ Red
     if (threadIdx.x < 32 && valid) P.sums[j][i] = s;
 }
 
-// fused: sums[j][i] = sum_y partial[y][j][i]; theta = theta - coef * sums (mini-batch SGD step, single GPU)
-struct ReduceSgdParams {
-    const float* partial;
-    rcmarl_sgd_job jobs[RCMARL_MAX_JOBS];
-    PartialSlots slots;
-};
-__global__ void __launch_bounds__(256) reduce_sgd_kernel(const __grid_constant__ ReduceSgdParams P) {
-    __shared__ float sh[256];
-    pdl_launch_dependents();     // the next grad kernel may start its prologue; it waits (pdl_wait) before reading
-#if RCMARL_PDL_REDUCE
-    pdl_wait();                  // launched as a programmatic dependent of the grad kernel: its partials must be complete
-#endif
-    const rcmarl_sgd_job& job = P.jobs[blockIdx.y];
-    const int i = blockIdx.x * 32 + (threadIdx.x & 31);
-    const bool valid = i <= job.n;
-    const float s = block_partial_sum(P.partial, P.slots, blockIdx.y, i, valid, sh);
-    if (threadIdx.x >= 32 || !valid) return;
-    if (i < job.n) {
-        const float v = job.src[i];
-        job.dst[i] = i >= job.first ? v - job.coef * s : v;
-    } else if (job.loss_out) {
-        const float l = job.loss_coef * s;
-        *job.loss_out = job.loss_accumulate ? *job.loss_out + l : l;
-    }
-}
-
-// Multi-GPU variant: reduce the CTA partials, exchange over NVLink peer memory (comm.cuh), write the global sums and
-// optionally apply the SGD step -- one kernel, no NCCL call, no host round trip.
+// Multi-GPU variant: reduce the CTA partials, exchange over NVLink peer memory (comm.cuh) and write the global sums --
+// one kernel, no NCCL call, no host round trip.
 struct ReduceCommParams {
     const float* partial;
     float* sums[RCMARL_MAX_JOBS];
     int32_t n[RCMARL_MAX_JOBS];
-    rcmarl_sgd_job sgd[RCMARL_MAX_JOBS];
     PartialSlots slots;
-    int32_t out_stride, fuse_sgd;     // out_stride: distance between the jobs' blocks in the exchange buffer
+    int32_t out_stride;               // distance between the jobs' blocks in the exchange buffer
     int32_t n_jobs, max_n;            // items = n_jobs x ceil(max_n / 32)
     CommDev comm;
 };
 __global__ void __launch_bounds__(256) reduce_comm_kernel(const __grid_constant__ ReduceCommParams P) {
     __shared__ float sh[256];
     pdl_launch_dependents();     // the next grad kernel may start its prologue; it waits (pdl_wait) before reading
-#if RCMARL_PDL_REDUCE
-    pdl_wait();
-#endif
+    pdl_wait();                  // launched as a programmatic dependent of the producer: its partials must be complete
     // One item = 32 consecutive elements of one job.  Items are independent (comm.cuh): a CTA walks its items in
     // ascending order on every rank, so any grid size is deadlock-free and nothing has to be co-resident.
     const int blocks_per_job = (P.max_n + 31) / 32;
@@ -221,16 +188,6 @@ __global__ void __launch_bounds__(256) reduce_comm_kernel(const __grid_constant_
             comm_push(P.comm, off, s);
             const float tot = comm_wait_total(P.comm, off);
             if (P.sums[j]) P.sums[j][i] = tot;
-            if (P.fuse_sgd) {
-                const rcmarl_sgd_job& job = P.sgd[j];
-                if (i < job.n) {
-                    const float v = job.src[i];
-                    job.dst[i] = i >= job.first ? v - job.coef * tot : v;
-                } else if (i == job.n && job.loss_out) {
-                    const float l = job.loss_coef * tot;
-                    *job.loss_out = job.loss_accumulate ? *job.loss_out + l : l;
-                }
-            }
         }
         __syncthreads();          // sh[] is reused by the next item
     }
@@ -458,10 +415,10 @@ static int launch_values(const ValuesParams& P, int n_jobs, cudaStream_t st) {
 
 template <int NA>
 static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st) {
-    constexpr int NWM = RC_GRAD_WARPS<NA, RCMARL_LOSS_MSE>(), NWC = RC_GRAD_WARPS<NA, RCMARL_LOSS_CE>();
-    constexpr size_t smem_mse = sizeof(float) * (RC_GRAD_SMEM<NA, 3 * NA, 1, NWM>() > RC_GRAD_SMEM<NA, 2 * NA, 1, NWM>()
-                                                     ? RC_GRAD_SMEM<NA, 3 * NA, 1, NWM>() : RC_GRAD_SMEM<NA, 2 * NA, 1, NWM>());
-    constexpr size_t smem_ce = sizeof(float) * RC_GRAD_SMEM<NA, 2 * NA, NACT, NWC>();
+    constexpr int NWM = grad_warps<NA, RCMARL_LOSS_MSE>(), NWC = grad_warps<NA, RCMARL_LOSS_CE>();
+    constexpr size_t smem_mse = sizeof(float) * (grad_smem_floats<NA, 3 * NA, 1, NWM>() > grad_smem_floats<NA, 2 * NA, 1, NWM>()
+                                                     ? grad_smem_floats<NA, 3 * NA, 1, NWM>() : grad_smem_floats<NA, 2 * NA, 1, NWM>());
+    constexpr size_t smem_ce = sizeof(float) * grad_smem_floats<NA, 2 * NA, NACT, NWC>();
     static_assert(smem_mse <= 227 * 1024 && smem_ce <= 227 * 1024, "grad kernel exceeds the 227 KB shared-memory limit");
     static bool attr_ce = false, attr_mse = false;     // opt-in to > 48 KB dynamic shared memory once per process
     cudaLaunchAttribute pdl;
@@ -474,20 +431,20 @@ static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st
     cfg.numAttrs = 1;
     if (loss_mode == RCMARL_LOSS_CE) {
         if (!attr_ce) {
-            if (set_smem(RC_GRAD_KERNEL<NA, RCMARL_LOSS_CE>, smem_ce)) return RCMARL_ERR_CUDA;
+            if (set_smem(grad_kernel<NA, RCMARL_LOSS_CE>, smem_ce)) return RCMARL_ERR_CUDA;
             attr_ce = true;
         }
         cfg.blockDim = dim3(32 * NWC);
         cfg.dynamicSmemBytes = smem_ce;
-        RC_CUDA(cudaLaunchKernelEx(&cfg, RC_GRAD_KERNEL<NA, RCMARL_LOSS_CE>, P));
+        RC_CUDA(cudaLaunchKernelEx(&cfg, grad_kernel<NA, RCMARL_LOSS_CE>, P));
     } else {
         if (!attr_mse) {
-            if (set_smem(RC_GRAD_KERNEL<NA, RCMARL_LOSS_MSE>, smem_mse)) return RCMARL_ERR_CUDA;
+            if (set_smem(grad_kernel<NA, RCMARL_LOSS_MSE>, smem_mse)) return RCMARL_ERR_CUDA;
             attr_mse = true;
         }
         cfg.blockDim = dim3(32 * NWM);
         cfg.dynamicSmemBytes = smem_mse;
-        RC_CUDA(cudaLaunchKernelEx(&cfg, RC_GRAD_KERNEL<NA, RCMARL_LOSS_MSE>, P));
+        RC_CUDA(cudaLaunchKernelEx(&cfg, grad_kernel<NA, RCMARL_LOSS_MSE>, P));
     }
     RC_CUDA(cudaGetLastError());
     return 0;
@@ -496,7 +453,7 @@ static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st
 // chunks (64 rows) one CTA of this configuration consumes per sweep
 template <int NA>
 static int grad_chunks_per_cta(int loss_mode) {
-    return loss_mode == RCMARL_LOSS_CE ? RC_GRAD_WARPS<NA, RCMARL_LOSS_CE>() : RC_GRAD_WARPS<NA, RCMARL_LOSS_MSE>();
+    return loss_mode == RCMARL_LOSS_CE ? grad_warps<NA, RCMARL_LOSS_CE>() : grad_warps<NA, RCMARL_LOSS_MSE>();
 }
 
 template <int NA>
@@ -508,24 +465,19 @@ static int launch_team(const TeamParams& P, int n_list, int gy, cudaStream_t st)
     return 0;
 }
 
-// launch of the fused reduce kernels of the mini-batch loop; with RCMARL_PDL_REDUCE as a programmatic dependent of the
-// grad kernel before it (the kernel itself waits for that grid with griddepcontrol.wait)
-template <typename K, typename PT>
-static int launch_reduce(K kernel, const PT& params, dim3 grid, cudaStream_t st) {
-#if RCMARL_PDL_REDUCE
+// reduce_comm_kernel as a programmatic dependent of the kernel before it, so that its grid is queued while the
+// producer's last CTAs drain (the kernel itself waits for that grid with griddepcontrol.wait)
+static int launch_reduce_comm(const ReduceCommParams& C, cudaStream_t st) {
     cudaLaunchAttribute pdl;
     pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     pdl.val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
+    cfg.gridDim = reduce_comm_grid(C.max_n, C.n_jobs);
     cfg.blockDim = dim3(256);
     cfg.stream = st;
     cfg.attrs = &pdl;
     cfg.numAttrs = 1;
-    RC_CUDA(cudaLaunchKernelEx(&cfg, kernel, params));
-#else
-    kernel<<<grid, 256, 0, st>>>(params);
-#endif
+    RC_CUDA(cudaLaunchKernelEx(&cfg, reduce_comm_kernel, C));
     RC_CUDA(cudaGetLastError());
     return 0;
 }
@@ -539,24 +491,13 @@ static int grid_y_for(int64_t work_items, int n_jobs, int ctas_per_sm) {
     return (int)(gy < 1 ? 1 : gy);
 }
 
-// Shares of the one-wave, 1-D grid of grad_kernel: job j owns the CTAs [cta_first[j], cta_first[j + 1]).
-// Default: equal shares, floor(SMs / n_jobs) CTAs per job (all jobs then sweep the rows in lock-step, which keeps the
-// buffer rows they share in L2).  RCMARL_BALANCED_GRID=1 in the environment sizes the shares by cost instead: a job's
-// cost per row depends on its network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks, greedy: the job that
-// currently finishes last gets the next CTA.  It stays opt-in: it has not been measured faster on the update round.
-#ifndef RCMARL_BALANCED_GRID_DEFAULT
-#define RCMARL_BALANCED_GRID_DEFAULT 0
-#endif
-static bool balanced_grid_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("RCMARL_BALANCED_GRID");
-        v = e ? (e[0] != '0') : RCMARL_BALANCED_GRID_DEFAULT;
-    }
-    return v != 0;
-}
-
-// g[j] = CTAs of job j; pure host arithmetic (also behind rcmarl_grad_grid_plan for the CPU tests)
+// Shares of a one-wave grid over n jobs: g[j] = CTAs of job j; pure host arithmetic (also behind rcmarl_grad_grid_plan
+// for the CPU tests).
+//   balanced = false (rcmarl_grad): equal shares, floor(SMs / n_jobs) CTAs per job.  All jobs then sweep the same rows in
+//     lock-step, which keeps the buffer rows they share in L2.
+//   balanced = true (rcmarl_minibatch_fit, whose chains read different rows): shares sized by cost.  A job's cost per row
+//     depends on its network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks; greedy: the job that
+//     currently finishes last gets the next CTA.
 static void plan_shares(int n, const int* cost, int64_t nchunks, int gw, int sms, bool balanced, int* g) {
     int64_t units = (nchunks + gw - 1) / gw;
     if (units < 1) units = 1;
@@ -584,10 +525,11 @@ static void plan_shares(int n, const int* cost, int64_t nchunks, int gw, int sms
     }
 }
 
-static int plan_grad_grid(GradParams& P, PartialSlots& S, const int* cost, int64_t nchunks, int gw) {
+// 1-D grid of grad_kernel: job j owns the CTAs [cta_first[j], cta_first[j + 1]), equal shares
+static int plan_grad_grid(GradParams& P, PartialSlots& S, int64_t nchunks, int gw) {
     const int n = P.n_jobs;
     int g[RCMARL_MAX_JOBS];
-    plan_shares(n, cost, nchunks, gw, sm_count_cached(), balanced_grid_enabled(), g);
+    plan_shares(n, nullptr, nchunks, gw, sm_count_cached(), false, g);
     int first = 0;
     for (int j = 0; j < n; ++j) {
         P.cta_first[j] = (int16_t)first;
@@ -691,7 +633,6 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
     ReduceParams Q;
     P.rows = *rows;
     int maxn = 0;
-    int cost[RCMARL_MAX_JOBS];
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_grad_job& q = jobs[j];
         if (!q.w || !q.target || !q.sums || q.kind < 0 || q.kind > 2 || q.target_stride < 1) return RCMARL_ERR_ARG;
@@ -703,7 +644,6 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
                                                    : param_count(q.kind == RCMARL_IN_SA ? 3 * NA : 2 * NA, 1);
         Q.sums[j] = q.sums;
         Q.n[j] = n + 1;
-        cost[j] = grad_job_cost(NA, q.kind, loss_mode);
         if (n + 1 > maxn) maxn = n + 1;
     }
     const int64_t nchunks = (rows->n_rows + 63) / 64;
@@ -712,7 +652,7 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
     P.n_jobs = n_jobs;
     P.stride = maxn;
     Q.slots.stride = maxn;
-    const int n_ctas = plan_grad_grid(P, Q.slots, cost, nchunks, cpc);
+    const int n_ctas = plan_grad_grid(P, Q.slots, nchunks, cpc);
     if ((int64_t)n_ctas * maxn * (int64_t)sizeof(float) > ws_bytes) return RCMARL_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
     int e = NA == 5 ? launch_grad<5>(P, loss_mode, n_ctas, st) : launch_grad<16>(P, loss_mode, n_ctas, st);
@@ -721,81 +661,13 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
     if (comm_bound()) {
         ReduceCommParams C;
         if (!comm_next(&C.comm, (int64_t)n_jobs * maxn)) return RCMARL_ERR_ARG;
-        C.partial = Q.partial; C.slots = Q.slots; C.out_stride = maxn; C.fuse_sgd = 0; C.n_jobs = n_jobs; C.max_n = maxn;
+        C.partial = Q.partial; C.slots = Q.slots; C.out_stride = maxn; C.n_jobs = n_jobs; C.max_n = maxn;
         for (int j = 0; j < n_jobs; ++j) { C.sums[j] = Q.sums[j]; C.n[j] = Q.n[j]; }
-        if (launch_reduce(reduce_comm_kernel, C, reduce_comm_grid(maxn, n_jobs), st)) return RCMARL_ERR_CUDA;
+        if (launch_reduce_comm(C, st)) return RCMARL_ERR_CUDA;
     } else {
         reduce_kernel<<<dim3((maxn + 31) / 32, n_jobs), 256, 0, st>>>(Q);
     }
     RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
-}
-
-int rcmarl_minibatch_sgd(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, const rcmarl_sgd_job* sjobs, int n_jobs,
-                         int epochs, int n_times, int mb_times, float lr, void* ws, int64_t ws_bytes, void* stream) {
-    if (!rows || !rows->sa || !rows->ns || !rows->r || rows->n_envs <= 0) return RCMARL_ERR_ARG;
-    if (rows->n_agents != 5 && rows->n_agents != 16) return RCMARL_ERR_ARG;
-    if (!gjobs || !sjobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS || !ws || epochs < 1 || n_times < 1 || mb_times < 1)
-        return RCMARL_ERR_ARG;
-    const int NA = rows->n_agents;
-    GradParams P;
-    ReduceSgdParams Q;
-    P.rows = *rows;
-    int maxn = 0;
-    int cost[RCMARL_MAX_JOBS];
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_grad_job& q = gjobs[j];
-        if (!q.w || !q.target || !q.time_idx || q.kind < 0 || q.kind > 2 || q.target_stride < 1) return RCMARL_ERR_ARG;
-        if (!sjobs[j].dst || sjobs[j].dst != sjobs[j].src || (const float*)sjobs[j].dst != q.w) return RCMARL_ERR_ARG;
-        const int n = param_count(q.kind == RCMARL_IN_SA ? 3 * NA : 2 * NA, 1);
-        if (sjobs[j].n != n) return RCMARL_ERR_ARG;
-        P.jobs[j] = q;
-        Q.jobs[j] = sjobs[j];
-        cost[j] = grad_job_cost(NA, q.kind, RCMARL_LOSS_MSE);
-        if (n + 1 > maxn) maxn = n + 1;
-    }
-    P.partial = (float*)ws;
-    P.n_jobs = n_jobs;
-    P.stride = maxn;
-    Q.partial = (const float*)ws;
-    Q.slots.stride = maxn;
-    int n_ctas = 0, planned_cnt = -1;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int cpc = NA == 5 ? grad_chunks_per_cta<5>(RCMARL_LOSS_MSE) : grad_chunks_per_cta<16>(RCMARL_LOSS_MSE);
-    for (int e = 0; e < epochs; ++e) {
-        for (int b = 0; b < n_times; b += mb_times) {
-            const int cnt = n_times - b < mb_times ? n_times - b : mb_times;
-            const int64_t n_rows = (int64_t)cnt * rows->n_envs;
-            P.rows.n_rows = n_rows;
-            if (cnt != planned_cnt) {                        // the grid only depends on the mini-batch size
-                n_ctas = plan_grad_grid(P, Q.slots, cost, (n_rows + 63) / 64, cpc);
-                if ((int64_t)n_ctas * maxn * (int64_t)sizeof(float) > ws_bytes) return RCMARL_ERR_WORKSPACE;
-                planned_cnt = cnt;
-            }
-            for (int j = 0; j < n_jobs; ++j) {
-                P.jobs[j].time_idx = gjobs[j].time_idx + (int64_t)e * n_times + b;
-                Q.jobs[j].coef = lr * 2.0f / (float)n_rows;
-                if (e > 0) Q.jobs[j].loss_out = nullptr;
-            }
-            P.rows.time_idx = P.jobs[0].time_idx;
-            int err = NA == 5 ? launch_grad<5>(P, RCMARL_LOSS_MSE, n_ctas, st) : launch_grad<16>(P, RCMARL_LOSS_MSE, n_ctas, st);
-            if (err) return err;
-            if (comm_bound()) {
-                ReduceCommParams C;
-                if (!comm_next(&C.comm, (int64_t)n_jobs * maxn)) return RCMARL_ERR_ARG;
-                C.partial = Q.partial; C.slots = Q.slots; C.out_stride = maxn; C.fuse_sgd = 1; C.n_jobs = n_jobs; C.max_n = maxn;
-                for (int j = 0; j < n_jobs; ++j) {
-                    C.sums[j] = nullptr;
-                    C.n[j] = Q.jobs[j].n + 1;
-                    C.sgd[j] = Q.jobs[j];
-                    C.sgd[j].coef = lr * 2.0f / ((float)n_rows * (float)C.comm.world);   // global batch
-                }
-                if (launch_reduce(reduce_comm_kernel, C, reduce_comm_grid(maxn, n_jobs), st)) return RCMARL_ERR_CUDA;
-            } else {
-                if (launch_reduce(reduce_sgd_kernel, Q, dim3((maxn + 31) / 32, n_jobs), st)) return RCMARL_ERR_CUDA;
-            }
-        }
-    }
     return RCMARL_OK;
 }
 
@@ -928,9 +800,9 @@ int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs
         if (comm_bound()) {
             ReduceCommParams C;
             if (!comm_next(&C.comm, (int64_t)n_jobs * TEAM_N)) return RCMARL_ERR_ARG;
-            C.partial = Q.partial; C.slots = Q.slots; C.out_stride = TEAM_N; C.fuse_sgd = 0; C.n_jobs = n_jobs; C.max_n = TEAM_N;
+            C.partial = Q.partial; C.slots = Q.slots; C.out_stride = TEAM_N; C.n_jobs = n_jobs; C.max_n = TEAM_N;
             for (int j = 0; j < n_jobs; ++j) { C.sums[j] = Q.sums[j]; C.n[j] = Q.n[j]; }
-            if (launch_reduce(reduce_comm_kernel, C, reduce_comm_grid(TEAM_N, n_jobs), st)) return RCMARL_ERR_CUDA;
+            if (launch_reduce_comm(C, st)) return RCMARL_ERR_CUDA;
         } else {
             reduce_kernel<<<dim3((TEAM_N + 31) / 32, n_jobs), 256, 0, st>>>(Q);
         }

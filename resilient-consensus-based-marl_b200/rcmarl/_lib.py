@@ -8,7 +8,8 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("RCMARL_LIB", os.path.join(_HERE, "librcmarl.so"))   # override: kernel experiments only
+# override: another build of the library, e.g. to compare two builds output by output (bench.py --dump-outputs)
+LIB_PATH = os.environ.get("RCMARL_LIB", os.path.join(_HERE, "librcmarl.so"))
 
 MAX_JOBS = 32
 MAX_TERMS = 3
@@ -89,8 +90,6 @@ SYMBOLS = [
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
     ("rcmarl_adam_apply", C.c_int, [C.POINTER(AdamJob), C.c_int, c_fp]),
-    ("rcmarl_minibatch_sgd", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.POINTER(SgdJob), C.c_int, C.c_int, C.c_int,
-                                       C.c_int, C.c_float, c_fp, C.c_int64, c_fp]),
     ("rcmarl_minibatch_cells_bytes", C.c_int64, [C.c_int, C.c_int]),
     ("rcmarl_minibatch_steps", C.c_int64, [C.c_int, C.c_int, C.c_int]),
     ("rcmarl_minibatch_fit", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.POINTER(SgdJob), C.c_int, C.c_int, C.c_int,
@@ -125,10 +124,7 @@ def lib():
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU / PyTorch fallback for the RPBCAC kernels)")
         l = C.CDLL(LIB_PATH)
-        lax = os.environ.get("RCMARL_LIB_LAX") == "1"      # kernel A/B runs against older builds only (tools/ab_grad.py)
         for name, res, args in SYMBOLS:
-            if lax and not hasattr(l, name):
-                continue
             f = getattr(l, name)          # AttributeError if the ABI and the header diverge
             f.restype = res
             f.argtypes = args

@@ -1,6 +1,6 @@
 """Peer-memory exchange context for data-parallel training on one node (include/rcmarl.h, csrc/comm.cuh):
 each rank allocates an exchange buffer, the CUDA IPC handles are swapped through torch.distributed (plumbing), and the
-context is bound so that rcmarl_grad / rcmarl_team / rcmarl_minibatch_sgd reduce across GPUs inside their own kernels
+context is bound so that rcmarl_grad / rcmarl_team / rcmarl_minibatch_fit reduce across GPUs inside their own kernels
 over NVLink -- no NCCL call per optimisation step."""
 import ctypes as C
 

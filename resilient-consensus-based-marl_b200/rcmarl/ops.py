@@ -139,16 +139,6 @@ def sgd_apply(jobs):
     L.check(L.lib().rcmarl_sgd_apply(a, len(a), _stream()), "rcmarl_sgd_apply")
 
 
-def minibatch_sgd(rows, gjobs, sjobs, epochs, n_times, mb_times, lr, ws=None):
-    """Whole mini-batch fit (all epochs, all steps) in one library call (single GPU)."""
-    ga = gjobs if isinstance(gjobs, C.Array) else _arr(L.GradJob, gjobs)
-    sa = sjobs if isinstance(sjobs, C.Array) else _arr(L.SgdJob, sjobs)
-    if ws is None:
-        ws = workspace()
-    L.check(L.lib().rcmarl_minibatch_sgd(C.byref(rows), ga, sa, len(ga), epochs, n_times, mb_times, lr, ws.data_ptr(),
-                                         ws.numel(), _stream()), "rcmarl_minibatch_sgd")
-
-
 class MinibatchCells:
     """Scratch of the persistent mini-batch kernel (rcmarl_minibatch_fit): zero-initialised {value, sequence} cells plus
     the host-side sequence counter (every step of every call consumes one number, never reused)."""
@@ -173,6 +163,28 @@ def minibatch_fit(rows, gjobs, sjobs, epochs, n_times, mb_times, lr, cells):
                                          cells.buf.data_ptr(), cells.buf.numel(), cells.seq, _stream()),
             "rcmarl_minibatch_fit")
     cells.seq += steps
+
+
+def minibatch_steps(rows, gjobs, sjobs, epochs, n_times, mb_times, lrs, world=1, allreduce=None, ws=None):
+    """The fit of minibatch_fit (same job tables; lrs[j] = learning rate of chain j) as rcmarl_grad -> allreduce() ->
+    rcmarl_sgd_apply per step: the data-parallel path without a peer-memory exchange, where allreduce() sums the
+    chains' gradient sums over the `world` ranks in place."""
+    ga, sa = _arr(L.GradJob, list(gjobs)), _arr(L.SgdJob, list(sjobs))     # copies: the loop rewrites them
+    tables = [g.time_idx for g in ga]
+    for e in range(epochs):
+        for b in range(0, n_times, mb_times):
+            rows.n_rows = min(mb_times, n_times - b) * rows.n_envs
+            for j, (g, s) in enumerate(zip(ga, sa)):
+                g.time_idx = tables[j] + 4 * (e * n_times + b)
+                s.coef = lrs[j] * 2.0 / (rows.n_rows * world)
+                if b > 0:
+                    s.loss_accumulate = 1                   # the loss is summed over the steps of epoch 0 ...
+                if e == 1 and b == 0:
+                    s.loss_out = None                       # ... only (history['loss'][0])
+            grad(rows, ga, L.LOSS_MSE, ws)
+            if allreduce is not None:
+                allreduce()
+            sgd_apply(sa)
 
 
 def adam_job(theta, m, v, sums, n, grad_scale, lr_t, beta1=0.9, beta2=0.999, eps=1e-7, loss_out=None, loss_coef=0.0,

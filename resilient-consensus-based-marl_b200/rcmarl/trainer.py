@@ -117,10 +117,8 @@ class Trainer:
         self.loss_t = torch.zeros(NA, **f32)
         self.loss_a = torch.zeros(NA, **f32)
         self.ws = ops.workspace(L.MAX_JOBS, self.PT if NA == 5 else L.param_count(48, 1))
-        # persistent mini-batch kernel (rcmarl_minibatch_fit); RCMARL_MB_PERSIST=0 selects the round-1 launch chain
-        self.mb_cells = None
-        if os.environ.get("RCMARL_MB_PERSIST", "1") != "0":
-            self.mb_cells = ops.MinibatchCells(L.MAX_JOBS, self.PT if NA == 5 else L.param_count(48, 1), self.dev)
+        # scratch of the persistent mini-batch kernel (rcmarl_minibatch_fit)
+        self.mb_cells = ops.MinibatchCells(L.MAX_JOBS, self.PT if NA == 5 else L.param_count(48, 1), self.dev)
         self.launches = 0                                 # kernels launched by this engine (bench: gpu_launches)
         self.profile = None                               # bench.py: {"fit_grad": [(start_evt, end_evt), ...], ...}
         self.h2d_bytes = 4 * sum(x.numel() for x in (self.actor, self.critic, self.tr, self.critic_local))
@@ -401,54 +399,27 @@ class Trainer:
 
     def _minibatch_sgd(self, chains, T):
         """10 epochs x ceil(T/32) sequential SGD steps per chain; a mini-batch = 32 time rows x all environments
-        (Appendix C).  All chains advance in lock-step: one grad launch + one apply launch per step."""
-        N, nb = self.N, (T + self.mb_times - 1) // self.mb_times
+        (Appendix C).  All chains advance in lock-step in ONE persistent kernel, or, data-parallel without the
+        peer-memory exchange, as rcmarl_grad -> NCCL all-reduce -> rcmarl_sgd_apply per step."""
         E = self.mb_epochs
         perms = torch.stack([torch.stack([self._perm(T) for _ in range(E)]) for _ in chains]).to(self.dev)  # [C,E,T]
         self.h2d_bytes += 4 * perms.numel()
-        base = perms.data_ptr()
         gj, aj = [], []
-        lrs = [ch[5] if len(ch) > 5 else self.fast_lr[0] for ch in chains]
-        for c, (w, kind, tgt, st, loss) in enumerate([ch[:5] for ch in chains]):
+        for c, (w, kind, tgt, st, loss, lr) in enumerate(chains):
             n = self.PT if kind == L.IN_SA else self.PC
             sums = self.sums_mb[c][:n + 1]
-            gj.append(ops.grad_job(w, tgt, sums, kind, target_stride=st, time_idx=perms))
-            persistent = self.mb_cells is not None and (self.world == 1 or self.comm is not None)
-            aj.append(ops.sgd_job(w, w, sums, n, 0.0, loss_out=loss, loss_coef=1.0 / (T * N * self.world),
-                                  loss_accumulate=0 if persistent else 1))     # the persistent kernel writes the epoch-0 loss once
-            if loss is not None and not persistent:
-                loss.zero_()
-        gj, aj = (L.GradJob * len(gj))(*gj), (L.SgdJob * len(aj))(*aj)
+            gj.append(ops.grad_job(w, tgt, sums, kind, target_stride=st, time_idx=perms[c]))
+            aj.append(ops.sgd_job(w, w, sums, n, lr, loss_out=loss, loss_coef=1.0 / (T * self.N * self.world)))
         rows = self._rows(0, 0, perms)
-        nC = len(chains)
-        nb_steps = E * nb
-        if self.world == 1 or self.comm is not None:       # whole fit in one library call (fused reduce [+ exchange] + apply)
-            for c in range(nC):
-                gj[c].time_idx = base + 4 * (c * E * T)
-            if self.mb_cells is not None:                   # one persistent kernel for the whole fit
-                for c in range(nC):
-                    aj[c].coef = lrs[c]                     # per-chain learning rate
-                ops.minibatch_fit(rows, gj, aj, E, T, self.mb_times, lrs[0], self.mb_cells)
-                self.launches += 1
-                return
-            if len(set(lrs)) != 1:
-                raise L.RcmarlError("the launch-chain mini-batch path takes one learning rate; use the persistent kernel")
-            ops.minibatch_sgd(rows, gj, aj, E, T, self.mb_times, lrs[0], self.ws)
-            self.launches += 2 * nb_steps
-            return
-        for e in range(E):
-            for b in range(nb):
-                cnt = min(self.mb_times, T - b * self.mb_times)
-                rows.n_rows = cnt * N
-                for c in range(nC):
-                    gj[c].time_idx = base + 4 * ((c * E + e) * T + b * self.mb_times)
-                    aj[c].coef = lrs[c] * 2.0 / (cnt * N * self.world)
-                    if e == 1 and b == 0:
-                        aj[c].loss_out = None                              # history['loss'][0]: epoch 0 only
-                ops.grad(rows, gj, L.LOSS_MSE, self.ws)
-                self._allreduce(self.sums_mb[:nC])
-                ops.sgd_apply(aj)
-                self.launches += 3
+        lrs = [ch[5] for ch in chains]
+        if self.world == 1 or self.comm is not None:
+            ops.minibatch_fit(rows, gj, aj, E, T, self.mb_times, lrs[0], self.mb_cells)
+            self.launches += 1
+        else:
+            nC = len(chains)
+            ops.minibatch_steps(rows, gj, aj, E, T, self.mb_times, lrs, self.world,
+                                lambda: self._allreduce(self.sums_mb[:nC]), self.ws)
+            self.launches += 3 * E * ((T + self.mb_times - 1) // self.mb_times)
 
     def _minibatch_adam(self, adv, T, Ta, a0):
         """actor.fit(batch_size=200, epochs=1) of the adversaries (adversarial:41,116,224)."""

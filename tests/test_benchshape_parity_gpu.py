@@ -1,7 +1,7 @@
 """Oracle parity AT THE BENCHMARKED SHAPES (one GPU):
  (a) a Malicious + cooperative update round through rcmarl.trainer.Trainer with n_envs in {64, 128}: gathered row mode
-     with n_envs % 64 == 0, i.e. the bulk-copy (TMA) staging branch of grad_kernel and the rcmarl_minibatch_sgd chain
-     that the C2 benchmark spends half of its step in -- against the fp64 oracle;
+     with n_envs % 64 == 0, i.e. the bulk-copy (TMA) staging branch of grad_kernel and the persistent mini-batch kernel
+     (rcmarl_minibatch_fit) that the C2 benchmark spends half of its step in -- against the fp64 oracle;
  (b) rcmarl_grad over 4.1 M buffer rows (the C2 row count of one block) against NumPy fp64 sums (chunked);
  (c) rcmarl_clip_mean on the C5 tensor (64 x 1 048 576), H in {0, 1, 2, 4}, against oracle.resilient_aggregation;
  (d) the reference's own train_RPBCAC run with a Greedy and a Faulty agent and common_reward=True

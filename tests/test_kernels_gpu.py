@@ -453,11 +453,12 @@ def test_env_step_matches_reference_fixture(K):
 
 # ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("NA,nrow,N,T", [(5, 5, 64, 40), (5, 5, 24, 37), (16, 10, 64, 33), (5, 5, 1, 96)])
-def test_minibatch_fit_persistent_kernel_matches_oracle_and_launch_chain(K, NA, nrow, N, T):
+def test_minibatch_fit_persistent_kernel_matches_oracle_and_step_loop(K, NA, nrow, N, T):
     """rcmarl_minibatch_fit (ONE persistent kernel: parameters resident in shared memory, cross-CTA reduction through
     {value, sequence} cells) against (a) the fp64 oracle's fit_minibatch with the same injected permutations
     (agents/adversarial_CAC_agents.py:133,150,163: fit(batch_size=32, epochs=E), Appendix C batching) and (b) the
-    round-1 launch chain rcmarl_minibatch_sgd; and bitwise reproducibility of two runs."""
+    per-step loop ops.minibatch_steps (rcmarl_grad -> rcmarl_sgd_apply, the data-parallel NCCL path) at world 1;
+    and bitwise reproducibility of two runs."""
     rs = np.random.RandomState(NA + N + T)
     E, mb, lr = 3, 32, 0.01
     B = N * T
@@ -488,7 +489,7 @@ def test_minibatch_fit_persistent_kernel_matches_oracle_and_launch_chain(K, NA, 
             K.ops.minibatch_fit(rows, gj, aj, E, T, mb, lr, cells)
             K.ops.minibatch_fit(rows, gj, aj, E, T, mb, 0.0 * lr + 1e-30, cells)     # second call on the same cells: a no-op step size
         else:
-            K.ops.minibatch_sgd(rows, gj, aj, E, T, mb, lr)
+            K.ops.minibatch_steps(rows, gj, aj, E, T, mb, [lr] * len(kinds))
         torch.cuda.synchronize()
         return [w.cpu().numpy() for w in ws], loss.cpu().numpy()
     w_p, loss_p = run(True)
