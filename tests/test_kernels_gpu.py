@@ -12,47 +12,13 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from golden_util import pretrained                     # noqa: E402
+from kernel_util import close, load_kernels, rand_net, synth, to_dev   # noqa: E402
 from oracle import rpbcac_oracle as O                  # noqa: E402  (checker only)
 
 
 @pytest.fixture(scope="module")
 def K():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    from rcmarl import ops, nets, _lib
-    _lib.lib()                                           # fail loudly if the .so is missing
-    class NS:                                            # noqa: E306
-        pass
-    k = NS()
-    k.ops, k.nets, k.L = ops, nets, _lib
-    k.dev = torch.device("cuda:0")
-    return k
-
-
-def synth(rs, B, NA=5, nrow=5):
-    pos = rs.randint(0, nrow, size=(B, NA, 2))
-    npos = np.clip(pos + rs.randint(-1, 2, size=pos.shape), 0, nrow - 1)
-    mean, std = (nrow - 1) / 2.0, np.std(np.arange(nrow))
-    s = ((pos - mean) / std).astype(np.float32)
-    ns = ((npos - mean) / std).astype(np.float32)
-    a = rs.randint(0, 5, size=(B, NA, 1)).astype(np.float32)
-    r = (-rs.randint(0, 2 * nrow, size=(B, NA, 1)) / 5.0).astype(np.float32)
-    return s, ns, a, r
-
-
-def rand_net(rs, d_in, n_out):
-    from rcmarl import nets
-    w = nets.glorot_uniform(d_in, n_out, rs)
-    return [x + (0.05 * rs.randn(*x.shape)).astype(np.float32) for x in w]
-
-
-def to_dev(K, *arrs):
-    return [torch.as_tensor(np.ascontiguousarray(a)).to(K.dev) for a in arrs]
-
-
-def close(got, want, rtol=1e-4, atol=1e-6):
-    got = got.detach().cpu().numpy() if isinstance(got, torch.Tensor) else np.asarray(got)
-    np.testing.assert_allclose(got.astype(np.float64), np.asarray(want, np.float64), rtol=rtol, atol=atol)
+    return load_kernels()
 
 
 # ------------------------------------------------------------------------------------------
