@@ -130,7 +130,7 @@ struct GradParams {
     float* partial;   // [CTA][stride]: one slot per CTA of the 1-D grid
     int32_t n_jobs;
     int32_t stride;
-    // job j owns the CTAs [cta_first[j], cta_first[j + 1]) of the 1-D grid (train_kernels.cu, plan_grad_grid)
+    // job j owns the CTAs [cta_first[j], cta_first[j + 1]) of the 1-D grid (train_kernels.cu, plan_grid)
     int16_t cta_first[RCMARL_MAX_JOBS + 1];
 };
 
@@ -469,7 +469,7 @@ __device__ __forceinline__ void grad_body(const GradParams& P, const rcmarl_grad
     core.write_pads();
     core.zero_acc();
     core.sweep(Rw, job, y, gy);
-    // a reduce kernel launched as a programmatic dependent (launch_reduce_comm, train_kernels.cu) is queued once every CTA is
+    // a reduce kernel launched as a programmatic dependent (reduce_partials, train_kernels.cu) is queued once every CTA is
     // past its row loop, i.e. before the last CTA exits; it waits for this grid with griddepcontrol.wait
     pdl_launch_dependents();
     float* out = P.partial + (int64_t)blockIdx.x * P.stride;
@@ -501,6 +501,19 @@ constexpr int grad_smem_floats() {
     static_assert(tiles >= red, "the CTA reduction buffer reuses the tile region");
     constexpr int stage = (grad_use_tma(NA) ? NW * L::ROWS * 3 * NA : 0) + 2 * NW + 8;   // staged rows + one mbarrier per warp
     return round4(param_count(DIN, NOUT)) + tiles + stage + 16;
+}
+
+// dynamic shared memory of grad_kernel<NA, LOSS> (and of mb_persist_kernel<NA>, LOSS = MSE): one launch serves every job
+// kind of its loss, so MSE takes the larger of the SA-net and S-net layouts
+template <int NA, int LOSS>
+constexpr size_t grad_smem_bytes() {
+    constexpr int NW = grad_warps<NA, LOSS>();
+    if constexpr (LOSS == RCMARL_LOSS_CE) {
+        return sizeof(float) * grad_smem_floats<NA, 2 * NA, NACT, NW>();
+    } else {
+        constexpr int sa = grad_smem_floats<NA, 3 * NA, 1, NW>(), s = grad_smem_floats<NA, 2 * NA, 1, NW>();
+        return sizeof(float) * (sa > s ? sa : s);
+    }
 }
 
 }  // namespace rcmarl

@@ -193,13 +193,6 @@ __global__ void __launch_bounds__(256) reduce_comm_kernel(const __grid_constant_
     }
 }
 
-// grid of reduce_comm_kernel: one CTA per item up to two resident CTAs per SM
-static dim3 reduce_comm_grid(int max_n, int n_jobs) {
-    const int items = ((max_n + 31) / 32) * n_jobs;
-    const int cap = sm_count_cached() * 2;
-    return dim3(items < cap ? items : cap);
-}
-
 // ============================================================================================
 // team: estimates + clipped mean + projection numerators
 // ============================================================================================
@@ -413,47 +406,36 @@ static int launch_values(const ValuesParams& P, int n_jobs, cudaStream_t st) {
     return 0;
 }
 
-template <int NA>
-static int launch_grad(GradParams& P, int loss_mode, int n_ctas, cudaStream_t st) {
-    constexpr int NWM = grad_warps<NA, RCMARL_LOSS_MSE>(), NWC = grad_warps<NA, RCMARL_LOSS_CE>();
-    constexpr size_t smem_mse = sizeof(float) * (grad_smem_floats<NA, 3 * NA, 1, NWM>() > grad_smem_floats<NA, 2 * NA, 1, NWM>()
-                                                     ? grad_smem_floats<NA, 3 * NA, 1, NWM>() : grad_smem_floats<NA, 2 * NA, 1, NWM>());
-    constexpr size_t smem_ce = sizeof(float) * grad_smem_floats<NA, 2 * NA, NACT, NWC>();
-    static_assert(smem_mse <= 227 * 1024 && smem_ce <= 227 * 1024, "grad kernel exceeds the 227 KB shared-memory limit");
-    static bool attr_ce = false, attr_mse = false;     // opt-in to > 48 KB dynamic shared memory once per process
+// Launch as a programmatic dependent of the kernel before it on the stream, so that its grid is queued while the
+// producer's last CTAs drain; the kernel waits for that grid itself (pdl_wait, griddepcontrol.wait) before it reads
+// the producer's output.
+template <typename K, typename Params>
+static int launch_pdl(K kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Params& P) {
     cudaLaunchAttribute pdl;
     pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     pdl.val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_ctas);
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cfg.attrs = &pdl;
     cfg.numAttrs = 1;
-    if (loss_mode == RCMARL_LOSS_CE) {
-        if (!attr_ce) {
-            if (set_smem(grad_kernel<NA, RCMARL_LOSS_CE>, smem_ce)) return RCMARL_ERR_CUDA;
-            attr_ce = true;
-        }
-        cfg.blockDim = dim3(32 * NWC);
-        cfg.dynamicSmemBytes = smem_ce;
-        RC_CUDA(cudaLaunchKernelEx(&cfg, grad_kernel<NA, RCMARL_LOSS_CE>, P));
-    } else {
-        if (!attr_mse) {
-            if (set_smem(grad_kernel<NA, RCMARL_LOSS_MSE>, smem_mse)) return RCMARL_ERR_CUDA;
-            attr_mse = true;
-        }
-        cfg.blockDim = dim3(32 * NWM);
-        cfg.dynamicSmemBytes = smem_mse;
-        RC_CUDA(cudaLaunchKernelEx(&cfg, grad_kernel<NA, RCMARL_LOSS_MSE>, P));
-    }
+    RC_CUDA(cudaLaunchKernelEx(&cfg, kernel, P));
     RC_CUDA(cudaGetLastError());
     return 0;
 }
 
-// chunks (64 rows) one CTA of this configuration consumes per sweep
-template <int NA>
-static int grad_chunks_per_cta(int loss_mode) {
-    return loss_mode == RCMARL_LOSS_CE ? grad_warps<NA, RCMARL_LOSS_CE>() : grad_warps<NA, RCMARL_LOSS_MSE>();
+template <int NA, int LOSS>
+static int launch_grad(const GradParams& P, int n_ctas, cudaStream_t st) {
+    constexpr size_t smem = grad_smem_bytes<NA, LOSS>();
+    static_assert(smem <= 227 * 1024, "grad kernel exceeds the 227 KB shared-memory limit");
+    static bool attr = false;                          // opt-in to > 48 KB dynamic shared memory once per process
+    if (!attr) {
+        if (set_smem(grad_kernel<NA, LOSS>, smem)) return RCMARL_ERR_CUDA;
+        attr = true;
+    }
+    return launch_pdl(grad_kernel<NA, LOSS>, dim3(n_ctas), dim3(32 * grad_warps<NA, LOSS>()), smem, st, P);
 }
 
 template <int NA>
@@ -465,21 +447,20 @@ static int launch_team(const TeamParams& P, int n_list, int gy, cudaStream_t st)
     return 0;
 }
 
-// reduce_comm_kernel as a programmatic dependent of the kernel before it, so that its grid is queued while the
-// producer's last CTAs drain (the kernel itself waits for that grid with griddepcontrol.wait)
-static int launch_reduce_comm(const ReduceCommParams& C, cudaStream_t st) {
-    cudaLaunchAttribute pdl;
-    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pdl.val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = reduce_comm_grid(C.max_n, C.n_jobs);
-    cfg.blockDim = dim3(256);
-    cfg.stream = st;
-    cfg.attrs = &pdl;
-    cfg.numAttrs = 1;
-    RC_CUDA(cudaLaunchKernelEx(&cfg, reduce_comm_kernel, C));
-    RC_CUDA(cudaGetLastError());
-    return 0;
+// Sum the CTA partials of n_jobs jobs (Q.n[j] <= max_n floats each) into Q.sums: reduce_kernel, or, with a bound
+// exchange context, reduce_comm_kernel, which also sums over the ranks.  Returns an RCMARL status.
+static int reduce_partials(const ReduceParams& Q, int n_jobs, int max_n, cudaStream_t st) {
+    if (!comm_bound()) {
+        reduce_kernel<<<dim3((max_n + 31) / 32, n_jobs), 256, 0, st>>>(Q);
+        RC_CUDA(cudaGetLastError());
+        return RCMARL_OK;
+    }
+    ReduceCommParams C;
+    if (!comm_next(&C.comm, (int64_t)n_jobs * max_n)) return RCMARL_ERR_ARG;
+    C.partial = Q.partial; C.slots = Q.slots; C.out_stride = max_n; C.n_jobs = n_jobs; C.max_n = max_n;
+    for (int j = 0; j < n_jobs; ++j) { C.sums[j] = Q.sums[j]; C.n[j] = Q.n[j]; }
+    const int items = ((max_n + 31) / 32) * n_jobs, cap = sm_count_cached() * 2;    // up to two resident CTAs per SM
+    return launch_pdl(reduce_comm_kernel, dim3(items < cap ? items : cap), dim3(256), 0, st, C);
 }
 
 static int grid_y_for(int64_t work_items, int n_jobs, int ctas_per_sm) {
@@ -525,20 +506,17 @@ static void plan_shares(int n, const int* cost, int64_t nchunks, int gw, int sms
     }
 }
 
-// 1-D grid of grad_kernel: job j owns the CTAs [cta_first[j], cta_first[j + 1]), equal shares
-static int plan_grad_grid(GradParams& P, PartialSlots& S, int64_t nchunks, int gw) {
-    const int n = P.n_jobs;
+// 1-D grid of grad_kernel / mb_persist_kernel with the plan_shares shares: job j owns the CTAs
+// [cta_first[j], cta_first[j + 1]).  Returns the CTA count.
+static int plan_grid(int n, const int* cost, int64_t nchunks, int gw, bool balanced, int16_t* cta_first) {
     int g[RCMARL_MAX_JOBS];
-    plan_shares(n, nullptr, nchunks, gw, sm_count_cached(), false, g);
+    plan_shares(n, cost, nchunks, gw, sm_count_cached(), balanced, g);
     int first = 0;
     for (int j = 0; j < n; ++j) {
-        P.cta_first[j] = (int16_t)first;
-        S.first[j] = first;
-        S.count[j] = g[j];
+        cta_first[j] = (int16_t)first;
         first += g[j];
     }
-    P.cta_first[n] = (int16_t)first;
-    S.step = 1;
+    cta_first[n] = (int16_t)first;
     return first;
 }
 
@@ -552,8 +530,7 @@ static int grad_job_cost(int na, int kind, int loss_mode) {
 template <int NA>
 static int launch_mb_persist(const MbParams& P, int n_ctas, cudaStream_t st) {
     constexpr int NW = grad_warps<NA, RCMARL_LOSS_MSE>();
-    constexpr size_t smem = sizeof(float) * (grad_smem_floats<NA, 3 * NA, 1, NW>() > grad_smem_floats<NA, 2 * NA, 1, NW>()
-                                                 ? grad_smem_floats<NA, 3 * NA, 1, NW>() : grad_smem_floats<NA, 2 * NA, 1, NW>());
+    constexpr size_t smem = grad_smem_bytes<NA, RCMARL_LOSS_MSE>();
     static int resident = -1;                          // CTAs that can be co-resident (the cells protocol needs all of them)
     if (resident < 0) {
         if (set_smem(mb_persist_kernel<NA>, smem)) return RCMARL_ERR_CUDA;
@@ -562,19 +539,7 @@ static int launch_mb_persist(const MbParams& P, int n_ctas, cudaStream_t st) {
         resident = per_sm * sm_count_cached();
     }
     if (n_ctas > resident) return RCMARL_ERR_ARG;
-    cudaLaunchAttribute pdl;
-    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pdl.val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(n_ctas);
-    cfg.blockDim = dim3(32 * NW);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cfg.attrs = &pdl;
-    cfg.numAttrs = 1;
-    RC_CUDA(cudaLaunchKernelEx(&cfg, mb_persist_kernel<NA>, P));
-    RC_CUDA(cudaGetLastError());
-    return 0;
+    return launch_pdl(mb_persist_kernel<NA>, dim3(n_ctas), dim3(32 * NW), smem, st, P);
 }
 
 }  // namespace rcmarl
@@ -599,7 +564,9 @@ int rcmarl_grad_grid_plan(int n_agents, const int32_t* kinds_host, int n_jobs, i
         if (kinds_host[j] < 0 || kinds_host[j] > 2) return RCMARL_ERR_ARG;
         cost[j] = grad_job_cost(n_agents, kinds_host[j], loss_mode);
     }
-    const int cpc = n_agents == 5 ? grad_chunks_per_cta<5>(loss_mode) : grad_chunks_per_cta<16>(loss_mode);
+    const bool ce = loss_mode == RCMARL_LOSS_CE;
+    const int cpc = n_agents == 5 ? (ce ? grad_warps<5, RCMARL_LOSS_CE>() : grad_warps<5, RCMARL_LOSS_MSE>())
+                                  : (ce ? grad_warps<16, RCMARL_LOSS_CE>() : grad_warps<16, RCMARL_LOSS_MSE>());
     plan_shares(n_jobs, cost, (n_rows + 63) / 64, cpc, sm_count, balanced != 0, g);
     for (int j = 0; j < n_jobs; ++j) ctas_host[j] = g[j];
     return RCMARL_OK;
@@ -646,29 +613,27 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
         Q.n[j] = n + 1;
         if (n + 1 > maxn) maxn = n + 1;
     }
-    const int64_t nchunks = (rows->n_rows + 63) / 64;
-    const int cpc = NA == 5 ? grad_chunks_per_cta<5>(loss_mode) : grad_chunks_per_cta<16>(loss_mode);
+    // equal CTA shares; each warp of a CTA takes one 64-row chunk per sweep
+    const bool ce = loss_mode == RCMARL_LOSS_CE;
+    const int cpc = NA == 5 ? (ce ? grad_warps<5, RCMARL_LOSS_CE>() : grad_warps<5, RCMARL_LOSS_MSE>())
+                            : (ce ? grad_warps<16, RCMARL_LOSS_CE>() : grad_warps<16, RCMARL_LOSS_MSE>());
     P.partial = (float*)ws;
     P.n_jobs = n_jobs;
     P.stride = maxn;
-    Q.slots.stride = maxn;
-    const int n_ctas = plan_grad_grid(P, Q.slots, nchunks, cpc);
+    const int n_ctas = plan_grid(n_jobs, nullptr, (rows->n_rows + 63) / 64, cpc, false, P.cta_first);
     if ((int64_t)n_ctas * maxn * (int64_t)sizeof(float) > ws_bytes) return RCMARL_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
-    int e = NA == 5 ? launch_grad<5>(P, loss_mode, n_ctas, st) : launch_grad<16>(P, loss_mode, n_ctas, st);
+    const int e = NA == 5 ? (ce ? launch_grad<5, RCMARL_LOSS_CE>(P, n_ctas, st) : launch_grad<5, RCMARL_LOSS_MSE>(P, n_ctas, st))
+                          : (ce ? launch_grad<16, RCMARL_LOSS_CE>(P, n_ctas, st) : launch_grad<16, RCMARL_LOSS_MSE>(P, n_ctas, st));
     if (e) return e;
     Q.partial = (const float*)ws;
-    if (comm_bound()) {
-        ReduceCommParams C;
-        if (!comm_next(&C.comm, (int64_t)n_jobs * maxn)) return RCMARL_ERR_ARG;
-        C.partial = Q.partial; C.slots = Q.slots; C.out_stride = maxn; C.n_jobs = n_jobs; C.max_n = maxn;
-        for (int j = 0; j < n_jobs; ++j) { C.sums[j] = Q.sums[j]; C.n[j] = Q.n[j]; }
-        if (launch_reduce_comm(C, st)) return RCMARL_ERR_CUDA;
-    } else {
-        reduce_kernel<<<dim3((maxn + 31) / 32, n_jobs), 256, 0, st>>>(Q);
+    Q.slots.step = 1;
+    Q.slots.stride = maxn;
+    for (int j = 0; j < n_jobs; ++j) {
+        Q.slots.first[j] = P.cta_first[j];
+        Q.slots.count[j] = P.cta_first[j + 1] - P.cta_first[j];
     }
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    return reduce_partials(Q, n_jobs, maxn, st);
 }
 
 int64_t rcmarl_minibatch_cells_bytes(int n_jobs, int max_params) {
@@ -686,16 +651,16 @@ int64_t rcmarl_minibatch_steps(int epochs, int n_times, int mb_times) {
 int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, const rcmarl_sgd_job* sjobs, int n_jobs,
                          int epochs, int n_times, int mb_times, float lr, void* cells, int64_t cells_bytes,
                          uint32_t seq_first, void* stream) {
-    if (!rows || !rows->sa || !rows->ns || !rows->r || rows->n_envs <= 0) return RCMARL_ERR_ARG;
-    if (rows->n_agents != 5 && rows->n_agents != 16) return RCMARL_ERR_ARG;
-    if (!gjobs || !sjobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS || !cells || epochs < 1 || n_times < 1 || mb_times < 1 ||
-        seq_first < 1)
-        return RCMARL_ERR_ARG;
-    const int NA = rows->n_agents;
+    if (!rows) return RCMARL_ERR_ARG;
     MbParams P;
     P.rows = *rows;
     P.rows.n_rows = 0;
     P.rows.time_idx = nullptr;
+    if (int e = check_rows(&P.rows)) return e;
+    if (!gjobs || !sjobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS || !cells || epochs < 1 || n_times < 1 || mb_times < 1 ||
+        seq_first < 1)
+        return RCMARL_ERR_ARG;
+    const int NA = rows->n_agents;
     int maxn = 0;
     int cost[RCMARL_MAX_JOBS];
     for (int j = 0; j < n_jobs; ++j) {
@@ -711,18 +676,12 @@ int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, 
         cost[j] = grad_job_cost(NA, q.kind, RCMARL_LOSS_MSE);
         if (n + 1 > maxn) maxn = n + 1;
     }
-    const int cpc = NA == 5 ? grad_chunks_per_cta<5>(RCMARL_LOSS_MSE) : grad_chunks_per_cta<16>(RCMARL_LOSS_MSE);
+    const int cpc = NA == 5 ? grad_warps<5, RCMARL_LOSS_MSE>() : grad_warps<16, RCMARL_LOSS_MSE>();
     const int64_t n_rows_mb = (int64_t)(n_times < mb_times ? n_times : mb_times) * rows->n_envs;
     // CTA shares by cost (the chains do not share rows in L2 the way the lock-step full-batch jobs do).  A mapping with every
     // CTA serving every chain in turn (reduction of a chain hidden behind the other chains' turns) was measured
     // slower and removed.
-    int n_ctas = 0;
-    {
-        int g[RCMARL_MAX_JOBS];
-        plan_shares(n_jobs, cost, (n_rows_mb + 63) / 64, cpc, sm_count_cached(), true, g);
-        for (int j = 0; j < n_jobs; ++j) { P.cta_first[j] = (int16_t)n_ctas; n_ctas += g[j]; }
-        P.cta_first[n_jobs] = (int16_t)n_ctas;
-    }
+    const int n_ctas = plan_grid(n_jobs, cost, (n_rows_mb + 63) / 64, cpc, true, P.cta_first);
     P.n_chains = n_jobs; P.epochs = epochs; P.n_times = n_times; P.mb_times = mb_times; P.stride = maxn;
     const int64_t steps = rcmarl_minibatch_steps(epochs, n_times, mb_times);
     if ((uint64_t)seq_first + (uint64_t)steps >= 0xFFFFFFFFull) return RCMARL_ERR_ARG;
@@ -792,23 +751,12 @@ int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs
         const int e = NA == 5 ? launch_team<5>(P, n_list[g], gy, st) : launch_team<16>(P, n_list[g], gy, st);
         if (e) return e;
     }
-    if (any_sums) {
-        Q.partial = (const float*)ws;
-        Q.slots.step = n_jobs;                    // team_kernel writes its partials [y][job] interleaved
-        Q.slots.stride = TEAM_N;
-        for (int j = 0; j < n_jobs; ++j) { Q.slots.first[j] = j; Q.slots.count[j] = gy_of[j]; }
-        if (comm_bound()) {
-            ReduceCommParams C;
-            if (!comm_next(&C.comm, (int64_t)n_jobs * TEAM_N)) return RCMARL_ERR_ARG;
-            C.partial = Q.partial; C.slots = Q.slots; C.out_stride = TEAM_N; C.n_jobs = n_jobs; C.max_n = TEAM_N;
-            for (int j = 0; j < n_jobs; ++j) { C.sums[j] = Q.sums[j]; C.n[j] = Q.n[j]; }
-            if (launch_reduce_comm(C, st)) return RCMARL_ERR_CUDA;
-        } else {
-            reduce_kernel<<<dim3((TEAM_N + 31) / 32, n_jobs), 256, 0, st>>>(Q);
-        }
-        RC_CUDA(cudaGetLastError());
-    }
-    return RCMARL_OK;
+    if (!any_sums) return RCMARL_OK;
+    Q.partial = (const float*)ws;
+    Q.slots.step = n_jobs;                        // team_kernel writes its partials [y][job] interleaved
+    Q.slots.stride = TEAM_N;
+    for (int j = 0; j < n_jobs; ++j) { Q.slots.first[j] = j; Q.slots.count[j] = gy_of[j]; }
+    return reduce_partials(Q, n_jobs, TEAM_N, st);
 }
 
 int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs, int n_jobs, void* stream) {

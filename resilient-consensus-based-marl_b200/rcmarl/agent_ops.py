@@ -75,21 +75,13 @@ def fit_minibatch(w, x, target, n_agents, lr, epochs, mb_times, perms, n_envs=1)
     permutations; a mini-batch is mb_times time rows x n_envs environments (SURVEY Appendix C)."""
     rows, kind, xf = rows_for(x, n_agents)
     B, n = xf.shape[0], w.numel()
-    T = B // n_envs
     rows.n_envs = n_envs
     rows.time_idx = perms.data_ptr()
     sums = torch.empty(n + 1, dtype=torch.float32, device=w.device)
     loss = torch.zeros(1, dtype=torch.float32, device=w.device)
-    gj = ops.grad_job(w, target, sums, kind, time_idx=perms)
-    base = perms.data_ptr()
-    for e in range(epochs):
-        for b in range(0, T, mb_times):
-            cnt = min(mb_times, T - b)
-            rows.n_rows = cnt * n_envs
-            gj.time_idx = base + 4 * (e * T + b)
-            ops.grad(rows, [gj], L.LOSS_MSE)
-            ops.sgd_apply([ops.sgd_job(w, w, sums, n, lr * 2.0 / (cnt * n_envs), loss_out=loss if e == 0 else None,
-                                       loss_coef=1.0 / B, loss_accumulate=1)])
+    ops.minibatch_steps(rows, [ops.grad_job(w, target, sums, kind, time_idx=perms)],
+                        [ops.sgd_job(w, w, sums, n, 0.0, loss_out=loss, loss_coef=1.0 / B, loss_accumulate=1)],
+                        epochs, B // n_envs, mb_times, [lr])
     return float(loss.item())
 
 
@@ -134,22 +126,14 @@ def actor_fit_minibatch(actor_w, adam, s, a_local, delta, n_agents, mb_times, pe
     """actor.fit(s, a_local, sample_weight=TD, batch_size=200, epochs=1) (agents/adversarial_CAC_agents.py:41,116,224)."""
     sa = _sa_with_action(s, a_local, n_agents)
     B, n = sa.shape[0], actor_w.numel()
-    T = B // n_envs
     rows = ops.make_rows(sa, None, None, nets.kernel_agents(n_agents), time_idx=perm, n_envs=n_envs)
     adam.ensure(actor_w)
     sums = torch.empty(n + 1, dtype=torch.float32, device=actor_w.device)
     loss = torch.zeros(1, dtype=torch.float32, device=actor_w.device)
-    gj = ops.grad_job(actor_w, delta, sums, L.IN_S, action_agent=0, time_idx=perm)
-    base = perm.data_ptr()
-    for b in range(0, T, mb_times):
-        cnt = min(mb_times, T - b)
-        rows.n_rows = cnt * n_envs
-        gj.time_idx = base + 4 * b
-        adam.t += 1
-        ops.grad(rows, [gj], L.LOSS_CE)
-        ops.adam_apply([ops.adam_job(actor_w, adam.m, adam.v, sums, n, 1.0 / (cnt * n_envs),
-                                     ops.keras_adam_lr_t(adam.lr, adam.t), loss_out=loss, loss_coef=1.0 / B,
-                                     loss_accumulate=1)])
+    adam.t += ops.adam_minibatch_steps(
+        rows, [ops.grad_job(actor_w, delta, sums, L.IN_S, action_agent=0, time_idx=perm)],
+        [ops.adam_job(actor_w, adam.m, adam.v, sums, n, 0.0, 0.0, loss_out=loss, loss_coef=1.0 / B, loss_accumulate=1)],
+        B // n_envs, mb_times, [adam.lr], [adam.t])
     return float(loss.item())
 
 

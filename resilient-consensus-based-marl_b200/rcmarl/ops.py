@@ -99,13 +99,13 @@ def value_job(out, terms, add=None, add_stride=1, add_off=0, add_scale=1.0, n_ou
     return j
 
 
-def _arr(cls, jobs):
-    a = (cls * len(jobs))(*jobs)
-    return a
+def job_array(cls, jobs):
+    """ctypes array of the job structs `jobs` (a list or another array; the structs are copied)."""
+    return (cls * len(jobs))(*jobs)
 
 
 def values(rows, jobs):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.ValueJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.ValueJob, jobs)
     L.check(L.lib().rcmarl_values(C.byref(rows), a, len(a), _stream()), "rcmarl_values")
 
 
@@ -119,7 +119,7 @@ def grad_job(w, target, sums, kind, action_agent=0, target_stride=1, time_idx=No
 
 
 def grad(rows, jobs, loss_mode, ws=None):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.GradJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.GradJob, jobs)
     if ws is None:
         ws = workspace()
     L.check(L.lib().rcmarl_grad(C.byref(rows), a, len(a), loss_mode, ws.data_ptr(), ws.numel(), _stream()),
@@ -135,7 +135,7 @@ def sgd_job(dst, src, sums, n, coef, first=0, loss_out=None, loss_coef=0.0, loss
 
 
 def sgd_apply(jobs):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.SgdJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.SgdJob, jobs)
     L.check(L.lib().rcmarl_sgd_apply(a, len(a), _stream()), "rcmarl_sgd_apply")
 
 
@@ -153,8 +153,8 @@ class MinibatchCells:
 
 def minibatch_fit(rows, gjobs, sjobs, epochs, n_times, mb_times, lr, cells):
     """Whole mini-batch fit (all epochs, all steps, all chains) as ONE persistent kernel (csrc/minibatch_persist.cuh)."""
-    ga = gjobs if isinstance(gjobs, C.Array) else _arr(L.GradJob, gjobs)
-    sa = sjobs if isinstance(sjobs, C.Array) else _arr(L.SgdJob, sjobs)
+    ga = gjobs if isinstance(gjobs, C.Array) else job_array(L.GradJob, gjobs)
+    sa = sjobs if isinstance(sjobs, C.Array) else job_array(L.SgdJob, sjobs)
     steps = L.lib().rcmarl_minibatch_steps(epochs, n_times, mb_times)
     if cells.seq + steps >= 0xFFFF0000:                       # 32-bit sequence numbers: start over on clean cells
         cells.buf.zero_()
@@ -165,26 +165,56 @@ def minibatch_fit(rows, gjobs, sjobs, epochs, n_times, mb_times, lr, cells):
     cells.seq += steps
 
 
+def _fit_steps(rows, gjobs, ajobs, epochs, n_times, mb_times):
+    """The steps of a Keras fit(batch_size=mb_times rows, shuffle=True) over the grad jobs' permutation tables
+    (time_idx of job j: int32 [epochs][n_times] time rows; a mini-batch is those rows x rows.n_envs environments).
+    Before each step it points rows and every grad job at the step's rows and does the Keras loss bookkeeping on the
+    apply jobs ajobs; it yields the step's row count."""
+    tables = [g.time_idx for g in gjobs]
+    for e in range(epochs):
+        for b in range(0, n_times, mb_times):
+            rows.n_rows = min(mb_times, n_times - b) * rows.n_envs
+            for g, table in zip(gjobs, tables):
+                g.time_idx = table + 4 * (e * n_times + b)
+            for a in ajobs:
+                if b > 0:
+                    a.loss_accumulate = 1                   # the loss is summed over the steps of epoch 0 ...
+                if e == 1 and b == 0:
+                    a.loss_out = None                       # ... only (history['loss'][0])
+            yield rows.n_rows
+
+
 def minibatch_steps(rows, gjobs, sjobs, epochs, n_times, mb_times, lrs, world=1, allreduce=None, ws=None):
     """The fit of minibatch_fit (same job tables; lrs[j] = learning rate of chain j) as rcmarl_grad -> allreduce() ->
     rcmarl_sgd_apply per step: the data-parallel path without a peer-memory exchange, where allreduce() sums the
     chains' gradient sums over the `world` ranks in place."""
-    ga, sa = _arr(L.GradJob, list(gjobs)), _arr(L.SgdJob, list(sjobs))     # copies: the loop rewrites them
-    tables = [g.time_idx for g in ga]
-    for e in range(epochs):
-        for b in range(0, n_times, mb_times):
-            rows.n_rows = min(mb_times, n_times - b) * rows.n_envs
-            for j, (g, s) in enumerate(zip(ga, sa)):
-                g.time_idx = tables[j] + 4 * (e * n_times + b)
-                s.coef = lrs[j] * 2.0 / (rows.n_rows * world)
-                if b > 0:
-                    s.loss_accumulate = 1                   # the loss is summed over the steps of epoch 0 ...
-                if e == 1 and b == 0:
-                    s.loss_out = None                       # ... only (history['loss'][0])
-            grad(rows, ga, L.LOSS_MSE, ws)
-            if allreduce is not None:
-                allreduce()
-            sgd_apply(sa)
+    ga, sa = job_array(L.GradJob, gjobs), job_array(L.SgdJob, sjobs)     # copies: the loop rewrites them
+    for n_rows in _fit_steps(rows, ga, sa, epochs, n_times, mb_times):
+        for s, lr in zip(sa, lrs):
+            s.coef = lr * 2.0 / (n_rows * world)
+        grad(rows, ga, L.LOSS_MSE, ws)
+        if allreduce is not None:
+            allreduce()
+        sgd_apply(sa)
+
+
+def adam_minibatch_steps(rows, gjobs, ajobs, n_times, mb_times, lrs, ts, world=1, allreduce=None, ws=None):
+    """One epoch of actor.fit(batch_size=mb_times) with Keras Adam as rcmarl_grad (CE) -> allreduce() ->
+    rcmarl_adam_apply per step.  The time_idx of grad job j is a one-epoch permutation table [n_times]; lrs[j] is chain
+    j's learning rate and ts[j] the Adam steps it took before.  Returns the number of steps taken (the caller advances
+    its step counters by it)."""
+    ga, aa = job_array(L.GradJob, gjobs), job_array(L.AdamJob, ajobs)     # copies: the loop rewrites them
+    k = 0
+    for n_rows in _fit_steps(rows, ga, aa, 1, n_times, mb_times):
+        k += 1
+        for a, lr, t in zip(aa, lrs, ts):
+            a.grad_scale = 1.0 / (n_rows * world)
+            a.lr_t = keras_adam_lr_t(lr, t + k)
+        grad(rows, ga, L.LOSS_CE, ws)
+        if allreduce is not None:
+            allreduce()
+        adam_apply(aa)
+    return k
 
 
 def adam_job(theta, m, v, sums, n, grad_scale, lr_t, beta1=0.9, beta2=0.999, eps=1e-7, loss_out=None, loss_coef=0.0,
@@ -198,7 +228,7 @@ def adam_job(theta, m, v, sums, n, grad_scale, lr_t, beta1=0.9, beta2=0.999, eps
 
 
 def adam_apply(jobs):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.AdamJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.AdamJob, jobs)
     L.check(L.lib().rcmarl_adam_apply(a, len(a), _stream()), "rcmarl_adam_apply")
 
 
@@ -219,7 +249,7 @@ def team_job(w, kind, msgs=None, msg_stride=0, in_nodes=(), H=0, sums=None, agg_
 
 
 def team(rows, jobs, ws=None):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.TeamJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.TeamJob, jobs)
     if ws is None:
         ws = workspace()
     L.check(L.lib().rcmarl_team(C.byref(rows), a, len(a), ws.data_ptr(), ws.numel(), _stream()), "rcmarl_team")
@@ -235,7 +265,7 @@ def consensus_job(dst, msgs, msg_stride, n_hidden, in_nodes, H):
 
 
 def consensus_hidden(jobs):
-    a = jobs if isinstance(jobs, C.Array) else _arr(L.ConsensusJob, jobs)
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.ConsensusJob, jobs)
     L.check(L.lib().rcmarl_consensus_hidden(a, len(a), _stream()), "rcmarl_consensus_hidden")
 
 

@@ -116,9 +116,9 @@ class Trainer:
         self.loss_c = torch.zeros(NA, **f32)
         self.loss_t = torch.zeros(NA, **f32)
         self.loss_a = torch.zeros(NA, **f32)
-        self.ws = ops.workspace(L.MAX_JOBS, self.PT if NA == 5 else L.param_count(48, 1))
+        self.ws = ops.workspace(L.MAX_JOBS, self.PT)      # the TR net (3 * NA inputs) is the largest
         # scratch of the persistent mini-batch kernel (rcmarl_minibatch_fit)
-        self.mb_cells = ops.MinibatchCells(L.MAX_JOBS, self.PT if NA == 5 else L.param_count(48, 1), self.dev)
+        self.mb_cells = ops.MinibatchCells(L.MAX_JOBS, self.PT, self.dev)
         self.launches = 0                                 # kernels launched by this engine (bench: gpu_launches)
         self.profile = None                               # bench.py: {"fit_grad": [(start_evt, end_evt), ...], ...}
         self.h2d_bytes = 4 * sum(x.numel() for x in (self.actor, self.critic, self.tr, self.critic_local))
@@ -284,7 +284,7 @@ class Trainer:
                                              add=r_col[i], add_stride=NA))                       # adversarial:148-149
                 td_jobs.append(ops.value_job(self.tdt[i], [(self.critic[i], L.IN_NS, self.gamma)],
                                              add=self.neg_r_coop, add_stride=1))                 # adversarial:131-132
-        td_arr = (L.ValueJob * len(td_jobs))(*td_jobs) if td_jobs else None
+        td_arr = ops.job_array(L.ValueJob, td_jobs)
 
         fit_first, fit_next, fit_apply_first, fit_apply_next = [], [], [], []
         for n, i in enumerate(coop):
@@ -302,9 +302,8 @@ class Trainer:
                                   loss_coef=1.0 / Bg)]
                 (fit_first if first else fit_next).extend(gj)
                 (fit_apply_first if first else fit_apply_next).extend(aj)
-        arr = lambda cls, js: (cls * len(js))(*js) if js else None
-        fit_first, fit_next = arr(L.GradJob, fit_first), arr(L.GradJob, fit_next)
-        fit_apply_first, fit_apply_next = arr(L.SgdJob, fit_apply_first), arr(L.SgdJob, fit_apply_next)
+        fit_first, fit_next = ops.job_array(L.GradJob, fit_first), ops.job_array(L.GradJob, fit_next)
+        fit_apply_first, fit_apply_next = ops.job_array(L.SgdJob, fit_apply_first), ops.job_array(L.SgdJob, fit_apply_next)
 
         # mini-batch chains of the adversaries (adversarial:133,150,163,239,251), node order = permutation order
         chains = []                                       # (weights in place, kind, target, stride, loss slot, lr)
@@ -328,11 +327,12 @@ class Trainer:
             team_jobs.append(ops.team_job(self.tr[i], L.IN_SA, self.msg_t, self.PT, nodes, self.H[i], sums=self.sums_team[2 * n + 1]))
             team_apply.append(ops.sgd_job(self.critic[i], self.critic[i], self.sums_team[2 * n], self.PC, -1.0 / Bg, first=self.PC - 21))
             team_apply.append(ops.sgd_job(self.tr[i], self.tr[i], self.sums_team[2 * n + 1], self.PT, -1.0 / Bg, first=self.PT - 21))
-        cons_jobs, team_jobs, team_apply = arr(L.ConsensusJob, cons_jobs), arr(L.TeamJob, team_jobs), arr(L.SgdJob, team_apply)
+        cons_jobs, team_jobs = ops.job_array(L.ConsensusJob, cons_jobs), ops.job_array(L.TeamJob, team_jobs)
+        team_apply = ops.job_array(L.SgdJob, team_apply)
 
         for _epoch in range(self.n_epochs):                                # :100
             # ---------------- I) local updates (:105-121)
-            if td_arr is not None:
+            if td_jobs:
                 ops.values(rows_all, td_arr)
                 self.launches += 1
             if coop:
@@ -369,7 +369,7 @@ class Trainer:
                 cw = self.critic_local[i] if lab[i] == MALICIOUS else self.critic[i]
                 d_jobs.append(ops.value_job(self.delta[i], [(cw, L.IN_NS, self.gamma), (cw, L.IN_S, -1.0)],
                                             add=r_col[i], add_stride=NA))
-        ops.values(rows_act, arr(L.ValueJob, d_jobs))
+        ops.values(rows_act, ops.job_array(L.ValueJob, d_jobs))
         self.launches += 1
         Bag = Ta * N * self.world
         if coop:
@@ -380,9 +380,9 @@ class Trainer:
                 aj.append(ops.adam_job(self.actor[i], self.adam_m[i], self.adam_v[i], self.sums_actor[n], self.PA, 1.0 / Bag,
                                        ops.keras_adam_lr_t(self.slow_lr[i], self.adam_t[i]), loss_out=self.loss_a[i:i + 1],
                                        loss_coef=1.0 / Bag))
-            ops.grad(rows_act, arr(L.GradJob, gj), L.LOSS_CE, self.ws)
+            ops.grad(rows_act, ops.job_array(L.GradJob, gj), L.LOSS_CE, self.ws)
             self._allreduce(self.sums_actor[:len(coop)])
-            ops.adam_apply(arr(L.AdamJob, aj))
+            ops.adam_apply(ops.job_array(L.AdamJob, aj))
             self.launches += 3
         adv = [i for i in range(self.n_real) if lab[i] != COOP]
         if adv:
@@ -423,31 +423,20 @@ class Trainer:
 
     def _minibatch_adam(self, adv, T, Ta, a0):
         """actor.fit(batch_size=200, epochs=1) of the adversaries (adversarial:41,116,224)."""
-        N = self.N
         perms = torch.stack([self._perm(Ta) for _ in adv]).to(self.dev)    # [A, Ta], indices inside the actor window
         self.h2d_bytes += 4 * perms.numel()
-        base = perms.data_ptr()
-        nb = (Ta + self.actor_mb_times - 1) // self.actor_mb_times
-        rows = self._rows(a0, 0, perms)
-        gj = []
+        gj, aj = [], []
         for n, i in enumerate(adv):
-            gj.append(ops.grad_job(self.actor[i], self.delta[i], self.sums_actor[n], L.IN_S, action_agent=i, time_idx=perms))
+            gj.append(ops.grad_job(self.actor[i], self.delta[i], self.sums_actor[n], L.IN_S, action_agent=i, time_idx=perms[n]))
+            aj.append(ops.adam_job(self.actor[i], self.adam_m[i], self.adam_v[i], self.sums_actor[n], self.PA, 0.0, 0.0,
+                                   loss_out=self.loss_a[i:i + 1], loss_coef=1.0 / (Ta * self.N * self.world), loss_accumulate=1))
             self.loss_a[i:i + 1].zero_()
-        gj = (L.GradJob * len(gj))(*gj)
-        for b in range(nb):
-            cnt = min(self.actor_mb_times, Ta - b * self.actor_mb_times)
-            rows.n_rows = cnt * N
-            aj = []
-            for n, i in enumerate(adv):
-                gj[n].time_idx = base + 4 * (n * Ta + b * self.actor_mb_times)
-                self.adam_t[i] += 1
-                aj.append(ops.adam_job(self.actor[i], self.adam_m[i], self.adam_v[i], self.sums_actor[n], self.PA,
-                                       1.0 / (cnt * N * self.world), ops.keras_adam_lr_t(self.slow_lr[i], self.adam_t[i]),
-                                       loss_out=self.loss_a[i:i + 1], loss_coef=1.0 / (Ta * N * self.world), loss_accumulate=1))
-            ops.grad(rows, gj, L.LOSS_CE, self.ws)
-            self._allreduce(self.sums_actor[:len(adv)])
-            ops.adam_apply(aj)
-            self.launches += 3
+        steps = ops.adam_minibatch_steps(self._rows(a0, 0, perms), gj, aj, Ta, self.actor_mb_times,
+                                         [self.slow_lr[i] for i in adv], [self.adam_t[i] for i in adv], self.world,
+                                         lambda: self._allreduce(self.sums_actor[:len(adv)]), self.ws)
+        for i in adv:
+            self.adam_t[i] += steps
+        self.launches += 3 * steps
 
     # ------------------------------------------------------------------ checkpoint / resume
     def state_dict(self, include_buffer=True):

@@ -205,18 +205,13 @@ class Sequential(Model):
     # -- execution ----------------------------------------------------------
     def _forward(self, x):
         import torch
-        from rcmarl import ops, _lib as L
+        from rcmarl import agent_ops, ops
         x = ops.dev_f32(x)
-        B = x.shape[0]
-        x = x.reshape(B, -1)
+        x = x.reshape(x.shape[0], -1)
         if x.shape[1] != self.d_in:
             raise ValueError(f"expected input with {self.d_in} features per row, got {x.shape[1]}")
-        out = torch.empty(B, self.n_out, dtype=torch.float32, device=x.device)
-        x = nets.pad_agent_slots(x, self.n_agents, self.n_kernel)
-        if self.n_feat == 3:
-            rows, kind = ops.make_rows(x, None, None, self.n_kernel), L.IN_SA
-        else:
-            rows, kind = ops.make_rows(None, x, None, self.n_kernel), L.IN_NS
+        rows, kind, x = agent_ops.rows_for(x, self.n_agents)
+        out = torch.empty(x.shape[0], self.n_out, dtype=torch.float32, device=x.device)
         ops.values(rows, [ops.value_job(out, [(self.flat, kind, 1.0)], n_out=self.n_out, softmax=int(self.softmax))])
         return out
 
