@@ -1,5 +1,8 @@
-"""Helpers shared by the kernel parity tests (test_kernels_gpu.py, test_kernel_shapes_gpu.py): the library handle,
-seeded synthetic buffer rows, random networks, host -> device copies and the tolerance check."""
+"""Helpers shared by the kernel parity tests (test_kernels_gpu.py, test_kernel_shapes_gpu.py, test_minibatch_fit_gpu.py):
+the library handle, the library's own CTA plan, seeded synthetic buffer rows, random networks, host -> device copies and
+the tolerance check."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
@@ -18,6 +21,17 @@ def load_kernels():
     k.ops, k.nets, k.L = ops, nets, _lib
     k.dev = torch.device("cuda:0")
     return k
+
+
+def grad_ctas(K, NA, kinds, loss, n_rows, sms, balanced=False):
+    """CTAs per job of a one-wave grid over n_rows rows on sms SMs, from the library's own plan: equal shares as
+    rcmarl_grad launches them, or cost-balanced shares (balanced=True) as rcmarl_minibatch_fit launches its chains
+    (n_rows = one mini-batch)."""
+    n = len(kinds)
+    out = (C.c_int32 * n)()
+    K.L.check(K.L.lib().rcmarl_grad_grid_plan(NA, (C.c_int32 * n)(*kinds), n, loss, n_rows, int(balanced), sms, out),
+              "rcmarl_grad_grid_plan")
+    return list(out)
 
 
 def synth(rs, B, NA=5, nrow=5):

@@ -1,7 +1,9 @@
 """Oracle parity AT THE BENCHMARKED SHAPES (one GPU):
- (a) a Malicious + cooperative update round through rcmarl.trainer.Trainer with n_envs in {64, 128}: gathered row mode
-     with n_envs % 64 == 0, i.e. the bulk-copy (TMA) staging branch of grad_kernel and the persistent mini-batch kernel
-     (rcmarl_minibatch_fit) that the C2 benchmark spends half of its step in -- against the fp64 oracle;
+ (a) a Malicious + cooperative update round through rcmarl.trainer.Trainer with n_envs in {64, 128, 4096}: gathered row
+     mode with n_envs % 64 == 0, i.e. the bulk-copy (TMA) staging branch of grad_kernel and the persistent mini-batch
+     kernel (rcmarl_minibatch_fit) that the C2 benchmark spends half of its step in, at 4096 on the C2 grid (more than 32
+     CTAs per chain); and the mixed team [Cooperative, Malicious, Greedy, Cooperative, Malicious] at n_envs = 1024, whose
+     8 chains share one launch -- against the fp64 oracle;
  (b) rcmarl_grad over 4.1 M buffer rows (the C2 row count of one block) against NumPy fp64 sums (chunked);
  (c) rcmarl_clip_mean on the C5 tensor (64 x 1 048 576), H in {0, 1, 2, 4}, against oracle.resilient_aggregation;
  (d) the reference's own train_RPBCAC run with a Greedy and a Faulty agent and common_reward=True
@@ -44,19 +46,26 @@ def synth(rs, B, NA=5, nrow=5):
 
 
 # ------------------------------------------------------------------------------------------ (a)
-@pytest.mark.parametrize("N", [64, 128])
-def test_malicious_round_at_staged_gather_shapes_matches_oracle(N):
+ONE_MALICIOUS = ['Cooperative'] * 4 + ['Malicious']
+MIXED = ['Cooperative', 'Malicious', 'Greedy', 'Cooperative', 'Malicious']
+
+
+@pytest.mark.parametrize("N,labels", [pytest.param(64, ONE_MALICIOUS, id="64"), pytest.param(128, ONE_MALICIOUS, id="128"),
+                                      pytest.param(4096, ONE_MALICIOUS, id="4096"),
+                                      pytest.param(1024, MIXED, id="1024-mixed")])
+def test_malicious_round_at_staged_gather_shapes_matches_oracle(N, labels):
     need_gpu()
     from rcmarl.trainer import Trainer
     rs = np.random.RandomState(N)
     T1, gamma = 40, 0.9                          # 40 time rows: mini-batches of 32 and 8 time rows x N environments
-    labels = ['Cooperative'] * 4 + ['Malicious']
     w, desired, _ = pretrained()
     agents = []
     for i, l in enumerate(labels):
         if l == 'Malicious':
-            agents.append(O.MaliciousOracleAgent(w[i][0], w[i][1], w[i][2], 0.002, 0.01, gamma, critic_local_w=w[i][3],
-                                                 dtype=np.float64))
+            agents.append(O.MaliciousOracleAgent(w[i][0], w[i][1], w[i][2], 0.002, 0.01, gamma,
+                                                 critic_local_w=w[i][3] if len(w[i]) > 3 else None, dtype=np.float64))
+        elif l == 'Greedy':
+            agents.append(O.GreedyOracleAgent(w[i][0], w[i][1], w[i][2], 0.002, 0.01, gamma, dtype=np.float64))
         else:
             agents.append(O.RPBCACOracleAgent(w[i][0], w[i][1], w[i][2], 0.002, 0.01, gamma, H=1, dtype=np.float64))
     rs_perm = np.random.RandomState(N + 1)

@@ -8,8 +8,6 @@ rtol 1e-4 with an atol floor growing with sqrt(B); forward values rtol 1e-5 / at
 terms and for the clipped mean of neighbour estimates, as in test_kernels_gpu.py); weights after a projection or
 consensus step rtol 1e-4 / atol 1e-6; discrete outputs exact.
 """
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -17,7 +15,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from golden_util import pretrained                     # noqa: E402
-from kernel_util import close, load_kernels, rand_net, synth, to_dev   # noqa: E402
+from kernel_util import close, grad_ctas, load_kernels, rand_net, synth, to_dev   # noqa: E402
 from oracle import rpbcac_oracle as O                  # noqa: E402  (checker only)
 
 f64 = np.float64
@@ -96,15 +94,6 @@ def oracle_ce_sums(w, X, idx, act, d):
 
 
 # ---------------------------------------------------------------------------------------------------------- grad helpers
-def grad_ctas(K, NA, kinds, loss, n_rows, sms):
-    """CTAs per job of rcmarl_grad's one-wave grid (equal shares), from the library's own plan."""
-    n = len(kinds)
-    out = (C.c_int32 * n)()
-    K.L.check(K.L.lib().rcmarl_grad_grid_plan(NA, (C.c_int32 * n)(*kinds), n, loss, n_rows, 0, sms, out),
-              "rcmarl_grad_grid_plan")
-    return list(out)
-
-
 def steady_rows(K, NA, kinds, loss, sms):
     """Rows for which every warp of every job sweeps at least 3 full 64-row chunks, plus a ragged tail of TAIL rows."""
     full = 3 * max(1, sms // len(kinds)) * MAX_GRAD_WARPS

@@ -12,7 +12,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 from golden_util import pretrained                     # noqa: E402
-from kernel_util import close, load_kernels, rand_net, synth, to_dev   # noqa: E402
+from kernel_util import close, grad_ctas, load_kernels, rand_net, synth, to_dev   # noqa: E402
 from oracle import rpbcac_oracle as O                  # noqa: E402  (checker only)
 
 
@@ -418,13 +418,22 @@ def test_env_step_matches_reference_fixture(K):
 
 
 # ------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("NA,nrow,N,T", [(5, 5, 64, 40), (5, 5, 24, 37), (16, 10, 64, 33), (5, 5, 1, 96)])
+# C2 width: one mini-batch is 32 time rows x 4096 (or 4000) environments, as in the benchmark's malicious-agent fit.
+MB_FULL_WIDTH = [(5, 5, 4096, 70), (5, 5, 4000, 70), (16, 10, 4096, 70)]
+
+
+@pytest.mark.parametrize("NA,nrow,N,T", [(5, 5, 64, 40), (5, 5, 24, 37), (16, 10, 64, 33), (5, 5, 1, 96)] + MB_FULL_WIDTH)
 def test_minibatch_fit_persistent_kernel_matches_oracle_and_step_loop(K, NA, nrow, N, T):
     """rcmarl_minibatch_fit (ONE persistent kernel: parameters resident in shared memory, cross-CTA reduction through
     {value, sequence} cells) against (a) the fp64 oracle's fit_minibatch with the same injected permutations
     (agents/adversarial_CAC_agents.py:133,150,163: fit(batch_size=32, epochs=E), Appendix C batching) and (b) the
     per-step loop ops.minibatch_steps (rcmarl_grad -> rcmarl_sgd_apply, the data-parallel NCCL path) at world 1;
-    and bitwise reproducibility of two runs."""
+    and bitwise reproducibility of two runs.  Each run makes two calls on the same cells, the second with half the step
+    size and its own permutations, so the second call's weights and its share of the accumulated loss show whether it
+    read any of the first call's cells.
+
+    The full-width cases run the C2 grid: T = 70 gives mini-batches of 32, 32 and 6 time rows, N = 4000 is not a
+    multiple of 64 (per-lane gathered loads, chunks straddling time rows), NA = 16 the 16-agent instantiation."""
     rs = np.random.RandomState(NA + N + T)
     E, mb, lr = 3, 32, 0.01
     B = N * T
@@ -434,42 +443,56 @@ def test_minibatch_fit_persistent_kernel_matches_oracle_and_step_loop(K, NA, nro
     nets0 = [rand_net(rs, 3 * NA if k == K.L.IN_SA else 2 * NA, 1) for k in kinds]
     tgts = [rs.randn(B).astype(np.float32) for _ in kinds]
     perms = np.stack([np.stack([rs.permutation(T) for _ in range(E)]) for _ in kinds]).astype(np.int32)     # [C, E, T]
+    perms2 = np.stack([np.stack([rs.permutation(T) for _ in range(E)]) for _ in kinds]).astype(np.int32)    # second call
+    calls = ((perms, lr), (perms2, lr / 2))
+    if (NA, nrow, N, T) in MB_FULL_WIDTH:
+        # More than 32 CTAs per chain: the level-1 gather runs S = 32 lanes per entry, each adding two or more CTAs,
+        # and each warp owns one entry per pass.  At 132 SMs (NA = 5) the plan is 43 / 46 / 43 CTAs and the last CTA of
+        # each chain owns an empty parameter slice (43 * 16 > 662 and 46 * 17 > 762 sums per chain).
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        ctas = grad_ctas(K, NA, kinds, K.L.LOSS_MSE, mb * N, sms, balanced=True)
+        assert min(ctas) > 32, (sms, ctas)
     dsa, dns, dr = to_dev(K, sa.reshape(B, -1), ns.reshape(B, -1), r.reshape(B, -1))
-    dperm = to_dev(K, perms)[0]
     dt = to_dev(K, *tgts)
 
     def run(persistent):
         ws = [to_dev(K, K.nets.pack(w))[0] for w in nets0]
         loss = torch.zeros(len(kinds), device=K.dev)
-        gj, aj = [], []
-        for c, kind in enumerate(kinds):
-            n = ws[c].numel()
-            sums = torch.zeros(n + 1, device=K.dev)
-            g = K.ops.grad_job(ws[c], dt[c], sums, kind, time_idx=dperm)
-            g.time_idx = dperm.data_ptr() + 4 * c * E * T
-            gj.append(g)
-            aj.append(K.ops.sgd_job(ws[c], ws[c], sums, n, 0.0, loss_out=loss[c:c + 1], loss_coef=1.0 / B, loss_accumulate=1))
-        rows = K.ops.make_rows(dsa, dns, dr, NA, 0, 0, dperm, N)
-        if persistent:
-            cells = K.ops.MinibatchCells(len(kinds), K.L.param_count(3 * NA, 1))
-            K.ops.minibatch_fit(rows, gj, aj, E, T, mb, lr, cells)
-            K.ops.minibatch_fit(rows, gj, aj, E, T, mb, 0.0 * lr + 1e-30, cells)     # second call on the same cells: a no-op step size
-        else:
-            K.ops.minibatch_steps(rows, gj, aj, E, T, mb, [lr] * len(kinds))
-        torch.cuda.synchronize()
-        return [w.cpu().numpy() for w in ws], loss.cpu().numpy()
+        cells = K.ops.MinibatchCells(len(kinds), K.L.param_count(3 * NA, 1))
+        after = []
+        for table, lr_k in calls:
+            dperm = to_dev(K, table)[0]
+            gj, aj = [], []
+            for c, kind in enumerate(kinds):
+                n = ws[c].numel()
+                sums = torch.zeros(n + 1, device=K.dev)
+                g = K.ops.grad_job(ws[c], dt[c], sums, kind, time_idx=dperm)
+                g.time_idx = dperm.data_ptr() + 4 * c * E * T
+                gj.append(g)
+                aj.append(K.ops.sgd_job(ws[c], ws[c], sums, n, 0.0, loss_out=loss[c:c + 1], loss_coef=1.0 / B,
+                                        loss_accumulate=1))
+            rows = K.ops.make_rows(dsa, dns, dr, NA, 0, 0, dperm, N)
+            if persistent:
+                K.ops.minibatch_fit(rows, gj, aj, E, T, mb, lr_k, cells)
+            else:
+                K.ops.minibatch_steps(rows, gj, aj, E, T, mb, [lr_k] * len(kinds))
+            torch.cuda.synchronize()
+            after.append([w.cpu().numpy() for w in ws])
+        return after, loss.cpu().numpy()
     w_p, loss_p = run(True)
     w_p2, _ = run(True)
     w_c, loss_c = run(False)
     for c, kind in enumerate(kinds):
-        assert np.array_equal(w_p[c], w_p2[c])                                 # fixed-order reductions
         x = O.flatten_rows(sa if kind == K.L.IN_SA else s, np.float64)
-        rp = [O.expand_time_perm(perms[c, e], N) for e in range(E)]
-        w64, l64 = O.fit_minibatch(O.cast_weights(nets0[c], np.float64), x, tgts[c].astype(np.float64).reshape(-1, 1), lr, E,
-                                   mb * N, rp)
-        want = K.nets.pack(w64)
-        np.testing.assert_allclose(w_p[c], want, rtol=2e-4, atol=2e-6)
-        np.testing.assert_allclose(w_p[c], w_c[c], rtol=1e-5, atol=1e-6)
-        # the second (tiny step size) call accumulated its own epoch-0 loss on top: compare the first call's share only
-        np.testing.assert_allclose(loss_c[c], l64, rtol=1e-4)
-    assert np.all(loss_p > loss_c * 1.05)                                      # two calls accumulated two epoch-0 losses
+        y = tgts[c].astype(np.float64).reshape(-1, 1)
+        w64, want_loss = O.cast_weights(nets0[c], np.float64), 0.0
+        for k, (table, lr_k) in enumerate(calls):
+            w64, l64 = O.fit_minibatch(w64, x, y, lr_k, E, mb * N, [O.expand_time_perm(table[c, e], N) for e in range(E)])
+            want_loss += float(l64)
+            msg = f"chain {c}, after call {k + 1}"
+            assert np.array_equal(w_p[k][c], w_p2[k][c]), msg                 # fixed-order reductions, no races
+            np.testing.assert_allclose(w_p[k][c], K.nets.pack(w64), rtol=2e-4, atol=2e-6, err_msg=msg)
+            np.testing.assert_allclose(w_p[k][c], w_c[k][c], rtol=1e-5, atol=1e-6, err_msg=msg)
+        # loss_accumulate = 1: the two calls' epoch-0 losses add up
+        np.testing.assert_allclose(loss_p[c], want_loss, rtol=1e-4)
+        np.testing.assert_allclose(loss_c[c], want_loss, rtol=1e-4)
