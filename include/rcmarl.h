@@ -93,11 +93,24 @@ int rcmarl_grad_grid_plan(int n_agents, const int32_t* kinds_host, int n_jobs, i
 int rcmarl_clip_mean(const float* vals, int n, int64_t P, int64_t row_stride, int H,
                      float* out, void* stream);
 
+/* Resilient aggregation rule of rcmarl_consensus_hidden and rcmarl_team, applied per coordinate to the n = n_in values
+ * v[0..n-1] of the in-neighbours, own = v[0].  rank(k) = #{m : v[m] < v[k] or (v[m] == v[k] and m < k)}.
+ *   CLIP  the reference's clipped mean: every v[k] clipped to [min(v_(H), own), max(v_(n-H-1), own)], mean of all n
+ *         (v_(r) = the value of rank r);                                                          0 <= H < n
+ *   TRIM  trimmed mean: mean of the v[k] with H <= rank(k) <= n-H-1 (at H = (n-1)/2, the median);  0 <= H, 2H < n
+ *   WMSR  W-MSR (LeBlanc et al., IEEE JSAC 2013): a = #{v > own}, b = #{v < own}; the v[k] with
+ *         rank(k) >= n - min(H, a) or rank(k) < min(H, b) are dropped, mean of the rest.  Own and every value equal
+ *         to it are kept;                                                                         0 <= H < n
+ * TRIM and WMSR add the kept values in index order, so a dropped value (1e30, +-inf) never enters the result.
+ * NaN inputs are not supported by any rule. */
+typedef enum { RCMARL_AGG_CLIP = 0, RCMARL_AGG_TRIM = 1, RCMARL_AGG_WMSR = 2 } rcmarl_agg_rule;
+
 /* Hidden-layer parameter consensus for many (agent, net) pairs in one launch:
- * dst[j][0:n_hidden] = clip_mean over k of msgs[in_nodes[j][k]][0:n_hidden]  (own = k 0).
+ * dst[j][0:n_hidden] = aggregate (rule) over k of msgs[in_nodes[j][k]][0:n_hidden]  (own = k 0).
  * Replaces resilient_consensus_critic_hidden / _TR_hidden
  * (agents/resilient_CAC_agents.py:142-166) incl. the neighbour gather at
- * training/train_agents.py:129-130.  The output layer of dst is left untouched (:153). */
+ * training/train_agents.py:129-130.  The output layer of dst is left untouched (:153).
+ * An unknown rule or an H the rule does not allow is refused (RCMARL_ERR_ARG) before anything is launched. */
 typedef struct {
     float* dst;                 /* the agent's own network (packed) */
     const float* msgs;          /* base of the message stack [n_agents][msg_stride] */
@@ -106,6 +119,7 @@ typedef struct {
     int32_t n_in;
     int32_t H;
     int32_t in_nodes[RCMARL_MAX_NEIGHBOURS];
+    int32_t rule;               /* rcmarl_agg_rule; 0 (a zero-initialised job) is CLIP */
 } rcmarl_consensus_job;
 int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs_host, int n_jobs, void* stream);
 
@@ -218,13 +232,13 @@ int rcmarl_adam_apply(const rcmarl_adam_job* jobs_host, int n_jobs, void* stream
 
 /* ---------------------------------------------------------------------------
  * K5 + K6 fused.  Per row: phi = features(x) with the agent's (aggregated) hidden layers;
- * est_k = phi . W3_k + b3_k for each neighbour head k (own first); agg = clip_mean_k(est, H);
+ * est_k = phi . W3_k + b3_k for each neighbour head k (own first); agg = aggregate_k(est, H, rule);
  * projection step on the agent's own output layer:
  *   sums[0:21] = sum_rows (agg - (phi.W3_own + b3_own)) * [phi;1] / (||phi||^2 + 1)
  * so that theta_out += sums / B reproduces train_on_batch with sample weights
  * 1/(2 lr (||phi||^2+1)).  Replaces resilient_consensus_critic/_TR and
  * critic_update_team/TR_update_team (agents/resilient_CAC_agents.py:60-84,168-206).
- * agg_out (optional) stores agg per absolute row; agg_in (optional) supplies it instead. */
+ * agg_out (optional) stores agg per absolute row; agg_in (optional) supplies it instead (msgs, n_in, H, rule unused). */
 typedef struct {
     const float* w;             /* agent's network: aggregated hidden + current own head */
     const float* msgs;          /* message stack base (heads are read at the W3/b3 offsets) */
@@ -236,6 +250,7 @@ typedef struct {
     int32_t n_in;
     int32_t H;
     int32_t in_nodes[RCMARL_MAX_NEIGHBOURS];
+    int32_t rule;               /* rcmarl_agg_rule; 0 (a zero-initialised job) is CLIP */
 } rcmarl_team_job;
 int rcmarl_team(const rcmarl_rows* rows_host, const rcmarl_team_job* jobs_host, int n_jobs,
                 void* ws, int64_t ws_bytes, void* stream);

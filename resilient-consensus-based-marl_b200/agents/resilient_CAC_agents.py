@@ -3,7 +3,8 @@ mfigura/Resilient-consensus-based-MARL), executed by the sm_90a kernels of librc
 
 Same constructor and method names, argument meaning and mutation conventions as the reference (SURVEY.md 8b):
   *_update_local            return (message copy, loss) and leave the agent's own networks untouched (:113,120)
-  resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166)
+  resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166), or
+                                 their trimmed / W-MSR mean with aggregation="trim" / "wmsr"
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
@@ -13,17 +14,22 @@ import torch
 
 from tensorflow import keras
 from tensorflow.keras import Tensor
+from rcmarl import _lib as L
 from rcmarl import agent_ops as A
 from rcmarl import nets, ops
 
 
 class RPBCAC_agent():
-    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0):
+    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip"):
         self.actor = actor
         self.critic = critic
         self.TR = team_reward
         self.gamma = gamma
         self.H = H
+        # resilient aggregation rule of every consensus step: "clip" (the reference's), "trim" or "wmsr"
+        # (include/rcmarl.h, rcmarl_agg_rule)
+        L.agg_rule(aggregation)
+        self.aggregation = aggregation
         self.n_actions = self.actor.output_shape[1]
         self.fast_lr = fast_lr
         self.slow_lr = slow_lr
@@ -36,7 +42,14 @@ class RPBCAC_agent():
     def _resilient_aggregation(self, values_innodes):
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
-        out = ops.clip_mean(v.reshape(v.shape[0], -1), self.H)
+        v = v.reshape(v.shape[0], -1)
+        if L.agg_rule(self.aggregation) == L.AGG_CLIP:
+            out = ops.clip_mean(v, self.H)
+        else:                         # the other rules: one consensus job over all P coordinates of the n rows
+            L.check_aggregation(self.aggregation, self.H, v.shape[0])
+            out = torch.empty(v.shape[1], dtype=torch.float32, device=v.device)
+            ops.consensus_hidden([ops.consensus_job(out, v, v.shape[1], v.shape[1], list(range(v.shape[0])), self.H,
+                                                    self.aggregation)])
         return Tensor(out.reshape(shape))
 
     # ------------------------------------------------------------------ projection step (:60-84)
@@ -77,7 +90,7 @@ class RPBCAC_agent():
         dev = model.flat.device
         stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
         ops.consensus_hidden([ops.consensus_job(model.flat, stack, stack.shape[1], nets.n_hidden_params(model.d_in_k),
-                                                list(range(len(msgs_innodes))), self.H)])
+                                                list(range(len(msgs_innodes))), self.H, self.aggregation)])
 
     def resilient_consensus_critic_hidden(self, critic_weights_innodes):
         self._hidden(self.critic, critic_weights_innodes)
@@ -92,7 +105,7 @@ class RPBCAC_agent():
         stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
         agg = torch.empty(xf.shape[0], dtype=torch.float32, device=dev)
         ops.team(rows, [ops.team_job(model.flat, kind, stack, stack.shape[1], list(range(len(msgs_innodes))), self.H,
-                                     agg_out=agg)])
+                                     agg_out=agg, rule=self.aggregation)])
         return Tensor(agg.reshape(-1, 1))
 
     def resilient_consensus_critic(self, s, critic_weights_innodes):

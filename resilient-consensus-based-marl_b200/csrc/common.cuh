@@ -169,6 +169,39 @@ __device__ __forceinline__ float clip_mean_small(const float (&v)[MAXN], int n, 
     return s / (float)n;
 }
 
+// Resilient aggregation of n values under rule (rcmarl_agg_rule, include/rcmarl.h), own = v[0].  CLIP is
+// clip_mean_small; TRIM and WMSR keep the ranks lo..hi of the same tie-broken rank count and add the kept values in
+// index order, so that a dropped outlier (1e30, +-inf) never touches the sum.  The branch is uniform per job.
+template <int MAXN>
+__device__ __forceinline__ float resilient_mean_small(const float (&v)[MAXN], int n, int H, int rule) {
+    if (rule == RCMARL_AGG_CLIP) return clip_mean_small<MAXN>(v, n, H);
+    int lo = H, hi = n - H - 1;
+    if (rule == RCMARL_AGG_WMSR) {            // at most H strictly above own and at most H strictly below it
+        int above = 0, below = 0;
+#pragma unroll
+        for (int k = 1; k < MAXN; ++k) {
+            if (k < n) {
+                above += v[k] > v[0] ? 1 : 0;
+                below += v[k] < v[0] ? 1 : 0;
+            }
+        }
+        lo = min(H, below);
+        hi = n - 1 - min(H, above);
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXN; ++k) {
+        if (k < n) {
+            int rank = 0;
+#pragma unroll
+            for (int m = 0; m < MAXN; ++m)
+                if (m < n) rank += (v[m] < v[k] || (v[m] == v[k] && m < k)) ? 1 : 0;
+            if (rank >= lo && rank <= hi) s += v[k];
+        }
+    }
+    return s / (float)(hi - lo + 1);
+}
+
 // A pair of fp32 values (two adjacent hidden units, or two accumulators) updated together.  Hopper has no packed fp32
 // FMA, so a pair operation is two IEEE fp32 FMAs (FFMA); the values are the same as one packed operation would give.
 typedef float2 f2;

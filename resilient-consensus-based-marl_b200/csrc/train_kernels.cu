@@ -265,8 +265,8 @@ __device__ __forceinline__ void team_body(const TeamParams& P, const rcmarl_team
                     est[1][k] = s1;
                 }
             }
-            agg[0] = clip_mean_small<MAXN>(est[0], job.n_in, job.H);
-            agg[1] = clip_mean_small<MAXN>(est[1], job.n_in, job.H);
+            agg[0] = resilient_mean_small<MAXN>(est[0], job.n_in, job.H, job.rule);
+            agg[1] = resilient_mean_small<MAXN>(est[1], job.n_in, job.H, job.rule);
         }
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(256) consensus_hidden_kernel(const __grid_cons
 #pragma unroll
     for (int k = 0; k < RCMARL_MAX_NEIGHBOURS; ++k)
         v[k] = k < job.n_in ? __ldg(job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride + i) : 0.f;
-    job.dst[i] = clip_mean_small<RCMARL_MAX_NEIGHBOURS>(v, job.n_in, job.H);
+    job.dst[i] = resilient_mean_small<RCMARL_MAX_NEIGHBOURS>(v, job.n_in, job.H, job.rule);
 }
 
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
@@ -703,6 +703,11 @@ int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, 
     return NA == 5 ? launch_mb_persist<5>(P, n_ctas, st) : launch_mb_persist<16>(P, n_ctas, st);
 }
 
+// an unknown rcmarl_agg_rule, or TRIM with fewer than 2H + 1 values (callers have checked 0 <= H < n_in)
+static bool bad_rule(int rule, int H, int n_in) {
+    return rule < RCMARL_AGG_CLIP || rule > RCMARL_AGG_WMSR || (rule == RCMARL_AGG_TRIM && 2 * H >= n_in);
+}
+
 int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs, void* ws, int64_t ws_bytes,
                 void* stream) {
     if (int e = check_rows(rows)) return e;
@@ -717,10 +722,12 @@ int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs
         if (!q.w || q.kind < 0 || q.kind > 2) return RCMARL_ERR_ARG;
         if (!q.agg_in) {
             if (!q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+            if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         }
         if (!q.sums && !q.agg_out) return RCMARL_ERR_ARG;
         any_sums |= (q.sums != nullptr);
         P.jobs[j] = q;
+        if (q.agg_in) P.jobs[j].n_in = 0;         // the aggregate is supplied: no neighbour head is staged or read
         Q.sums[j] = q.sums;
         Q.n[j] = q.sums ? TEAM_N : 0;
     }
@@ -767,6 +774,7 @@ int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs, int n_jobs, void* 
         const rcmarl_consensus_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in || q.n_hidden < 1)
             return RCMARL_ERR_ARG;
+        if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         P.jobs[j] = q;
         if (q.n_hidden > maxn) maxn = q.n_hidden;
     }

@@ -21,6 +21,8 @@ N_ACTIONS = 5
 
 IN_S, IN_SA, IN_NS = 0, 1, 2
 LOSS_MSE, LOSS_CE = 0, 1
+AGG_CLIP, AGG_TRIM, AGG_WMSR = 0, 1, 2            # rcmarl_agg_rule
+AGG_RULES = {"clip": AGG_CLIP, "trim": AGG_TRIM, "wmsr": AGG_WMSR}
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -32,7 +34,7 @@ class Rows(C.Structure):
 
 class ConsensusJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("n_hidden", C.c_int32),
-                ("n_in", C.c_int32), ("H", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS)]
+                ("n_in", C.c_int32), ("H", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS), ("rule", C.c_int32)]
 
 
 class ValueJob(C.Structure):
@@ -61,7 +63,7 @@ class AdamJob(C.Structure):
 class TeamJob(C.Structure):
     _fields_ = [("w", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("sums", c_fp), ("agg_out", c_fp),
                 ("agg_in", c_fp), ("kind", C.c_int32), ("n_in", C.c_int32), ("H", C.c_int32),
-                ("in_nodes", C.c_int32 * MAX_NEIGHBOURS)]
+                ("in_nodes", C.c_int32 * MAX_NEIGHBOURS), ("rule", C.c_int32)]
 
 
 class RolloutArgs(C.Structure):
@@ -137,6 +139,28 @@ def check(status, what):
         l = lib()
         msg = l.rcmarl_status_string(status).decode()
         raise RcmarlError(f"{what}: {msg} (status {status}, cudaError {l.rcmarl_last_cuda_error()})")
+
+
+def agg_rule(rule):
+    """Aggregation rule name ("clip", "trim", "wmsr") or rcmarl_agg_rule id -> id.  Ids are passed through unchecked
+    (the library refuses unknown ones); an unknown name raises."""
+    if isinstance(rule, str):
+        if rule not in AGG_RULES:
+            raise RcmarlError(f"unknown aggregation rule {rule!r}: expected one of {sorted(AGG_RULES)}")
+        return AGG_RULES[rule]
+    return int(rule)
+
+
+def check_aggregation(rule, H, n_in):
+    """Raise RcmarlError unless `rule` is known and allows H trimmed values out of n_in (include/rcmarl.h): for every
+    rule 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in, for trim also 2H < n_in."""
+    r = agg_rule(rule)
+    if r not in AGG_RULES.values():
+        raise RcmarlError(f"unknown aggregation rule id {r}")
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in) or (r == AGG_TRIM and 2 * H >= n_in):
+        raise RcmarlError(f"aggregation {rule!r} with H={H} needs 0 <= H < n_in" + (" and 2H < n_in" if r == AGG_TRIM else "")
+                          + f" (n_in={n_in}, at most {MAX_NEIGHBOURS})")
+    return r
 
 
 def param_count(d_in, n_out):

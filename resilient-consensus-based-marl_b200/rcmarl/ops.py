@@ -237,11 +237,12 @@ def keras_adam_lr_t(lr, t, beta1=0.9, beta2=0.999):
     return float(np.float32(lr * np.sqrt(1.0 - beta2 ** t) / (1.0 - beta1 ** t)))
 
 
-def team_job(w, kind, msgs=None, msg_stride=0, in_nodes=(), H=0, sums=None, agg_out=None, agg_in=None):
+def team_job(w, kind, msgs=None, msg_stride=0, in_nodes=(), H=0, sums=None, agg_out=None, agg_in=None, rule="clip"):
+    """rule: aggregation rule name or rcmarl_agg_rule id (include/rcmarl.h)."""
     j = L.TeamJob()
     j.w, j.msgs, j.msg_stride = w.data_ptr(), ptr(msgs), msg_stride
     j.sums, j.agg_out, j.agg_in = ptr(sums), ptr(agg_out), ptr(agg_in)
-    j.kind, j.n_in, j.H = kind, len(in_nodes), H
+    j.kind, j.n_in, j.H, j.rule = kind, len(in_nodes), H, L.agg_rule(rule)
     for k, v in enumerate(in_nodes):
         j.in_nodes[k] = v
     j._keep = (w, msgs, sums, agg_out, agg_in)
@@ -255,9 +256,11 @@ def team(rows, jobs, ws=None):
     L.check(L.lib().rcmarl_team(C.byref(rows), a, len(a), ws.data_ptr(), ws.numel(), _stream()), "rcmarl_team")
 
 
-def consensus_job(dst, msgs, msg_stride, n_hidden, in_nodes, H):
+def consensus_job(dst, msgs, msg_stride, n_hidden, in_nodes, H, rule="clip"):
+    """rule: aggregation rule name or rcmarl_agg_rule id (include/rcmarl.h)."""
     j = L.ConsensusJob()
     j.dst, j.msgs, j.msg_stride, j.n_hidden, j.n_in, j.H = dst.data_ptr(), msgs.data_ptr(), msg_stride, n_hidden, len(in_nodes), H
+    j.rule = L.agg_rule(rule)
     for k, v in enumerate(in_nodes):
         j.in_nodes[k] = v
     j._keep = (dst, msgs)

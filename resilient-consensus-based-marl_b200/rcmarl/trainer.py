@@ -28,7 +28,7 @@ class Trainer:
                  fast_lr=0.01, slow_lr=0.01, max_ep_len=20, n_ep_fixed=50, n_epochs=10, buffer_size=2000,
                  common_reward=False, mu=0.1, seed=0, device=None, rank=0, world=1, group=None,
                  perm_source=None, local_steps=5, mb_epochs=10, mb_times=32, actor_mb_times=200,
-                 capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None):
+                 capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip"):
         L.lib()
         # Any team size up to 16 (main.py:26): the kernels are instantiated for 5 and 16 agents, a team of n_real agents
         # runs on the next instantiation with the extra agent slots zero (inputs and W1 rows, rcmarl/nets.py) -- exactly the
@@ -52,6 +52,14 @@ class Trainer:
             raise L.RcmarlError("H / fast_lr must be scalars or one value per agent")
         self.H += [0] * (NA - n_real)
         self.fast_lr += [self.fast_lr[0]] * (NA - n_real)
+        # per-agent resilient aggregation rule of the consensus and projection steps ("clip" is the reference's),
+        # checked against each cooperative agent's neighbour count and H before anything runs on the device
+        agg = [aggregation] * n_real if isinstance(aggregation, (str, int)) else list(aggregation)
+        if len(agg) != n_real:
+            raise L.RcmarlError("aggregation must be one rule or one rule per agent")
+        self.aggregation = [L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
+        for i in self.coop:
+            L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -320,11 +328,11 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            nodes = self.in_nodes[i]
-            cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, self.H[i]))
-            cons_jobs.append(ops.consensus_job(self.tr[i], self.msg_t, self.PT, nets.n_hidden_params(3 * NA), nodes, self.H[i]))
-            team_jobs.append(ops.team_job(self.critic[i], L.IN_S, self.msg_c, self.PC, nodes, self.H[i], sums=self.sums_team[2 * n]))
-            team_jobs.append(ops.team_job(self.tr[i], L.IN_SA, self.msg_t, self.PT, nodes, self.H[i], sums=self.sums_team[2 * n + 1]))
+            nodes, H, rule = self.in_nodes[i], self.H[i], self.aggregation[i]
+            cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
+            cons_jobs.append(ops.consensus_job(self.tr[i], self.msg_t, self.PT, nets.n_hidden_params(3 * NA), nodes, H, rule))
+            team_jobs.append(ops.team_job(self.critic[i], L.IN_S, self.msg_c, self.PC, nodes, H, sums=self.sums_team[2 * n], rule=rule))
+            team_jobs.append(ops.team_job(self.tr[i], L.IN_SA, self.msg_t, self.PT, nodes, H, sums=self.sums_team[2 * n + 1], rule=rule))
             team_apply.append(ops.sgd_job(self.critic[i], self.critic[i], self.sums_team[2 * n], self.PC, -1.0 / Bg, first=self.PC - 21))
             team_apply.append(ops.sgd_job(self.tr[i], self.tr[i], self.sums_team[2 * n + 1], self.PT, -1.0 / Bg, first=self.PT - 21))
         cons_jobs, team_jobs = ops.job_array(L.ConsensusJob, cons_jobs), ops.job_array(L.TeamJob, team_jobs)

@@ -39,6 +39,7 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
     # per-agent hyper-parameters, as the reference stores them (agents/resilient_CAC_agents.py:28-36)
     fast = [float(getattr(ag, 'fast_lr', args.get('fast_lr', 0.01))) for ag in agents]
     H = [int(getattr(ag, 'H', 0)) for ag in agents]
+    aggregation = [getattr(ag, 'aggregation', 'clip') for ag in agents]
     adam = [(ag.adam.m, ag.adam.v, ag.adam.t) if getattr(ag, 'adam', None) is not None and ag.adam.m is not None else None
             for ag in agents]
     rank, world = _dist_info()
@@ -49,7 +50,7 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
               n_envs=getattr(env, 'n_envs', 1), nrow=env.nrow, ncol=env.ncol, gamma=args['gamma'], H=H, fast_lr=fast, slow_lr=slow_lr, max_ep_len=args['max_ep_len'],
               n_ep_fixed=args['n_ep_fixed'], n_epochs=args['n_epochs'], buffer_size=args['buffer_size'],
               common_reward=bool(args['common_reward']), seed=int(args.get('random_seed', 0)), adam_state=adam,
-              rank=rank, world=world)
+              rank=rank, world=world, aggregation=aggregation)
     kw.update(overrides)
     tr = Trainer(**kw)
     if exp_buffer:                                                             # :36-40

@@ -5,6 +5,10 @@ of the last 500 episodes is printed next to the mean of the last 500 episodes of
 
     python tools/learning_harness.py [n_blocks=40] [n_envs=256] [filter]      -> gpurun_out/learning_harness.{json,md}
 
+An optional fourth argument, `rule` (default clip), is the cooperative agents' resilient aggregation (clip = the
+reference's, trim, wmsr; include/rcmarl.h), so the published scenarios can be rerun under each rule; the reference columns
+always come from the reference's clipped mean.
+
 The comparison is qualitative by construction (the published runs trained one environment for 8 000 episodes with an older
 code version, SURVEY 6): the reproduced claims are
   (1) under attack (faulty / greedy / malicious, local or team-average rewards) H = 1 keeps the cooperative team's return
@@ -26,6 +30,7 @@ from rcmarl.trainer import Trainer             # noqa: E402
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 only = sys.argv[3] if len(sys.argv) > 3 else ""
+rule = sys.argv[4] if len(sys.argv) > 4 else "clip"
 z = np.load(os.path.join(ROOT, "tests", "golden", "ref_learning.npz"))
 runs = [str(r) for r in z["runs"] if only in str(r)]
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
@@ -42,7 +47,7 @@ for tag in runs:
             n += 1
         w.append(nets_i)
     tr = Trainer(labels=labels, in_nodes=bench.IN_NODES5, weights=w, desired=z[f"{tag}/desired"], n_envs=n_envs, H=H, seed=seed,
-                 common_reward=bool(z[f"{tag}/common_reward"]), **bench.HYPER)
+                 common_reward=bool(z[f"{tag}/common_reward"]), aggregation=rule, **bench.HYPER)
     coop = [i for i, l in enumerate(labels) if l == "Cooperative"]
     adv = [i for i, l in enumerate(labels) if l != "Cooperative"]
     team, est, advr = [], [], []
@@ -78,7 +83,7 @@ for scen in ("malicious", "malicious_global"):
         checks.append(dict(claim=f"{scen} H=0: critic estimate poisoned above the true return", ours=a["ours_est"] - a["ours_team"],
                            reference=a["ref_est"] - a["ref_team"], holds=bool(a["ours_est"] - a["ours_team"] > 2.0)))
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(dict(n_blocks=n_blocks, n_envs=n_envs, runs=rows, summary=summary, checks=checks),
+json.dump(dict(n_blocks=n_blocks, n_envs=n_envs, rule=rule, runs=rows, summary=summary, checks=checks),
           open(os.path.join(ROOT, "gpurun_out", "learning_harness.json"), "w"))
 with open(os.path.join(ROOT, "gpurun_out", "learning_harness.md"), "w") as f:
     f.write(f"| scenario / H | seeds | ours team | ref team | ours estimate | ref estimate | ours adversary | ref adversary |\n|---|---|---|---|---|---|---|---|\n")
