@@ -407,9 +407,12 @@ class Trainer:
 
     def _minibatch_sgd(self, chains, T):
         """10 epochs x ceil(T/32) sequential SGD steps per chain; a mini-batch = 32 time rows x all environments
-        (Appendix C).  All chains advance in lock-step in ONE persistent kernel, or, data-parallel without the
-        peer-memory exchange, as rcmarl_grad -> NCCL all-reduce -> rcmarl_sgd_apply per step."""
+        (Appendix C).  The chains advance in lock-step in ONE persistent kernel, or, data-parallel without the
+        peer-memory exchange, as rcmarl_grad -> NCCL all-reduce -> rcmarl_sgd_apply per step.  Both take at most
+        MAX_JOBS chains, and a team of 16 adversaries has up to 48: the chains, which are independent, then run in
+        consecutive groups of MAX_JOBS."""
         E = self.mb_epochs
+        # every permutation is drawn before the first group runs, chain-major (the order of the reference's fits)
         perms = torch.stack([torch.stack([self._perm(T) for _ in range(E)]) for _ in chains]).to(self.dev)  # [C,E,T]
         self.h2d_bytes += 4 * perms.numel()
         gj, aj = [], []
@@ -420,14 +423,15 @@ class Trainer:
             aj.append(ops.sgd_job(w, w, sums, n, lr, loss_out=loss, loss_coef=1.0 / (T * self.N * self.world)))
         rows = self._rows(0, 0, perms)
         lrs = [ch[5] for ch in chains]
-        if self.world == 1 or self.comm is not None:
-            ops.minibatch_fit(rows, gj, aj, E, T, self.mb_times, lrs[0], self.mb_cells)
-            self.launches += 1
-        else:
-            nC = len(chains)
-            ops.minibatch_steps(rows, gj, aj, E, T, self.mb_times, lrs, self.world,
-                                lambda: self._allreduce(self.sums_mb[:nC]), self.ws)
-            self.launches += 3 * E * ((T + self.mb_times - 1) // self.mb_times)
+        for g0 in range(0, len(chains), L.MAX_JOBS):
+            g = slice(g0, g0 + L.MAX_JOBS)
+            if self.world == 1 or self.comm is not None:
+                ops.minibatch_fit(rows, gj[g], aj[g], E, T, self.mb_times, lrs[0], self.mb_cells)
+                self.launches += 1
+            else:
+                ops.minibatch_steps(rows, gj[g], aj[g], E, T, self.mb_times, lrs[g], self.world,
+                                    lambda s=self.sums_mb[g]: self._allreduce(s), self.ws)
+                self.launches += 3 * E * ((T + self.mb_times - 1) // self.mb_times)
 
     def _minibatch_adam(self, adv, T, Ta, a0):
         """actor.fit(batch_size=200, epochs=1) of the adversaries (adversarial:41,116,224)."""
