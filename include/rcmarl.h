@@ -123,6 +123,38 @@ typedef struct {
 } rcmarl_consensus_job;
 int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs_host, int n_jobs, void* stream);
 
+/* Byzantine messages crafted for one receiver (threat model: DESIGN.md section 1).  A Byzantine agent is omniscient
+ * about its receiver j's neighbourhood: over the honest set S_j (the cooperative agents of in_nodes[j], in list order,
+ * repeats included, n = n_honest), per packed parameter p,
+ *   mu_p = (sum_k v_k,p) / n   (summed in S_j order),   sigma_p = sqrt(sum_k (v_k,p - mu_p)^2 / n)   (population std,
+ * two passes), with v_k = msgs + honest[k] * msg_stride, and it sends j
+ *   ALIE   (Baruch et al., NeurIPS 2019, "A Little Is Enough"), param z:   m_p = mu_p - z * sigma_p
+ *   IPM    (Xie et al., UAI 2019, inner-product manipulation), param eps:  m_p = -eps * mu_p
+ *   GAUSS  param s >= 0:                                                    m_p = mu_p + s * xi_p,  xi_p ~ N(0, 1)
+ * xi_p comes from the rollout's counter-based Philox4x32-10 with key (seed low word, seed high word) and counter
+ *   (p, attacker | receiver << 8 | 0x40000000, round, epoch)
+ * (bit 30 of word 1 keeps these streams apart from the rollout's); of its output (x, y, ., .), Box-Muller takes
+ * u1 = ((x >> 8) + 1) * 2^-24 in (0, 1] and u2 = (y >> 8) * 2^-24 and gives xi = sqrt(-2 ln u1) * cos(2 pi u2).  The
+ * draw depends on (seed, round, epoch, attacker, receiver, p) only, never on the launch or the job order.
+ * One thread per coordinate, fixed summation order, no atomics: bitwise reproducible.  dst[0:n] = m; dst must not
+ * overlap the honest rows.  Refused (RCMARL_ERR_ARG, nothing launched, dst untouched): a null pointer, n < 1, n_honest
+ * outside 1..RCMARL_MAX_NEIGHBOURS, a negative honest index, an unknown kind, a non-finite param, GAUSS with s < 0,
+ * attacker or receiver outside 0..255 (the counter holds 8 bits of each). */
+typedef enum { RCMARL_ATTACK_ALIE = 0, RCMARL_ATTACK_IPM = 1, RCMARL_ATTACK_GAUSS = 2 } rcmarl_attack_kind;
+typedef struct {
+    float* dst;                 /* the crafted message (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    int32_t n;                  /* parameters crafted: dst[0:n] from msgs[honest[k]][0:n] */
+    int32_t n_honest;
+    int32_t honest[RCMARL_MAX_NEIGHBOURS];
+    int32_t kind;               /* rcmarl_attack_kind */
+    float param;                /* z, eps or s */
+    uint64_t seed;              /* Philox key (GAUSS) */
+    uint32_t attacker, receiver, round, epoch;   /* Philox counter words (GAUSS) */
+} rcmarl_attack_job;
+int rcmarl_attack(const rcmarl_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

@@ -4,6 +4,7 @@ mfigura/Resilient-consensus-based-MARL) on the sm_90a kernels of librcmarl.so.
   Faulty_CAC_agent     :5-72    transmits fixed critic / TR parameters, trains only its actor
   Malicious_CAC_agent  :74-182  private local critic + compromised critic / TR trained on -r_coop and transmitted
   Greedy_CAC_agent     :184-275 trains critic / TR on its own reward and transmits them
+  Byzantine_CAC_agent  (not in the reference) learns like Faulty; sends each cooperative receiver its own crafted message
 Mini-batch fits use Keras defaults (batch_size rows shuffled per epoch, SURVEY Appendix A.3).  The shuffle stream is
 private (like TF's); `perm_source` (callable T -> permutation) can be set on an agent to inject it."""
 import numpy as np
@@ -69,6 +70,20 @@ class Faulty_CAC_agent(_AdversaryBase):
 
     def get_TR_weights(self):                                                       # :51-55
         return A.DeviceWeights(self.TR.flat.clone(), self.TR.d_in, 1)
+
+
+class Byzantine_CAC_agent(Faulty_CAC_agent):
+    """Learns like Faulty_CAC_agent; what it transmits is crafted by the training loop for each cooperative receiver
+    from that receiver's honest neighbours (`attack` = ("alie", z), ("ipm", eps) or ("gauss", s); threat model at
+    rcmarl_attack in include/rcmarl.h).  The reference has no such agent: train_RPBCAC reads `attack` from it, under
+    the label "Byzantine".  get_critic_weights / get_TR_weights return the untouched nets, as Faulty's do: an agent
+    alone has no view of its receivers' neighbourhoods."""
+
+    def __init__(self, actor, critic, team_reward, slow_lr, gamma=0.95, attack=None):
+        super().__init__(actor, critic, team_reward, slow_lr, gamma)
+        from rcmarl import _lib
+        _lib.check_attack(attack)
+        self.attack = (attack[0], float(attack[1]))
 
 
 class Malicious_CAC_agent(_AdversaryBase):

@@ -272,4 +272,17 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// Philox4x32-10 (Salmon et al.), counter-based: the rollout's action / reset draws and rcmarl_attack's Gaussian messages
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+        k.x += 0x9E3779B9u;
+        k.y += 0xBB67AE85u;
+    }
+    return c;
+}
+
 }  // namespace rcmarl

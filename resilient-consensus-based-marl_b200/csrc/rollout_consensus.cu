@@ -290,18 +290,7 @@ __global__ void __launch_bounds__(256) env_step_kernel(int32_t* __restrict__ sta
     state[2 * i + 1] = y;
 }
 
-// Philox4x32-10 (Salmon et al.), counter-based: one call per (env, episode, step, agent)
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-    for (int i = 0; i < 10; ++i) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-        k.x += 0x9E3779B9u;
-        k.y += 0xBB67AE85u;
-    }
-    return c;
-}
+// Philox4x32-10 (common.cuh): one call per (env, episode, step, agent)
 __device__ __forceinline__ float u01(uint32_t x) { return (float)(x >> 8) * (1.0f / 16777216.0f); }
 
 // get_action (agents/resilient_CAC_agents.py:208-219) from three uniforms:

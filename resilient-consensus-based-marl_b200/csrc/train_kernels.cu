@@ -8,10 +8,12 @@
 //                            outer products, accumulated in registers across ALL rows of the CTA;
 //                   deterministic two-level reduction (CTA partials -> reduce_kernel).
 //   team_kernel     K5+K6  neighbour-head estimates, clipped mean, projection numerators
+//   attack_kernel   Byzantine messages crafted per receiver (ALIE / IPM / Gaussian, rcmarl_attack)
 //   consensus, sgd/adam apply, reward mix: the small glue kernels.
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
 // training/train_agents.py:86-163 (cited per entry point in include/rcmarl.h).
+#include <cmath>
 #include "common.cuh"
 #include "grad_kernel.cuh"
 #include "comm.cuh"
@@ -330,6 +332,42 @@ __global__ void __launch_bounds__(256) consensus_hidden_kernel(const __grid_cons
     for (int k = 0; k < RCMARL_MAX_NEIGHBOURS; ++k)
         v[k] = k < job.n_in ? __ldg(job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride + i) : 0.f;
     job.dst[i] = resilient_mean_small<RCMARL_MAX_NEIGHBOURS>(v, job.n_in, job.H, job.rule);
+}
+
+// Byzantine messages (rcmarl_attack, include/rcmarl.h): one thread per coordinate; mean and population std over the
+// honest set in list order (two passes over registers), then the attack
+struct AttackParams { rcmarl_attack_job jobs[RCMARL_MAX_JOBS]; };
+__global__ void __launch_bounds__(256) attack_kernel(const __grid_constant__ AttackParams P) {
+    const rcmarl_attack_job& job = P.jobs[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= job.n) return;
+    const int n = job.n_honest;
+    float v[RCMARL_MAX_NEIGHBOURS];
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < RCMARL_MAX_NEIGHBOURS; ++k) {
+        v[k] = k < n ? __ldg(job.msgs + (int64_t)job.honest[k] * job.msg_stride + i) : 0.f;
+        if (k < n) s += v[k];
+    }
+    const float mu = s / (float)n;
+    float m;
+    if (job.kind == RCMARL_ATTACK_ALIE) {
+        float q = 0.f;
+#pragma unroll
+        for (int k = 0; k < RCMARL_MAX_NEIGHBOURS; ++k)
+            if (k < n) q = fmaf(v[k] - mu, v[k] - mu, q);
+        m = mu - job.param * sqrtf(q / (float)n);
+    } else if (job.kind == RCMARL_ATTACK_IPM) {
+        m = -job.param * mu;
+    } else {
+        const uint4 r = philox4x32_10(make_uint4((uint32_t)i, job.attacker | job.receiver << 8 | 0x40000000u, job.round,
+                                                 job.epoch),
+                                      make_uint2((uint32_t)job.seed, (uint32_t)(job.seed >> 32)));
+        const float u1 = (float)((r.x >> 8) + 1) * (1.0f / 16777216.0f);
+        const float u2 = (float)(r.y >> 8) * (1.0f / 16777216.0f);
+        m = mu + job.param * (sqrtf(-2.f * logf(u1)) * cospif(2.f * u2));
+    }
+    job.dst[i] = m;
 }
 
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
@@ -779,6 +817,26 @@ int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs, int n_jobs, void* 
         if (q.n_hidden > maxn) maxn = q.n_hidden;
     }
     consensus_hidden_kernel<<<dim3((maxn + 255) / 256, n_jobs), 256, 0, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_attack(const rcmarl_attack_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    AttackParams P;
+    int maxn = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_attack_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_honest; ++k)
+            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (q.kind < RCMARL_ATTACK_ALIE || q.kind > RCMARL_ATTACK_GAUSS || !std::isfinite(q.param)) return RCMARL_ERR_ARG;
+        if (q.kind == RCMARL_ATTACK_GAUSS && q.param < 0.f) return RCMARL_ERR_ARG;
+        if (q.attacker > 255u || q.receiver > 255u) return RCMARL_ERR_ARG;
+        P.jobs[j] = q;
+        if (q.n > maxn) maxn = q.n;
+    }
+    attack_kernel<<<dim3((maxn + 255) / 256, n_jobs), 256, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

@@ -5,6 +5,7 @@ fails, an exception is raised.  The library is built in-tree by
 ``__graft_entry__.build()`` / ``make -C resilient-consensus-based-marl_b200/csrc``.
 """
 import ctypes as C
+import math
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -23,6 +24,8 @@ IN_S, IN_SA, IN_NS = 0, 1, 2
 LOSS_MSE, LOSS_CE = 0, 1
 AGG_CLIP, AGG_TRIM, AGG_WMSR = 0, 1, 2            # rcmarl_agg_rule
 AGG_RULES = {"clip": AGG_CLIP, "trim": AGG_TRIM, "wmsr": AGG_WMSR}
+ATTACK_ALIE, ATTACK_IPM, ATTACK_GAUSS = 0, 1, 2   # rcmarl_attack_kind
+ATTACKS = {"alie": ATTACK_ALIE, "ipm": ATTACK_IPM, "gauss": ATTACK_GAUSS}
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -35,6 +38,12 @@ class Rows(C.Structure):
 class ConsensusJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("n_hidden", C.c_int32),
                 ("n_in", C.c_int32), ("H", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS), ("rule", C.c_int32)]
+
+
+class AttackJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("n", C.c_int32), ("n_honest", C.c_int32),
+                ("honest", C.c_int32 * MAX_NEIGHBOURS), ("kind", C.c_int32), ("param", C.c_float), ("seed", C.c_uint64),
+                ("attacker", C.c_uint32), ("receiver", C.c_uint32), ("round", C.c_uint32), ("epoch", C.c_uint32)]
 
 
 class ValueJob(C.Structure):
@@ -88,6 +97,7 @@ SYMBOLS = [
                                         C.POINTER(C.c_int32)]),
     ("rcmarl_clip_mean", C.c_int, [c_fp, C.c_int, C.c_int64, C.c_int64, C.c_int, c_fp, c_fp]),
     ("rcmarl_consensus_hidden", C.c_int, [C.POINTER(ConsensusJob), C.c_int, c_fp]),
+    ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
@@ -161,6 +171,21 @@ def check_aggregation(rule, H, n_in):
         raise RcmarlError(f"aggregation {rule!r} with H={H} needs 0 <= H < n_in" + (" and 2H < n_in" if r == AGG_TRIM else "")
                           + f" (n_in={n_in}, at most {MAX_NEIGHBOURS})")
     return r
+
+
+def check_attack(attack):
+    """(name, param) -> (rcmarl_attack_kind, float param); raise RcmarlError unless the name is known and the parameter
+    finite (and, for "gauss", s >= 0), as rcmarl_attack requires (include/rcmarl.h)."""
+    try:
+        name, param = attack
+        param = float(param)
+    except (TypeError, ValueError):
+        raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
+    if not isinstance(name, str) or name not in ATTACKS:
+        raise RcmarlError(f"unknown attack {name!r}: expected one of {sorted(ATTACKS)}")
+    if not math.isfinite(param) or (name == "gauss" and param < 0):
+        raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if name == "gauss" else "") + f", got {param}")
+    return ATTACKS[name], param
 
 
 def param_count(d_in, n_out):

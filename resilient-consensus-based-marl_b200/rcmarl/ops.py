@@ -272,6 +272,29 @@ def consensus_hidden(jobs):
     L.check(L.lib().rcmarl_consensus_hidden(a, len(a), _stream()), "rcmarl_consensus_hidden")
 
 
+def attack_job(dst, msgs, msg_stride, n, honest, kind, param, seed=0, attacker=0, receiver=0, round=0, epoch=0):
+    """kind: attack name ("alie", "ipm", "gauss") or rcmarl_attack_kind id; honest: the message rows of the honest set
+    in list order (include/rcmarl.h).  Names are checked here, ids and parameters by the library."""
+    j = L.AttackJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.n_honest = len(honest)
+    for k, v in enumerate(honest[:L.MAX_NEIGHBOURS]):
+        j.honest[k] = v
+    if isinstance(kind, str):
+        if kind not in L.ATTACKS:
+            raise L.RcmarlError(f"unknown attack {kind!r}: expected one of {sorted(L.ATTACKS)}")
+        kind = L.ATTACKS[kind]
+    j.kind, j.param = int(kind), param
+    j.seed, j.attacker, j.receiver, j.round, j.epoch = int(seed), attacker, receiver, round, epoch
+    j._keep = (dst, msgs)
+    return j
+
+
+def attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.AttackJob, jobs)
+    L.check(L.lib().rcmarl_attack(a, len(a), _stream()), "rcmarl_attack")
+
+
 def reward_mix(r, agents, out=None, scale=1.0):
     """r: [rows, n_agents]; out[row] = scale * sum_k r[row, agents[k]] / len(agents) in list order."""
     n_rows, n_agents = r.shape

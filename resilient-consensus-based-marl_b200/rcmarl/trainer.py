@@ -19,7 +19,7 @@ import torch
 from . import _lib as L
 from . import dist_util, nets, ops
 
-COOP, GREEDY, MALICIOUS, FAULTY = "Cooperative", "Greedy", "Malicious", "Faulty"
+COOP, GREEDY, MALICIOUS, FAULTY, BYZANTINE = "Cooperative", "Greedy", "Malicious", "Faulty", "Byzantine"
 PAD = "(unused agent slot)"
 
 
@@ -28,7 +28,8 @@ class Trainer:
                  fast_lr=0.01, slow_lr=0.01, max_ep_len=20, n_ep_fixed=50, n_epochs=10, buffer_size=2000,
                  common_reward=False, mu=0.1, seed=0, device=None, rank=0, world=1, group=None,
                  perm_source=None, local_steps=5, mb_epochs=10, mb_times=32, actor_mb_times=200,
-                 capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip"):
+                 capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip",
+                 attack=None):
         L.lib()
         # Any team size up to 16 (main.py:26): the kernels are instantiated for 5 and 16 agents, a team of n_real agents
         # runs on the next instantiation with the extra agent slots zero (inputs and W1 rows, rcmarl/nets.py) -- exactly the
@@ -60,6 +61,7 @@ class Trainer:
         self.aggregation = [L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
         for i in self.coop:
             L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
+        self._init_attacks(attack)
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -89,8 +91,9 @@ class Trainer:
             self.critic[i].copy_(torch.as_tensor(nets.pack_padded(w[1], 2 * NA)))
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
-        self.msg_c = torch.zeros(NA, self.PC, **f32)
-        self.msg_t = torch.zeros(NA, self.PT, **f32)
+        # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e
+        self.msg_c = torch.zeros(NA + len(self.byz_pairs), self.PC, **f32)
+        self.msg_t = torch.zeros(NA + len(self.byz_pairs), self.PT, **f32)
         self.adam_m = torch.zeros(NA, self.PA, **f32)
         self.adam_v = torch.zeros(NA, self.PA, **f32)
         self.adam_t = [0] * NA
@@ -138,6 +141,42 @@ class Trainer:
             self.comm = self._try_peer_comm()
 
     # ------------------------------------------------------------------ helpers
+    def _init_attacks(self, attack):
+        """Check the Byzantine agents' attacks and list the (attacker, cooperative receiver) pairs, each with its own
+        crafted message row, before anything runs on the device.  attack: None, one (name, param) for every Byzantine
+        agent, or one entry per agent (None for the agents that are not Byzantine)."""
+        n_real, lab = self.n_real, self.labels
+        if attack is None or (isinstance(attack, tuple) and len(attack) == 2 and isinstance(attack[0], str)):
+            att = [attack if lab[i] == BYZANTINE else None for i in range(n_real)]
+        else:
+            att = list(attack)
+            if len(att) != n_real:
+                raise L.RcmarlError("attack must be one (name, param) pair or one entry per agent")
+        self.attack = [None] * n_real
+        for i in range(n_real):
+            if (att[i] is None) != (lab[i] != BYZANTINE):
+                raise L.RcmarlError(f"agent {i} ({lab[i]}): " + ("a Byzantine agent needs an attack" if att[i] is None
+                                                                 else "only a Byzantine agent takes an attack"))
+            if att[i] is not None:
+                self.attack[i] = L.check_attack(att[i])
+        # pair e = (attacker b, receiver j, honest set S_j: the cooperative agents of in_nodes[j] in list order)
+        self.byz_pairs = []
+        for b in range(n_real):
+            if lab[b] != BYZANTINE:
+                continue
+            for j in self.coop:
+                if b in self.in_nodes[j]:
+                    honest = [k for k in self.in_nodes[j] if lab[k] == COOP]
+                    if not honest:
+                        raise L.RcmarlError(f"cooperative agent {j} hears Byzantine agent {b} but no cooperative agent: "
+                                            "the attack has no honest set")
+                    self.byz_pairs.append((b, j, honest))
+
+    def _receiver_nodes(self, j):
+        """in_nodes[j] with each Byzantine neighbour replaced by the message row crafted for receiver j."""
+        row = {b: self.NA + e for e, (b, r, _) in enumerate(self.byz_pairs) if r == j}
+        return [row.get(k, k) for k in self.in_nodes[j]]
+
     def _try_peer_comm(self):
         """Set up the peer-memory exchange on every rank, or on none: the ranks agree (MIN all-reduce of a success
         flag) so that a box without IPC / peer access falls back to the NCCL path consistently instead of deadlocking."""
@@ -328,7 +367,7 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            nodes, H, rule = self.in_nodes[i], self.H[i], self.aggregation[i]
+            nodes, H, rule = self._receiver_nodes(i), self.H[i], self.aggregation[i]
             cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
             cons_jobs.append(ops.consensus_job(self.tr[i], self.msg_t, self.PT, nets.n_hidden_params(3 * NA), nodes, H, rule))
             team_jobs.append(ops.team_job(self.critic[i], L.IN_S, self.msg_c, self.PC, nodes, H, sums=self.sums_team[2 * n], rule=rule))
@@ -338,7 +377,16 @@ class Trainer:
         cons_jobs, team_jobs = ops.job_array(L.ConsensusJob, cons_jobs), ops.job_array(L.TeamJob, team_jobs)
         team_apply = ops.job_array(L.SgdJob, team_apply)
 
-        for _epoch in range(self.n_epochs):                                # :100
+        # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
+        att_jobs = []
+        for e, (b, j, honest) in enumerate(self.byz_pairs):
+            kind, param = self.attack[b]
+            for msgs, P in ((self.msg_c, self.PC), (self.msg_t, self.PT)):
+                att_jobs.append(ops.attack_job(msgs[NA + e], msgs, P, P, honest, kind, param, seed=self.seed, attacker=b,
+                                               receiver=j, round=self.episodes_done & 0xFFFFFFFF))
+        att_groups = [ops.job_array(L.AttackJob, att_jobs[g:g + L.MAX_JOBS]) for g in range(0, len(att_jobs), L.MAX_JOBS)]
+
+        for epoch in range(self.n_epochs):                                 # :100
             # ---------------- I) local updates (:105-121)
             if td_jobs:
                 ops.values(rows_all, td_arr)
@@ -355,6 +403,11 @@ class Trainer:
                 if lab[i] != COOP:
                     self.msg_c[i].copy_(self.critic[i])
                     self.msg_t[i].copy_(self.tr[i])
+            for g in att_groups:
+                for job in g:
+                    job.epoch = epoch
+                ops.attack(g)
+                self.launches += 1
             # ---------------- II) resilient consensus (:125-145)
             if coop:
                 ops.consensus_hidden(cons_jobs)

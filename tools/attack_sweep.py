@@ -1,0 +1,116 @@
+"""Byzantine attacks against each resilient aggregation rule on the C2 team: 4 cooperative agents (H = 1) and agent 4
+Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (clip, trim, wmsr) x attack (alie, ipm, gauss) over the
+learning harness's seeds (tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed;
+agent 4 keeps its weights and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the
+cooperative critics' estimate of it, means of the last 500 episodes, over the seeds.
+
+Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
+agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).
+
+    python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
+        -> out_dir/attack_sweep.{json,md} (a relative out_dir is taken from the current directory)
+"""
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "resilient-consensus-based-marl_b200"))
+import bench                                   # noqa: E402
+import torch                                   # noqa: E402
+from rcmarl.trainer import Trainer             # noqa: E402
+
+RULES = ("clip", "trim", "wmsr")
+ATTACKS = (("alie", 1.0), ("ipm", 0.5), ("gauss", 0.3))
+n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
+n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
+timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
+out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_out")
+tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return name, float(out.splitlines()[0])
+    except Exception:
+        return name, None
+
+
+def timing():
+    """ms per update round (median over rounds) with agent 4 Faulty and Byzantine, both at the benchmark's C2 shape."""
+    cfg = bench.workload("C2", 0)
+    base = dict(cfg, labels=["Cooperative"] * 4 + ["Faulty"])
+    trs = {"Faulty": Trainer(**base), "Byzantine": Trainer(**dict(base, labels=["Cooperative"] * 4 + ["Byzantine"],
+                                                                   attack=("gauss", 0.3)))}
+    ms = {k: [] for k in trs}
+    for r in range(timed_rounds + 1):
+        for k, tr in trs.items():
+            tr.rollout_block()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            a.record()
+            tr.update_round()
+            b.record()
+            torch.cuda.synchronize()
+            if r > 0:                                   # round 0 warms up
+                ms[k].append(a.elapsed_time(b))
+    out = {k: dict(median_ms=float(np.median(v)), rounds_ms=v) for k, v in ms.items()}
+    out["added_ms"] = out["Byzantine"]["median_ms"] - out["Faulty"]["median_ms"]
+    out["n_envs"] = cfg["n_envs"]
+    out["attack_launches_per_round"] = trs["Byzantine"].n_epochs
+    return out
+
+
+z = np.load(os.path.join(ROOT, "tests", "golden", "ref_learning.npz"))
+runs = [str(r) for r in z["runs"] if str(r).startswith("malicious/H1/")]
+name, power = card()
+result = dict(card=name, power_limit_w=power, n_blocks=n_blocks, n_envs=n_envs, timing=timing(), cells=[])
+print(f"{name}, power limit {power} W: update round {result['timing']['Faulty']['median_ms']:.2f} ms (Faulty) vs "
+      f"{result['timing']['Byzantine']['median_ms']:.2f} ms (Byzantine)", flush=True)
+for rule in RULES:
+    for attack in ATTACKS:
+        team, est = [], []
+        for tag in runs:
+            _, _, ss = tag.split("/")
+            labels = [str(x) for x in z[f"{tag}/labels"]]
+            assert labels == ["Cooperative"] * 4 + ["Malicious"]
+            w = []
+            for i in range(5):
+                nets_i, n = [], 0
+                while f"{tag}/agent{i}/n{n}_k0" in z.files:
+                    nets_i.append([z[f"{tag}/agent{i}/n{n}_k{k}"] for k in range(6)])
+                    n += 1
+                w.append(nets_i[:3])
+            tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
+                         desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=rule, attack=attack,
+                         **bench.HYPER)
+            t, e = [], []
+            for _ in range(n_blocks):
+                ee, rr = tr.rollout_block()
+                tr.update_round()
+                t.append(float(rr[:, :4].mean())); e.append(float(ee[:, :4].mean()))
+            team.append(float(np.mean(t[-tail:]))); est.append(float(np.mean(e[-tail:])))
+        cell = dict(rule=rule, attack=attack[0], param=attack[1], seeds=len(runs), team=float(np.mean(team)),
+                    est=float(np.mean(est)), team_per_seed=team, est_per_seed=est)
+        result["cells"].append(cell)
+        print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}", flush=True)
+
+os.makedirs(out_dir, exist_ok=True)
+json.dump(result, open(os.path.join(out_dir, "attack_sweep.json"), "w"))
+with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
+    f.write(f"{name}, power limit {power} W; {len(runs)} seeds, {n_blocks} blocks x 50 episodes, {n_envs} environments; "
+            "means of the last 500 episodes\n\n| rule | attack | team return | critic estimate |\n|---|---|---|---|\n")
+    for c in result["cells"]:
+        f.write(f"| {c['rule']} | {c['attack']} {c['param']} | {c['team']:.2f} | {c['est']:.2f} |\n")
+    t = result["timing"]
+    f.write(f"\nC2 update round at {t['n_envs']} environments (median of {timed_rounds}, alternated): "
+            f"{t['Faulty']['median_ms']:.2f} ms with agent 4 Faulty, {t['Byzantine']['median_ms']:.2f} ms Byzantine (gauss), "
+            f"{t['added_ms']:+.2f} ms\n")
+print(open(os.path.join(out_dir, "attack_sweep.md")).read())
