@@ -313,8 +313,20 @@ int rcmarl_comm_destroy(void* comm);
  * K1 + K8.  A block of episodes under a fixed policy for n_envs environments
  * (training/train_agents.py:46-80 + environments/grid_world.py:37-72 +
  * get_action, agents/resilient_CAC_agents.py:208-219): one thread per (episode, env).
- * Randomness: Philox4x32-10 keyed by (seed, env_offset+env, episode_offset+episode, step, agent)
- * or, for parity tests, injected through `uniforms` / `init_state`. */
+ * Randomness, unless injected through `uniforms` / `init_state` (parity tests): Philox4x32-10 (Salmon et al. 2011,
+ * the generator of rcmarl_attack) with key (seed low word, seed high word).  With g = env_offset + env (64 bits),
+ * ep = the low 32 bits of episode_offset + episode, NA = n_agents (the 5- or 16-agent instantiation, also when
+ * n_active is smaller), j = step, i = agent < n_active, and u01(w) = (w >> 8) * 2^-24 (exact in fp32, in [0, 1)):
+ *   reset   counter (g low, g high ^ 0x80000000, ep, i)  -> (x, y, ., .):  px = umulhi(x, nrow) = (x * nrow) >> 32,
+ *                                                                           py = umulhi(y, ncol)
+ *   action  counter (g low, g high, ep, j * NA + i)      -> (x, y, z, .):  u0 = u01(x), u1 = u01(y), u2 = u01(z)
+ * and get_action takes random_action = min(floor(u0 * 5), 4), the policy action = #{o : cdf_o / cdf_4 <= u1} (capped
+ * at 4, cdf in fp32), and the policy action if u2 < 1 - mu, else the random one.  Word 1 keeps the streams apart: bit
+ * 31 is set in every reset counter and clear in every action counter, and rcmarl_attack's word 1 (attacker | receiver
+ * << 8 | 0x40000000) has bit 31 clear and bit 30 set, so while g < 2^62 no two of the three streams share a counter.
+ * Within a stream the counters are distinct while j * NA + i < 2^32; the episode word repeats after 2^32 episodes.
+ * An injected `uniforms` / `init_state` replaces the draws one for one, laid out [episode][step][env][n_active][3] and
+ * [episode][env][n_active][2]. */
 typedef struct {
     const float* actor_w;       /* [n_agents][P_actor] */
     const float* critic_w;      /* [n_agents][P_critic] for the est_returns log (train_agents.py:62) */

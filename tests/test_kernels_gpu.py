@@ -370,7 +370,9 @@ def test_rollout_matches_oracle_with_injected_randomness(K, NA, nrow, N):
 
 def test_rollout_philox_statistics_and_determinism(K):
     """Without injected randomness: same seed -> identical rows; env shards are independent of the launch
-    decomposition (env_offset); resets are uniform over the grid; mu-mixture is respected."""
+    decomposition (env_offset); another seed gives other rows; agent 0's reset x covers the grid; actions are in
+    0..4 and rewards in range.  The draws themselves (reset and action counters, u01, the mu-mixture) are pinned
+    exactly in test_rollout_philox_gpu.py and test_rollout_streams_cpu.py."""
     NA, N, n_ep, L_ = 5, 256, 10, 20
     w, desired, _ = pretrained()
     aw, cw = to_dev(K, np.stack([K.nets.pack(w[i][0]) for i in range(5)]), np.stack([K.nets.pack(w[i][1]) for i in range(5)]))
