@@ -162,10 +162,17 @@ def fit_minibatch(w, x, y, lr, epochs, batch_size, perms):
 
 class KerasAdam:
     """Adam as implemented by TF-2.x Keras (Appendix A.5): epsilon added to
-    sqrt(v) without bias correction, lr_t = lr*sqrt(1-b2^t)/(1-b1^t)."""
+    sqrt(v) without bias correction, lr_t = lr*sqrt(1-b2^t)/(1-b1^t).
 
-    def __init__(self, lr, beta1=0.9, beta2=0.999, eps=1e-7):
+    fp32_betas=True: the moment updates take beta1, beta2 as the float32
+    constants (0.9f, 0.999f) and 1 - beta as their float32 difference
+    (1.f - 0.999f = 0.00099998713, 1.3e-5 below 0.001), as TF does for
+    float32 variables and as rcmarl_adam_apply does; lr_t keeps the exact
+    constants (ops.keras_adam_lr_t).  The default keeps 1 - 0.999 exact."""
+
+    def __init__(self, lr, beta1=0.9, beta2=0.999, eps=1e-7, fp32_betas=False):
         self.lr, self.b1, self.b2, self.eps = lr, beta1, beta2, eps
+        self.fp32_betas = fp32_betas
         self.t = 0
         self.m = None
         self.v = None
@@ -177,10 +184,13 @@ class KerasAdam:
             self.v = [np.zeros_like(a) for a in w]
         self.t += 1
         lr_t = dt(self.lr * np.sqrt(1.0 - self.b2 ** self.t) / (1.0 - self.b1 ** self.t))
+        b1, b2 = self.b1, self.b2
+        if self.fp32_betas:                          # 1 - b is then exact in fp64 (Sterbenz)
+            b1, b2 = float(np.float32(b1)), float(np.float32(b2))
         out = []
         for i, (a, ga) in enumerate(zip(w, g)):
-            self.m[i] = dt(self.b1) * self.m[i] + dt(1.0 - self.b1) * ga
-            self.v[i] = dt(self.b2) * self.v[i] + dt(1.0 - self.b2) * ga * ga
+            self.m[i] = dt(b1) * self.m[i] + dt(1.0 - b1) * ga
+            self.v[i] = dt(b2) * self.v[i] + dt(1.0 - b2) * ga * ga
             out.append(a - lr_t * self.m[i] / (np.sqrt(self.v[i]) + dt(self.eps)))
         return out
 

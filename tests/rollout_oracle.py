@@ -7,9 +7,18 @@ pieces that let the fp64 oracle (oracle/rpbcac_oracle.py) follow the Trainer's d
                          their Philox counters (also used to check that the streams never share a counter);
   default_perm_source    the Trainer's own mini-batch shuffles (perm_source=None);
   oracle_agents_from_trainer / trainer_rows
-                         oracle agents and buffer rows read back from a Trainer.
+                         oracle agents and buffer rows read back from a Trainer;
+  oracle_rollout / check_rows
+                         the oracle's rollout of a block on restated draws, and the exact row comparison with ties
+                         excluded;
+  round_perms / reassociated / with_kernel_adam / yardstick_rounds / yardstick / parallel_map
+                         the fp32-spread yardstick of whole update rounds at the reference hyper-parameters.
 
 Philox4x32-10 itself is attack_oracle.philox4x32_10 (integer-exact, checked against the Random123 known answers)."""
+import os
+from concurrent.futures import ProcessPoolExecutor
+import multiprocessing
+
 import numpy as np
 
 from attack_oracle import philox4x32_10
@@ -129,3 +138,176 @@ def trainer_rows(tr, t0, t1):
     ns = tr.ns[lo:hi].view(-1, NA, 2)[:, :n].cpu().numpy()
     r = tr.r[lo:hi].view(-1, NA, 1)[:, :n].cpu().numpy()
     return sa[:, :, :2].copy(), ns, sa[:, :, 2:].copy(), r
+
+
+def oracle_rollout(agents, desired, nrow, ncol, draws, gamma, mu=0.1, scaling=True):
+    """O.rollout_block on the restated draws; every agent logs est (the kernel computes it for all agents)."""
+    init, U = draws
+    n_ep, L_, N, n = U.shape[:4]
+    env = O.GridWorldOracle(nrow, ncol, n, desired, n_envs=N, scaling=scaling)
+    S, NS, A, Rw, est, ret = O.rollout_block(env, agents, ["Cooperative"] * n, n_episodes=n_ep, max_ep_len=L_,
+                                             gamma=gamma, init_states=init, uniforms=U, mu=mu)
+    return (S, NS, A, Rw), est, ret
+
+
+def check_rows(got, want, n_ep, L_, N):
+    """got / want: (s, ns, a, r) of n_ep episodes x L_ steps x N environments.  -> ok[n_ep, N]: episodes free of ties,
+    whose rows must then be exactly the oracle's."""
+    act_equal = got[2][..., 0] == want[2][..., 0]
+    assert act_equal.mean() > 0.999, act_equal.mean()
+    ok = np.ones((n_ep, N), bool)
+    for row, _ in np.argwhere(~act_equal):
+        t, e = divmod(row, N)
+        ok[t // L_, e] = False
+    assert ok.mean() > 0.9, ok.mean()
+    mask = np.repeat(ok, L_, axis=0).reshape(-1)
+    for g, w, name in zip(got, want, ("s", "ns", "a", "r")):
+        assert np.array_equal(g[mask], np.asarray(w, np.float32)[mask]), name
+    return ok
+
+
+# ------------------------------------------------------------------------------------------ the fp32-spread yardstick
+# Measured on an H100 (the cases of test_reference_scale_gpu.py): ||gpu - o64|| / s up to 5.5 normwise and 7.1 in the
+# max norm over weights and Adam slots; c = 4 failed on those.
+YARD_C = 8.0            # ||gpu - o64|| may be this many times the fp32 spread s ...
+YARD_C_INF = 12.0       # ... (max |gpu - o64| this many times s_inf) ...
+YARD_FLOOR = 1e-6       # ... or of YARD_FLOOR x ||o64||, whichever is larger
+
+
+def round_perms(perm_source, labels, T, *, n_epochs, n_actor_steps):
+    """The time-row permutations one O.update_round draws from perm_source, in its draw order: per epoch 20 per Greedy
+    and 30 per Malicious agent (10 per mini-batch fit), then one actor window's per non-cooperative agent."""
+    n_fit = n_epochs * sum({"Greedy": 20, "Malicious": 30}.get(lab, 0) for lab in labels)
+    n_act = sum(lab != "Cooperative" for lab in labels)
+    return [np.asarray(perm_source(T)) for _ in range(n_fit)] + \
+        [np.asarray(perm_source(min(n_actor_steps, T))) for _ in range(n_act)]
+
+
+def reassociated(buf, perms, *, n_envs, n_actor_steps, n_act, mb_times=32, actor_mb_times=200):
+    """The same update round with another summation order: the buffer's time rows reversed inside the part before the
+    actor window and inside the window, its environments reversed inside every time row, and the permutations mapped
+    so that each mini-batch holds the same rows, in reverse order.  The last n_act permutations are the actor
+    windows'.  Every sum sees the same terms, so only the rounding changes."""
+    N = n_envs
+    T = buf[0].shape[0] // N
+    Ta = min(n_actor_steps, T)
+    rho = np.concatenate([np.arange(T - Ta)[::-1], T - Ta + np.arange(Ta)[::-1]])    # an involution of the time rows
+    rows = (rho[:, None] * N + np.arange(N)[::-1][None, :]).reshape(-1)
+
+    def flipped(p, mb):
+        q = np.array(p)
+        for k in range(0, len(q), mb):
+            q[k:k + mb] = q[k:k + mb][::-1].copy()
+        return q
+    n_fit = len(perms) - n_act
+    return (tuple(np.ascontiguousarray(x[rows]) for x in buf),
+            [flipped(rho[p], mb_times) for p in perms[:n_fit]] +
+            [flipped(Ta - 1 - np.asarray(p), actor_mb_times) for p in perms[n_fit:]])
+
+
+def with_kernel_adam(agents):
+    """agents whose Keras Adam uses the kernel's float32 constants (O.KerasAdam fp32_betas): rcmarl_adam_apply forms
+    1 - 0.999 as 1.f - 0.999f, 1.3e-5 below 0.001, which puts every Adam v 1.3e-5 relative away from the exact
+    constant's -- a fixed difference of the formula, not rounding, so the yardstick's oracle rounds use it."""
+    for ag in agents:
+        ag.adam.fp32_betas = True
+    return agents
+
+def _oracle_round(agents, labels, in_nodes, buf, perms, kw):
+    left = list(perms)
+
+    def source(T):
+        p = left.pop(0)
+        assert len(p) == T
+        return p
+    loss = O.update_round(agents, labels, in_nodes, *buf, perm_source=source, **kw)
+    assert not left
+    return agents, loss
+
+
+def yardstick_rounds(rounds, *, workers=None):
+    """rounds: one dict per update round with the oracle agents at the Trainer's state before it in fp64 ("a64") and
+    twice in fp32 ("a32", "a32b"), labels, in_nodes, the Trainer's buffer rows ("buf"), the permutations the Trainer
+    drew ("perms", round_perms) and the O.update_round keywords ("kw").  Runs the three oracle rounds of every entry:
+    fp64, fp32, and fp32 on reassociated(...).  They are independent, so they run in parallel worker processes.
+    Returns per round [(agents, losses) of fp64, fp32, fp32 reassociated]."""
+    jobs = []
+    for r in rounds:
+        kw = r["kw"]
+        n_act = sum(lab != "Cooperative" for lab in r["labels"])
+        alt_buf, alt_perms = reassociated(r["buf"], r["perms"], n_envs=kw["n_envs"], n_actor_steps=kw["n_actor_steps"],
+                                          n_act=n_act)
+        jobs += [(r["a64"], r["labels"], r["in_nodes"], r["buf"], r["perms"], kw),
+                 (r["a32"], r["labels"], r["in_nodes"], r["buf"], r["perms"], kw),
+                 (r["a32b"], r["labels"], r["in_nodes"], alt_buf, alt_perms, kw)]
+    out = parallel_map(_oracle_round, jobs, workers)
+    return [out[3 * k:3 * k + 3] for k in range(len(rounds))]
+
+
+def parallel_map(fn, jobs, workers=None):
+    """[fn(*args) for args in jobs] in spawned worker processes, each with one BLAS thread (the oracle's matrices are
+    small; the jobs, not the threads, fill the cores)."""
+    names = ("OMP_NUM_THREADS", "OPENBLAS_NUM_THREADS", "MKL_NUM_THREADS")
+    saved = {k: os.environ.get(k) for k in names}
+    os.environ.update({k: "1" for k in names})
+    try:
+        with ProcessPoolExecutor(workers or min(len(jobs), os.cpu_count() or 1),
+                                 mp_context=multiprocessing.get_context("spawn")) as ex:
+            return list(ex.map(fn, *zip(*jobs)))
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def round_tensors(agents):
+    """name -> array of the state an update round leaves: every agent's nets (actor, critic, TR, critic_local) and its
+    Keras-Adam m and v."""
+    out = {}
+    for i, ag in enumerate(agents):
+        for n, net in enumerate(ag.get_parameters()):
+            for k, x in enumerate(net):
+                out[f"agent {i} net {n} array {k}"] = x
+        for k in range(6):
+            out[f"agent {i} adam_m {k}"] = ag.adam.m[k]
+            out[f"agent {i} adam_v {k}"] = ag.adam.v[k]
+    return out
+
+
+def yardstick(got, o64, o32s, *, c=YARD_C, c_inf=YARD_C_INF, floor=YARD_FLOOR, msg=""):
+    """The fp32-spread yardstick.  For every tensor x of an update round (round_tensors: weights, Adam m and v), with o64 the fp64 oracle's and o32s the fp32 oracle's in two summation orders (yardstick_rounds):
+
+        s     = max over the fp32 runs of ||o32 - o64||          (Frobenius norm)
+        s_inf = max over the fp32 runs of max |o32 - o64|        (element-wise)
+        ||got - o64||       <= c x max(s,     floor x ||o64||)
+        max |got - o64|     <= c_inf x max(s_inf, floor x max |o64|)
+
+    At 10 epochs a fixed element-wise tolerance does not work: an fp32 restatement of the same maths already misses
+    fp64 by several times DESIGN.md's whole-round tolerance on some seeds, because ten epochs of consensus and
+    projection amplify rounding.  s is the rounding error of fp32 arithmetic on these very inputs, so a kernel must
+    stay within a few times of it.  (A scalar such as a loss gives s from a single error sample, too noisy for this;
+    losses keep the whole-round tolerance.)  Prints and returns the largest ||got - o64|| / max(s, floor ||o64||) and the median
+    ||o32 - o32b|| / s over the tensors: the second tells rounding (about 1) from a systematic fp32 / fp64 difference
+    (much less than 1)."""
+    rows, bad = [], []
+    for name, x in o64.items():
+        x = np.asarray(x, np.float64)
+        g = np.asarray(got[name], np.float64)
+        d = [np.asarray(o[name], np.float64) - x for o in o32s]
+        s, s_inf = max(np.linalg.norm(e) for e in d), max(np.abs(e).max() for e in d)
+        tol, tol_inf = max(s, floor * np.linalg.norm(x)), max(s_inf, floor * np.abs(x).max())
+        err, err_inf = np.linalg.norm(g - x), np.abs(g - x).max()
+        if not (err <= c * tol and err_inf <= c_inf * tol_inf):
+            bad.append(f"{name}: ||gpu - o64|| = {err:.3e} (max {err_inf:.3e}) > {c} x fp32 spread {tol:.3e} "
+                       f"(max: {c_inf} x {tol_inf:.3e})")
+        rows.append((name, err / tol if tol > 0 else 0.0, err_inf / tol_inf if tol_inf > 0 else 0.0,
+                     np.linalg.norm(d[0] - d[1]) / s if s > 0 else 0.0, err / max(np.linalg.norm(x), 1e-300)))
+    worst = max(rows, key=lambda row: row[1])
+    print(f"\n{msg}: largest ||gpu - o64|| / s = {worst[1]:.2f} ({worst[0]}); largest max-norm ratio "
+          f"{max(row[2] for row in rows):.2f}; median ||o32 - o32b|| / s = {np.median([row[3] for row in rows]):.2f}")
+    for row in sorted(rows, key=lambda row: -max(row[1], row[2]))[:4]:
+        print(f"    {row[0]}: {row[1]:.2f} / max-norm {row[2]:.2f}, ||gpu - o64|| / ||o64|| = {row[4]:.1e}")
+    assert not bad, f"{msg}: " + "; ".join(bad)
+    return worst[1], float(np.median([row[3] for row in rows]))

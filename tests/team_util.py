@@ -1,11 +1,14 @@
-"""Teams shared by the trainer parity tests (test_trainer_gpu.py, test_dp_single_gpu.py): 16-agent teams with several
-adversaries on the 10x10 grid with circulant in-neighbourhoods of 6, their fp64 oracle agents, seeded
-buffer rows, and the oracle side of update rounds whose shuffles the Trainer replays."""
+"""Teams shared by the trainer parity tests (test_trainer_gpu.py, test_dp_single_gpu.py, test_rollout_philox_gpu.py,
+test_reference_scale_gpu.py): 16-agent teams with several adversaries on the 10x10 grid with circulant
+in-neighbourhoods of 6, their fp64 oracle agents, seeded buffer rows, the oracle side of update rounds whose shuffles
+the Trainer replays, and the Trainer configurations of the default-loop tests (loop_team)."""
 import numpy as np
 
+from golden_util import pretrained
 from oracle import rpbcac_oracle as O
 
 C, M, G, F = 'Cooperative', 'Malicious', 'Greedy', 'Faulty'
+IN5 = [[0, 1, 2, 3], [1, 2, 3, 4], [2, 3, 4, 0], [3, 4, 0, 1], [4, 0, 1, 2]]
 TEAMS16 = {
     # 9 cooperative, 4 malicious, 2 greedy, 1 faulty agents: 4 x 3 + 2 x 2 = 16 mini-batch chains
     "M16": [C, M, C, G, C, M, C, F, C, M, C, G, C, M, C, C],
@@ -30,6 +33,26 @@ def team16(name, rs):
         if labels[i] == M:
             w[i].append(nets.glorot_uniform(32, 1, local))
     return labels, in_nodes, w, desired, [i % 3 for i in range(NA)], [0.01 + 0.001 * (i % 4) for i in range(NA)]
+
+
+def loop_team(name):
+    """Trainer keywords (team, grid, H, fast_lr) of the default-loop tests: "c2" (the pretrained C2 team),
+    "greedy_faulty" (its weights with agents 3, 4 Greedy and Faulty, common_reward), "M16" (team16) and any other name a
+    padded 3-agent team on the 5-agent instantiation, 4 x 6 grid."""
+    w, desired, labels = pretrained()
+    if name == "c2":
+        return dict(labels=labels, in_nodes=IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, fast_lr=0.01)
+    if name == "greedy_faulty":
+        return dict(labels=[C, C, C, G, F], in_nodes=IN5, weights=[x[:3] for x in w], desired=desired, nrow=5, ncol=5,
+                    H=1, fast_lr=0.01, common_reward=True)
+    if name == "M16":
+        labels, in_nodes, w16, des, H, fast = team16("M16", np.random.RandomState(31))
+        return dict(labels=labels, in_nodes=in_nodes, weights=w16, desired=des, nrow=10, ncol=10, H=H, fast_lr=fast)
+    rs = np.random.RandomState(7)                                         # 3 agents on the 5-agent instantiation
+    from rcmarl import nets
+    w3 = [[nets.glorot_uniform(6, 5, rs), nets.glorot_uniform(6, 1, rs), nets.glorot_uniform(9, 1, rs)] for _ in range(3)]
+    return dict(labels=[C, C, M], in_nodes=[[0, 1, 2], [1, 2, 0], [2, 0, 1]], weights=w3,
+                desired=np.array([[1, 2], [3, 5], [0, 0]]), nrow=4, ncol=6, H=1, fast_lr=0.01)
 
 
 def oracle_agents(labels, w, H, fast, gamma, slow_lr=0.002):

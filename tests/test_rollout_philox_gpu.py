@@ -27,8 +27,7 @@ from oracle import rpbcac_oracle as O                 # noqa: E402  (checker onl
 
 f64 = np.float64
 NAN = float("nan")
-C, M, G, F = "Cooperative", "Malicious", "Greedy", "Faulty"
-IN5 = [[0, 1, 2, 3], [1, 2, 3, 4], [2, 3, 4, 0], [3, 4, 0, 1], [4, 0, 1, 2]]
+C = "Cooperative"
 SEED2 = 0x9E3779B97F4A7C15                            # both key words non-zero
 N_EP, LEN = 3, 7
 
@@ -44,32 +43,6 @@ def rows_of(sa, ns, r, NA, nact, t0, t1, N):
     sa = sa[t0 * N:t1 * N].view(-1, NA, 3)[:, :nact].cpu().numpy()
     return (sa[:, :, :2], ns[t0 * N:t1 * N].view(-1, NA, 2)[:, :nact].cpu().numpy(), sa[:, :, 2:],
             r[t0 * N:t1 * N].view(-1, NA, 1)[:, :nact].cpu().numpy())
-
-
-def check_rows(got, want, n_ep, L_, N):
-    """got / want: (s, ns, a, r) of n_ep episodes x L_ steps x N environments.  -> ok[n_ep, N]: episodes free of ties,
-    whose rows must then be exactly the oracle's."""
-    act_equal = got[2][..., 0] == want[2][..., 0]
-    assert act_equal.mean() > 0.999, act_equal.mean()
-    ok = np.ones((n_ep, N), bool)
-    for row, _ in np.argwhere(~act_equal):
-        t, e = divmod(row, N)
-        ok[t // L_, e] = False
-    assert ok.mean() > 0.9, ok.mean()
-    mask = np.repeat(ok, L_, axis=0).reshape(-1)
-    for g, w, name in zip(got, want, ("s", "ns", "a", "r")):
-        assert np.array_equal(g[mask], np.asarray(w, np.float32)[mask]), name
-    return ok
-
-
-def oracle_rollout(agents, desired, nrow, ncol, draws, gamma, mu=0.1, scaling=True):
-    """O.rollout_block on the restated draws; every agent logs est (the kernel computes it for all agents)."""
-    init, U = draws
-    n_ep, L_, N, n = U.shape[:4]
-    env = O.GridWorldOracle(nrow, ncol, n, desired, n_envs=N, scaling=scaling)
-    S, NS, A, Rw, est, ret = O.rollout_block(env, agents, [C] * n, n_episodes=n_ep, max_ep_len=L_, gamma=gamma,
-                                             init_states=init, uniforms=U, mu=mu)
-    return (S, NS, A, Rw), est, ret
 
 
 # --------------------------------------------------------------------------------------------------- (a), (b) kernel
@@ -146,8 +119,8 @@ def test_philox_launch_matches_oracle(K, case):
     got = launch(K, case, st, injected=False)
     agents = [O.RPBCACOracleAgent(st["actors"][i], st["critics"][i], rand_net(np.random.RandomState(i), 3 * nact, 1),
                                   0.002, 0.01, 0.9, dtype=f64) for i in range(nact)]
-    want, est, ret = oracle_rollout(agents, st["desired"], nrow, ncol, st["draws"], 0.9, mu, st["scaling"])
-    ok = check_rows(rows_of(got["sa"], got["ns"], got["r"], NA, nact, tb, tb + N_EP * LEN, N), want, N_EP, LEN, N)
+    want, est, ret = R.oracle_rollout(agents, st["desired"], nrow, ncol, st["draws"], 0.9, mu, st["scaling"])
+    ok = R.check_rows(rows_of(got["sa"], got["ns"], got["r"], NA, nact, tb, tb + N_EP * LEN, N), want, N_EP, LEN, N)
     block = slice(tb * N, (tb + N_EP * LEN) * N)
     for name in ("sa", "ns", "r"):
         x = got[name][block].view(N_EP * LEN * N, NA, -1)[:, nact:]
@@ -167,14 +140,14 @@ def test_bench_first_block_matches_oracle(K):
     from rcmarl.trainer import Trainer
     w, desired, labels = pretrained()
     N, n_ep, L_ = 4096, 50, 20
-    tr = Trainer(labels=labels, in_nodes=IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, n_envs=N, gamma=0.9,
+    tr = Trainer(labels=labels, in_nodes=T16.IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, n_envs=N, gamma=0.9,
                  fast_lr=0.01, slow_lr=0.002, max_ep_len=L_, n_ep_fixed=n_ep, n_epochs=10, buffer_size=2000, seed=1234)
     est_m, ret_m = tr.rollout_block()
     agents = [O.RPBCACOracleAgent(w[i][0], w[i][1], w[i][2], 0.002, 0.01, 0.9, dtype=f64) for i in range(5)]
     draws = R.rollout_draws(1234, env_offset=0, n_envs=N, episode_offset=0, n_episodes=n_ep, max_ep_len=L_, n_slots=5,
                             n_active=5, nrow=5, ncol=5)
-    want, est, ret = oracle_rollout(agents, desired, 5, 5, draws, 0.9)
-    ok = check_rows(R.trainer_rows(tr, 0, n_ep * L_), want, n_ep, L_, N)
+    want, est, ret = R.oracle_rollout(agents, desired, 5, 5, draws, 0.9)
+    ok = R.check_rows(R.trainer_rows(tr, 0, n_ep * L_), want, n_ep, L_, N)
     close(est_m, est.mean(1), rtol=1e-5, atol=3e-6)
     full = ok.all(1)                                                      # episodes without a tie in any environment
     assert full.mean() > 0.5, full.mean()
@@ -186,23 +159,6 @@ LOOP = dict(gamma=0.9, max_ep_len=5, n_ep_fixed=4, n_epochs=2, buffer_size=30, s
 LOOP_SEED = 11          # the fp32 oracle stays within 1 % of the whole-round tolerance on every team below
 
 
-def loop_team(name):
-    w, desired, labels = pretrained()
-    if name == "c2":
-        return dict(labels=labels, in_nodes=IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, fast_lr=0.01)
-    if name == "greedy_faulty":
-        return dict(labels=[C, C, C, G, F], in_nodes=IN5, weights=[x[:3] for x in w], desired=desired, nrow=5, ncol=5,
-                    H=1, fast_lr=0.01, common_reward=True)
-    if name == "M16":
-        labels, in_nodes, w16, des, H, fast = T16.team16("M16", np.random.RandomState(31))
-        return dict(labels=labels, in_nodes=in_nodes, weights=w16, desired=des, nrow=10, ncol=10, H=H, fast_lr=fast)
-    rs = np.random.RandomState(7)                                         # 3 agents on the 5-agent instantiation
-    from rcmarl import nets
-    w3 = [[nets.glorot_uniform(6, 5, rs), nets.glorot_uniform(6, 1, rs), nets.glorot_uniform(9, 1, rs)] for _ in range(3)]
-    return dict(labels=[C, C, M], in_nodes=[[0, 1, 2], [1, 2, 0], [2, 0, 1]], weights=w3,
-                desired=np.array([[1, 2], [3, 5], [0, 0]]), nrow=4, ncol=6, H=1, fast_lr=0.01)
-
-
 @pytest.mark.parametrize("name,N", [("c2", 1), ("c2", 64), ("greedy_faulty", 16), ("M16", 8), ("team3_4x6", 16)])
 def test_default_training_loop_matches_oracle(K, name, N):
     """(d) Three rollout blocks + update rounds of a Trainer with no injected draws, rows or shuffles, buffer_size =
@@ -212,7 +168,7 @@ def test_default_training_loop_matches_oracle(K, name, N):
     Trainer's own shuffles (default_perm_source) must give its weights and losses; the kept buffer must be the newest
     buffer_size time rows."""
     from rcmarl.trainer import Trainer
-    team = loop_team(name)
+    team = T16.loop_team(name)
     n = len(team["labels"])
     tr = Trainer(**team, n_envs=N, seed=LOOP_SEED, **LOOP)
     L_, ne, block = LOOP["max_ep_len"], LOOP["n_ep_fixed"], LOOP["max_ep_len"] * LOOP["n_ep_fixed"]
@@ -224,8 +180,8 @@ def test_default_training_loop_matches_oracle(K, name, N):
                                 max_ep_len=L_, n_slots=tr.NA, n_active=n, nrow=team["nrow"], ncol=team["ncol"])
         t0 = tr.t_filled
         est_m, ret_m = tr.rollout_block()
-        want, est, ret = oracle_rollout(agents, team["desired"], team["nrow"], team["ncol"], draws, LOOP["gamma"])
-        ok = check_rows(R.trainer_rows(tr, t0, t0 + block), want, ne, L_, N)
+        want, est, ret = R.oracle_rollout(agents, team["desired"], team["nrow"], team["ncol"], draws, LOOP["gamma"])
+        ok = R.check_rows(R.trainer_rows(tr, t0, t0 + block), want, ne, L_, N)
         close(est_m, est.mean(1), rtol=1e-5, atol=3e-6, err_msg=f"round {k} est")
         full = ok.all(1)
         close(ret_m[full], ret[full].mean(1), rtol=1e-5, atol=1e-5, err_msg=f"round {k} ret")
@@ -255,7 +211,7 @@ def test_train_rpbcac_sim_data_matches_oracle(K, n_envs):
     from rcmarl import api
     import training.train_agents as training
     w, desired, labels = pretrained()
-    cfg = dict(labels=labels, in_nodes=IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, n_envs=n_envs, gamma=0.9,
+    cfg = dict(labels=labels, in_nodes=T16.IN5, weights=w, desired=desired, nrow=5, ncol=5, H=1, n_envs=n_envs, gamma=0.9,
                fast_lr=0.01, slow_lr=0.002, max_ep_len=6, n_ep_fixed=8, n_epochs=2, buffer_size=96)
     env, agents, args = api.build_reference_objects(cfg)
     ne, L_ = cfg["n_ep_fixed"], cfg["max_ep_len"]
@@ -269,8 +225,8 @@ def test_train_rpbcac_sim_data_matches_oracle(K, n_envs):
         ags = [O.RPBCACOracleAgent(ws[i][0], ws[i][1], ws[i][2], 0.002, 0.01, 0.9, dtype=f64) for i in range(5)]
         draws = R.rollout_draws(tr.seed, env_offset=0, n_envs=n_envs, episode_offset=ep0, n_episodes=n_ep, max_ep_len=L_,
                                 n_slots=5, n_active=5, nrow=5, ncol=5)
-        want, est, ret = oracle_rollout(ags, desired, 5, 5, draws, 0.9)
-        ok = check_rows(R.trainer_rows(tr, ep0 * L_, (ep0 + n_ep) * L_), want, n_ep, L_, n_envs)
+        want, est, ret = R.oracle_rollout(ags, desired, 5, 5, draws, 0.9)
+        ok = R.check_rows(R.trainer_rows(tr, ep0 * L_, (ep0 + n_ep) * L_), want, n_ep, L_, n_envs)
         assert ok.all()
         est, ret = est.mean(1), ret.mean(1)
         return np.stack([ret[:, coop].sum(1) / len(coop), ret[:, adv].sum(1) / len(adv), est[:, coop].mean(1)], 1)
