@@ -155,6 +155,52 @@ typedef struct {
 } rcmarl_attack_job;
 int rcmarl_attack(const rcmarl_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* Distance-based resilient aggregation of whole messages (rcmarl_vector_aggregate).  The rules above are coordinate-wise;
+ * these compare the in-neighbours' messages as vectors.  One job: its n = n_in messages x_k = msgs + in_nodes[k] *
+ * msg_stride, k = 0 .. n-1 (k = 0 is the receiver's own; repeats in in_nodes count), each of P = job.n packed
+ * parameters (the whole network, hidden layers and head).  In fp32:
+ *   D_kl = sum_p (x_k,p - x_l,p)^2,   d_k(z) = sqrt(sum_p (x_k,p - z_p)^2);
+ * a distance that is not finite (overflow, e.g. a message of 1e30, or +-inf) counts as +inf.  Every rule outputs
+ *   out = sum_k w_k x_k,   w_k >= 0,   sum_k w_k = 1,
+ * and writes w to weights_out when it is not NULL.
+ *   KRUM    (Blanchard et al., NeurIPS 2017)  n >= H + 3.  score_k = the sum of the n - H - 2 smallest D_kl over l != k,
+ *   MKRUM   added in ascending order.  The m smallest scores are selected (ties to the lower index), m = 1 for KRUM and
+ *           m = n - H for MKRUM (multi-Krum); out = (sum over the selected k, index order, of x_k) / m, w_k = 1/m or 0.
+ *   SCCLIP  self-centred clipping (after He, Karimireddy & Jaggi 2022, ClippedGossip).  The clipping radius is set by H,
+ *           not by the paper's adaptive rule (this library's choice): d_k = d_k(x_0) for k >= 1, tau = the (H+1)-th
+ *           largest d_k (0 if H >= n - 1), c_k = 0 if d_k is not finite, 1 if d_k <= tau, tau / d_k otherwise;
+ *           out = x_0 + (sum_{k>=1, index order, c_k != 0} c_k (x_k - x_0)) / n, w_k = c_k / n (k >= 1),
+ *           w_0 = 1 - sum_{k>=1} w_k.  H = 0 gives the plain mean.
+ *   GMED    geometric median by smoothed Weiszfeld (Pillutla et al., RFA).  z^0 = the coordinate-wise median (TRIM at
+ *           H' = (n-1)/2); then RCMARL_GMED_ITERS times: beta_k = 0 if d_k(z) is not finite, else
+ *           1 / max(d_k(z), RCMARL_GMED_NU), z <- (sum_k beta_k x_k) / sum_k beta_k (index order, beta_k = 0 terms
+ *           skipped); out = the last z, w_k = the last beta_k / sum beta.  If no distance is finite, beta = (1, 0, ...):
+ *           out = x_0.  H is not used (0 <= H < n).
+ * NaN inputs are not supported.  At most H messages of 1e30 or +-inf get weight 0 (KRUM / MKRUM: while n >= 2H + 3;
+ * GMED: while 2H < n).  One CTA per job, fixed summation orders, no atomics: bitwise reproducible, independent of the
+ * job order and of how jobs are split over launches.  dst[0:n] = out.  Refused (RCMARL_ERR_ARG, nothing launched, dst
+ * and weights_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_in outside
+ * 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, an unknown rule, H outside [0, n_in), KRUM / MKRUM with n_in < H + 3,
+ * (n_in + 1) * n > RCMARL_VECTOR_MAX_FLOATS (the messages are staged in shared memory), a dst or weights_out that
+ * overlaps an in-node row of any job of the launch, and two written ranges (dsts, weights_outs) of the launch that
+ * overlap. */
+#define RCMARL_GMED_ITERS 8
+#define RCMARL_GMED_NU 1e-6f
+#define RCMARL_VECTOR_MAX_FLOATS (48 * 1024)
+typedef enum { RCMARL_VEC_KRUM = 0, RCMARL_VEC_MKRUM = 1, RCMARL_VEC_SCCLIP = 2, RCMARL_VEC_GMED = 3 } rcmarl_vector_rule;
+typedef struct {
+    float* dst;                 /* the aggregate (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    float* weights_out;         /* optional [n_in]: w_k */
+    int32_t n;                  /* parameters per message */
+    int32_t n_in;
+    int32_t H;
+    int32_t rule;               /* rcmarl_vector_rule */
+    int32_t in_nodes[RCMARL_MAX_NEIGHBOURS];
+} rcmarl_vector_job;
+int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

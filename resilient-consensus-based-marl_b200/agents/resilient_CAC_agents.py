@@ -4,7 +4,8 @@ mfigura/Resilient-consensus-based-MARL), executed by the sm_90a kernels of librc
 Same constructor and method names, argument meaning and mutation conventions as the reference (SURVEY.md 8b):
   *_update_local            return (message copy, loss) and leave the agent's own networks untouched (:113,120)
   resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166), or
-                                 their trimmed / W-MSR mean with aggregation="trim" / "wmsr"
+                                 their trimmed / W-MSR mean with aggregation="trim" / "wmsr", or the hidden layers
+                                 of a distance-based aggregate ("krum", "mkrum", "scclip", "gmed") of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
@@ -27,8 +28,10 @@ class RPBCAC_agent():
         self.gamma = gamma
         self.H = H
         # resilient aggregation rule of every consensus step: "clip" (the reference's), "trim" or "wmsr"
-        # (include/rcmarl.h, rcmarl_agg_rule)
-        L.agg_rule(aggregation)
+        # (include/rcmarl.h, rcmarl_agg_rule), or a distance-based rule over whole messages: "krum", "mkrum", "scclip"
+        # or "gmed" (rcmarl_vector_rule)
+        if not L.is_vector_rule(aggregation):
+            L.agg_rule(aggregation)
         self.aggregation = aggregation
         self.n_actions = self.actor.output_shape[1]
         self.fast_lr = fast_lr
@@ -43,7 +46,9 @@ class RPBCAC_agent():
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
         v = v.reshape(v.shape[0], -1)
-        if L.agg_rule(self.aggregation) == L.AGG_CLIP:
+        if L.is_vector_rule(self.aggregation):    # the rows as whole vectors: out = sum_k w_k v_k
+            out = self._with_aggregate(v)[-1]
+        elif L.agg_rule(self.aggregation) == L.AGG_CLIP:
             out = ops.clip_mean(v, self.H)
         else:                         # the other rules: one consensus job over all P coordinates of the n rows
             L.check_aggregation(self.aggregation, self.H, v.shape[0])
@@ -51,6 +56,21 @@ class RPBCAC_agent():
             ops.consensus_hidden([ops.consensus_job(out, v, v.shape[1], v.shape[1], list(range(v.shape[0])), self.H,
                                                     self.aggregation)])
         return Tensor(out.reshape(shape))
+
+    def _with_aggregate(self, stack):
+        """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based rule."""
+        n, P = stack.shape
+        L.check_vector_rule(self.aggregation, self.H, n)
+        out = torch.cat([stack, torch.empty(1, P, dtype=stack.dtype, device=stack.device)])
+        ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
+        return out
+
+    def _consensus_inputs(self, stack):
+        """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
+        distance-based rule's aggregate becomes the single in-node under clip, which returns it exactly, as in Trainer."""
+        if L.is_vector_rule(self.aggregation):
+            return self._with_aggregate(stack), [stack.shape[0]], 0, "clip"
+        return stack, list(range(stack.shape[0])), self.H, self.aggregation
 
     # ------------------------------------------------------------------ projection step (:60-84)
     def _team(self, model, x, agg):
@@ -88,9 +108,9 @@ class RPBCAC_agent():
     # ------------------------------------------------------------------ hidden-layer consensus (:142-166)
     def _hidden(self, model, msgs_innodes):
         dev = model.flat.device
-        stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
+        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]))
         ops.consensus_hidden([ops.consensus_job(model.flat, stack, stack.shape[1], nets.n_hidden_params(model.d_in_k),
-                                                list(range(len(msgs_innodes))), self.H, self.aggregation)])
+                                                nodes, H, rule)])
 
     def resilient_consensus_critic_hidden(self, critic_weights_innodes):
         self._hidden(self.critic, critic_weights_innodes)
@@ -102,10 +122,9 @@ class RPBCAC_agent():
     def _estimates(self, model, x, msgs_innodes):
         rows, kind, xf = A.rows_for(x, self.n_agents)
         dev = xf.device
-        stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
+        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]))
         agg = torch.empty(xf.shape[0], dtype=torch.float32, device=dev)
-        ops.team(rows, [ops.team_job(model.flat, kind, stack, stack.shape[1], list(range(len(msgs_innodes))), self.H,
-                                     agg_out=agg, rule=self.aggregation)])
+        ops.team(rows, [ops.team_job(model.flat, kind, stack, stack.shape[1], nodes, H, agg_out=agg, rule=rule)])
         return Tensor(agg.reshape(-1, 1))
 
     def resilient_consensus_critic(self, s, critic_weights_innodes):

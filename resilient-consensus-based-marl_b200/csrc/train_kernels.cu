@@ -9,6 +9,8 @@
 //                   deterministic two-level reduction (CTA partials -> reduce_kernel).
 //   team_kernel     K5+K6  neighbour-head estimates, clipped mean, projection numerators
 //   attack_kernel   Byzantine messages crafted per receiver (ALIE / IPM / Gaussian, rcmarl_attack)
+//   vector_agg_kernel  distance-based rules over whole messages (Krum, multi-Krum, self-centred clipping, geometric
+//                   median; rcmarl_vector_aggregate)
 //   consensus, sgd/adam apply, reward mix: the small glue kernels.
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
@@ -368,6 +370,180 @@ __global__ void __launch_bounds__(256) attack_kernel(const __grid_constant__ Att
         m = mu + job.param * (sqrtf(-2.f * logf(u1)) * cospif(2.f * u2));
     }
     job.dst[i] = m;
+}
+
+// Distance-based rules over whole messages (rcmarl_vector_aggregate, include/rcmarl.h): one CTA of 256 threads per job.
+// The n_in messages are staged in shared memory; every distance is summed by ONE warp (lane-strided partials, then the
+// fixed xor butterfly of warp_sum), so its value does not depend on which warp takes it.  Scores, order statistics and
+// weights for n_in <= 16 run on warp 0, one lane per message, on registers and shared memory (no local arrays); the
+// output takes one thread per coordinate and adds the messages in index order.
+struct VectorParams { rcmarl_vector_job jobs[RCMARL_MAX_JOBS]; };
+constexpr int VEC_THREADS = 256;
+
+// squared distance of two shared-memory vectors of n floats, in every lane of the calling warp; not finite -> +inf
+__device__ __forceinline__ float warp_sqdist(const float* a, const float* b, int n, int lane) {
+    float s = 0.f;
+    for (int p = lane; p < n; p += 32) {
+        const float d = a[p] - b[p];
+        s = fmaf(d, d, s);
+    }
+    s = warp_sum(s);
+    return isfinite(s) ? s : INFINITY;
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];    // KRUM / MKRUM: D_kl; SCCLIP: d_k in dist[k]
+    __shared__ float wt[MAXN];             // KRUM / MKRUM: w_k; SCCLIP: c_k; GMED: beta_k
+    __shared__ float score[MAXN];
+    __shared__ float total;                // GMED: sum beta
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in, H = job.H, rule = job.rule;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    constexpr int NW = VEC_THREADS / 32;
+    float* xs = smem;                              // [n_in][n]
+    float* z = smem + (int64_t)nin * n;            // GMED iterate [n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+
+    if (rule == RCMARL_VEC_KRUM || rule == RCMARL_VEC_MKRUM) {
+        for (int t = warp; t < nin * (nin - 1) / 2; t += NW) {       // unordered pairs k < l
+            int k = 0, r = t;
+            while (r >= nin - 1 - k) { r -= nin - 1 - k; ++k; }
+            const int l = k + 1 + r;
+            const float d = warp_sqdist(xs + k * n, xs + l * n, n, lane);
+            if (lane == 0) { dist[k * MAXN + l] = d; dist[l * MAXN + k] = d; }
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const int k = lane, cnt = nin - H - 2, m = rule == RCMARL_VEC_KRUM ? 1 : nin - H;
+            if (k < nin) {
+                float v[MAXN];
+                int rk[MAXN];
+#pragma unroll
+                for (int l = 0; l < MAXN; ++l) v[l] = (l < nin && l != k) ? dist[k * MAXN + l] : 0.f;
+#pragma unroll
+                for (int l = 0; l < MAXN; ++l) {          // rank of D_kl among the l != k, ties to the lower index
+                    int r = 0;
+#pragma unroll
+                    for (int q = 0; q < MAXN; ++q)
+                        if (q < nin && q != k) r += (v[q] < v[l] || (v[q] == v[l] && q < l)) ? 1 : 0;
+                    rk[l] = (l < nin && l != k) ? r : MAXN;
+                }
+                float s = 0.f;
+#pragma unroll
+                for (int q = 0; q < MAXN - 1; ++q) {      // the cnt smallest, in ascending order
+                    if (q < cnt) {
+#pragma unroll
+                        for (int l = 0; l < MAXN; ++l)
+                            if (rk[l] == q) s += v[l];
+                    }
+                }
+                score[k] = s;
+            }
+            __syncwarp();
+            if (k < nin) {
+                const float sk = score[k];
+                int r = 0;
+#pragma unroll
+                for (int q = 0; q < MAXN; ++q)
+                    if (q < nin) r += (score[q] < sk || (score[q] == sk && q < k)) ? 1 : 0;
+                wt[k] = r < m ? 1.f / (float)m : 0.f;
+            }
+        }
+        __syncthreads();
+        const float fm = rule == RCMARL_VEC_KRUM ? 1.f : (float)(nin - H);
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            float s = 0.f;
+            for (int k = 0; k < nin; ++k)
+                if (wt[k] != 0.f) s += xs[k * n + p];
+            job.dst[p] = s / fm;
+        }
+    } else if (rule == RCMARL_VEC_SCCLIP) {
+        for (int k = 1 + warp; k < nin; k += NW) {
+            const float d = sqrtf(warp_sqdist(xs + k * n, xs, n, lane));
+            if (lane == 0) dist[k] = d;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const int k = lane;
+            if (k >= 1 && k < nin && H < nin - 1) {       // tau = the d_k of descending rank H (ties to the lower index)
+                const float dk = dist[k];
+                int r = 0;
+                for (int q = 1; q < nin; ++q) r += (dist[q] > dk || (dist[q] == dk && q < k)) ? 1 : 0;
+                if (r == H) score[0] = dk;
+            }
+            __syncwarp();
+            const float tau = H < nin - 1 ? score[0] : 0.f;
+            if (k >= 1 && k < nin) {
+                const float dk = dist[k];
+                wt[k] = !isfinite(dk) ? 0.f : (dk <= tau ? 1.f : tau / dk);
+            }
+        }
+        __syncthreads();
+        const float fn = (float)nin;
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            const float x0 = xs[p];
+            float s = 0.f;
+            for (int k = 1; k < nin; ++k) {
+                const float c = wt[k];
+                if (c != 0.f) s = fmaf(c, xs[k * n + p] - x0, s);
+            }
+            job.dst[p] = x0 + s / fn;
+        }
+        __syncthreads();                                              // every c_k read
+        if (tid == 0) {
+            float sw = 0.f;
+            for (int k = 1; k < nin; ++k) {
+                wt[k] = wt[k] / fn;
+                sw += wt[k];
+            }
+            wt[0] = 1.f - sw;
+        }
+    } else {                                                          // GMED
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            float v[MAXN];
+#pragma unroll
+            for (int k = 0; k < MAXN; ++k) v[k] = k < nin ? xs[k * n + p] : 0.f;
+            z[p] = resilient_mean_small<MAXN>(v, nin, (nin - 1) / 2, RCMARL_AGG_TRIM);
+        }
+        for (int it = 0; it < RCMARL_GMED_ITERS; ++it) {
+            __syncthreads();                                          // z complete
+            for (int k = warp; k < nin; k += NW) {
+                const float d = sqrtf(warp_sqdist(xs + k * n, z, n, lane));
+                if (lane == 0) wt[k] = isfinite(d) ? 1.f / fmaxf(d, RCMARL_GMED_NU) : 0.f;
+            }
+            __syncthreads();
+            if (tid == 0) {
+                float s = 0.f;
+                for (int k = 0; k < nin; ++k) s += wt[k];
+                if (s == 0.f) { wt[0] = 1.f; s = 1.f; }               // no finite distance: out = x_0
+                total = s;
+            }
+            __syncthreads();
+            const float S = total;
+            float* out = it == RCMARL_GMED_ITERS - 1 ? job.dst : z;
+            for (int p = tid; p < n; p += VEC_THREADS) {
+                float s = 0.f;
+                for (int k = 0; k < nin; ++k) {
+                    const float b = wt[k];
+                    if (b != 0.f) s = fmaf(b, xs[k * n + p], s);
+                }
+                out[p] = s / S;
+            }
+        }
+        __syncthreads();                                              // every beta_k read
+        if (tid == 0)
+            for (int k = 0; k < nin; ++k) wt[k] = wt[k] / total;
+    }
+    if (job.weights_out) {
+        __syncthreads();
+        if (tid < nin) job.weights_out[tid] = wt[tid];
+    }
 }
 
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
@@ -837,6 +1013,65 @@ int rcmarl_attack(const rcmarl_attack_job* jobs, int n_jobs, void* stream) {
         if (q.n > maxn) maxn = q.n;
     }
     attack_kernel<<<dim3((maxn + 255) / 256, n_jobs), 256, 0, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+// [first, last) byte range of n floats at base + row * stride floats
+static void float_range(const float* base, int64_t row, int64_t stride, int64_t n, uintptr_t& first, uintptr_t& last) {
+    first = (uintptr_t)base + (uintptr_t)(row * stride * (int64_t)sizeof(float));
+    last = first + (uintptr_t)(n * (int64_t)sizeof(float));
+}
+
+int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.rule < RCMARL_VEC_KRUM || q.rule > RCMARL_VEC_GMED || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+        if ((q.rule == RCMARL_VEC_KRUM || q.rule == RCMARL_VEC_MKRUM) && q.n_in < q.H + 3) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_in + 1) * q.n;
+        if (floats > RCMARL_VECTOR_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // The CTAs stage their inputs before anything is written, but the CTAs of other jobs run concurrently: no written
+    // range (a dst, a weights_out) may overlap an in-node row of any job of the launch or another written range.
+    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (jobs[j].weights_out) {
+            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
+            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
+    }
+    for (int a = 0; a < n_w; ++a) {
+        for (int b = a + 1; b < n_w; ++b)
+            if (w0[a] < w1[b] && w0[b] < w1[a]) return RCMARL_ERR_ARG;
+        for (int r = 0; r < n_r; ++r)
+            if (w0[a] < r1[r] && r0[r] < w1[a]) return RCMARL_ERR_ARG;
+    }
+    // The kernel also has static shared memory, so the default 48 KB limit applies to static + dynamic: opt in to the
+    // largest staging size, once per device, before the first launch there (independent of any other launch).
+    static bool opted[64] = {};
+    int dev = 0;
+    RC_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64 || !opted[dev]) {
+        RC_CUDA(cudaFuncSetAttribute(vector_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * RCMARL_VECTOR_MAX_FLOATS)));
+        if (dev >= 0 && dev < 64) opted[dev] = true;
+    }
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    vector_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

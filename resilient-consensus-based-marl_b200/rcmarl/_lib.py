@@ -26,6 +26,11 @@ AGG_CLIP, AGG_TRIM, AGG_WMSR = 0, 1, 2            # rcmarl_agg_rule
 AGG_RULES = {"clip": AGG_CLIP, "trim": AGG_TRIM, "wmsr": AGG_WMSR}
 ATTACK_ALIE, ATTACK_IPM, ATTACK_GAUSS = 0, 1, 2   # rcmarl_attack_kind
 ATTACKS = {"alie": ATTACK_ALIE, "ipm": ATTACK_IPM, "gauss": ATTACK_GAUSS}
+VEC_KRUM, VEC_MKRUM, VEC_SCCLIP, VEC_GMED = 0, 1, 2, 3   # rcmarl_vector_rule
+VECTOR_RULES = {"krum": VEC_KRUM, "mkrum": VEC_MKRUM, "scclip": VEC_SCCLIP, "gmed": VEC_GMED}
+GMED_ITERS = 8
+GMED_NU = 1e-6
+VECTOR_MAX_FLOATS = 48 * 1024
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -44,6 +49,11 @@ class AttackJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("n", C.c_int32), ("n_honest", C.c_int32),
                 ("honest", C.c_int32 * MAX_NEIGHBOURS), ("kind", C.c_int32), ("param", C.c_float), ("seed", C.c_uint64),
                 ("attacker", C.c_uint32), ("receiver", C.c_uint32), ("round", C.c_uint32), ("epoch", C.c_uint32)]
+
+
+class VectorJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("weights_out", c_fp), ("n", C.c_int32),
+                ("n_in", C.c_int32), ("H", C.c_int32), ("rule", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS)]
 
 
 class ValueJob(C.Structure):
@@ -98,6 +108,7 @@ SYMBOLS = [
     ("rcmarl_clip_mean", C.c_int, [c_fp, C.c_int, C.c_int64, C.c_int64, C.c_int, c_fp, c_fp]),
     ("rcmarl_consensus_hidden", C.c_int, [C.POINTER(ConsensusJob), C.c_int, c_fp]),
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
+    ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
@@ -171,6 +182,24 @@ def check_aggregation(rule, H, n_in):
         raise RcmarlError(f"aggregation {rule!r} with H={H} needs 0 <= H < n_in" + (" and 2H < n_in" if r == AGG_TRIM else "")
                           + f" (n_in={n_in}, at most {MAX_NEIGHBOURS})")
     return r
+
+
+def is_vector_rule(rule):
+    """True for the name of a distance-based rule (rcmarl_vector_rule): "krum", "mkrum", "scclip", "gmed"."""
+    return isinstance(rule, str) and rule in VECTOR_RULES
+
+
+def check_vector_rule(rule, H, n_in):
+    """Raise RcmarlError unless `rule` names a distance-based rule that allows H out of n_in messages
+    (include/rcmarl.h): 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in, for krum / mkrum also n_in >= H + 3.
+    Returns the rcmarl_vector_rule id."""
+    if not is_vector_rule(rule):
+        raise RcmarlError(f"unknown distance-based aggregation rule {rule!r}: expected one of {sorted(VECTOR_RULES)}")
+    krum = rule in ("krum", "mkrum")
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in) or (krum and n_in < H + 3):
+        raise RcmarlError(f"aggregation {rule!r} with H={H} needs 0 <= H < n_in" + (" and n_in >= H + 3" if krum else "")
+                          + f" (n_in={n_in}, at most {MAX_NEIGHBOURS})")
+    return VECTOR_RULES[rule]
 
 
 def check_attack(attack):

@@ -295,6 +295,29 @@ def attack(jobs):
     L.check(L.lib().rcmarl_attack(a, len(a), _stream()), "rcmarl_attack")
 
 
+def vector_job(dst, msgs, msg_stride, n, in_nodes, H, rule, weights_out=None):
+    """rule: distance-based rule name ("krum", "mkrum", "scclip", "gmed") or rcmarl_vector_rule id (include/rcmarl.h).
+    Names are checked here, ids and limits by the library."""
+    j = L.VectorJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.weights_out = ptr(weights_out)
+    j.n_in, j.H = len(in_nodes), H
+    for k, v in enumerate(in_nodes[:L.MAX_NEIGHBOURS]):
+        j.in_nodes[k] = v
+    if isinstance(rule, str):
+        if not L.is_vector_rule(rule):
+            raise L.RcmarlError(f"unknown distance-based aggregation rule {rule!r}: expected one of {sorted(L.VECTOR_RULES)}")
+        rule = L.VECTOR_RULES[rule]
+    j.rule = int(rule)
+    j._keep = (dst, msgs, weights_out)
+    return j
+
+
+def vector_aggregate(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_vector_aggregate(a, len(a), _stream()), "rcmarl_vector_aggregate")
+
+
 def reward_mix(r, agents, out=None, scale=1.0):
     """r: [rows, n_agents]; out[row] = scale * sum_k r[row, agents[k]] / len(agents) in list order."""
     n_rows, n_agents = r.shape

@@ -58,10 +58,20 @@ class Trainer:
         agg = [aggregation] * n_real if isinstance(aggregation, (str, int)) else list(aggregation)
         if len(agg) != n_real:
             raise L.RcmarlError("aggregation must be one rule or one rule per agent")
-        self.aggregation = [L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
+        # A distance-based rule ("krum", "mkrum", "scclip", "gmed") aggregates whole messages into one extra message row
+        # per such agent; its consensus and team jobs then read that row as their only in-node under clip, which returns
+        # it exactly (the projection target phi.W3 + b3 is linear in the head).
+        self.vector_rule = [L.VECTOR_RULES[a] if L.is_vector_rule(a) else None for a in agg] + [None] * (NA - n_real)
+        self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) else L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
         for i in self.coop:
-            L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
+            if self.vector_rule[i] is not None:
+                L.check_vector_rule(agg[i], self.H[i], len(self.in_nodes[i]))
+            else:
+                L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
         self._init_attacks(attack)
+        # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows
+        self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
+        self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -91,9 +101,13 @@ class Trainer:
             self.critic[i].copy_(torch.as_tensor(nets.pack_padded(w[1], 2 * NA)))
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
-        # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e
-        self.msg_c = torch.zeros(NA + len(self.byz_pairs), self.PC, **f32)
-        self.msg_t = torch.zeros(NA + len(self.byz_pairs), self.PT, **f32)
+        # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
+        # vec_row[i] the aggregate of cooperative agent i's distance-based rule
+        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents)
+        self.msg_c = torch.zeros(n_rows, self.PC, **f32)
+        self.msg_t = torch.zeros(n_rows, self.PT, **f32)
+        # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
+        self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
         self.adam_m = torch.zeros(NA, self.PA, **f32)
         self.adam_v = torch.zeros(NA, self.PA, **f32)
         self.adam_t = [0] * NA
@@ -176,6 +190,16 @@ class Trainer:
         """in_nodes[j] with each Byzantine neighbour replaced by the message row crafted for receiver j."""
         row = {b: self.NA + e for e, (b, r, _) in enumerate(self.byz_pairs) if r == j}
         return [row.get(k, k) for k in self.in_nodes[j]]
+
+    def neighbour_weights(self):
+        """{cooperative agent i with a distance-based rule: float32 [2, n_in]}: the weight w_k its rule gave each
+        in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in the
+        last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net."""
+        if not self.vec_agents:
+            return {}
+        w = self.vec_weights.cpu().numpy()
+        self.d2h_bytes += w.nbytes
+        return {i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(self.vec_agents)}
 
     def _try_peer_comm(self):
         """Set up the peer-memory exchange on every rank, or on none: the ranks agree (MIN all-reduce of a success
@@ -367,7 +391,10 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            nodes, H, rule = self._receiver_nodes(i), self.H[i], self.aggregation[i]
+            if i in self.vec_row:                  # the aggregate as the single in-node: clip returns it exactly
+                nodes, H, rule = [self.vec_row[i]], 0, L.AGG_CLIP
+            else:
+                nodes, H, rule = self._receiver_nodes(i), self.H[i], self.aggregation[i]
             cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
             cons_jobs.append(ops.consensus_job(self.tr[i], self.msg_t, self.PT, nets.n_hidden_params(3 * NA), nodes, H, rule))
             team_jobs.append(ops.team_job(self.critic[i], L.IN_S, self.msg_c, self.PC, nodes, H, sums=self.sums_team[2 * n], rule=rule))
@@ -385,6 +412,16 @@ class Trainer:
                 att_jobs.append(ops.attack_job(msgs[NA + e], msgs, P, P, honest, kind, param, seed=self.seed, attacker=b,
                                                receiver=j, round=self.episodes_done & 0xFFFFFFFF))
         att_groups = [ops.job_array(L.AttackJob, att_jobs[g:g + L.MAX_JOBS]) for g in range(0, len(att_jobs), L.MAX_JOBS)]
+
+        # distance-based aggregates over the messages each receiver hears (crafted Byzantine ones included): at most 16
+        # cooperative agents x 2 nets, so one launch per epoch
+        vec_jobs = []
+        for q, i in enumerate(self.vec_agents):
+            nodes, row = self._receiver_nodes(i), self.vec_row[i]
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                vec_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], self.vector_rule[i],
+                                               weights_out=self.vec_weights[2 * q + t]))
+        vec_jobs = ops.job_array(L.VectorJob, vec_jobs) if vec_jobs else None
 
         for epoch in range(self.n_epochs):                                 # :100
             # ---------------- I) local updates (:105-121)
@@ -407,6 +444,9 @@ class Trainer:
                 for job in g:
                     job.epoch = epoch
                 ops.attack(g)
+                self.launches += 1
+            if vec_jobs is not None:
+                ops.vector_aggregate(vec_jobs)
                 self.launches += 1
             # ---------------- II) resilient consensus (:125-145)
             if coop:

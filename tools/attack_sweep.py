@@ -1,13 +1,19 @@
 """Byzantine attacks against each resilient aggregation rule on the C2 team: 4 cooperative agents (H = 1) and agent 4
-Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (clip, trim, wmsr) x attack (alie, ipm, gauss) over the
-learning harness's seeds (tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed;
-agent 4 keeps its weights and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the
-cooperative critics' estimate of it, means of the last 500 episodes, over the seeds.
+Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (by default clip, trim, wmsr; any of the coordinate rules and
+the distance-based krum, mkrum, scclip, gmed) x attack (alie, ipm, gauss) over the learning harness's seeds
+(tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed; agent 4 keeps its weights
+and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the cooperative critics' estimate
+of it, means of the last 500 episodes, over the seeds; for a distance-based rule also the mean weight the receivers of
+agent 4 gave its crafted message in the last epoch of the last round (Trainer.neighbour_weights, both nets), over the
+seeds.
 
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
-agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).
+agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
+a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
+alternated the same way.
 
     python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
+                                 [rules=clip,trim,wmsr]
         -> out_dir/attack_sweep.{json,md} (a relative out_dir is taken from the current directory)
 """
 import json
@@ -24,12 +30,13 @@ import bench                                   # noqa: E402
 import torch                                   # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
-RULES = ("clip", "trim", "wmsr")
 ATTACKS = (("alie", 1.0), ("ipm", 0.5), ("gauss", 0.3))
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
 out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_out")
+RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
+VECTOR = ("krum", "mkrum", "scclip", "gmed")
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
 
 
@@ -68,15 +75,55 @@ def timing():
     return out
 
 
+def rule_timing():
+    """ms per update round (median over rounds) with agent 4 Byzantine (gauss) and every cooperative agent on clip, gmed
+    and mkrum, at the benchmark's C2 shape, the three trainers alternated round by round."""
+    cfg = dict(bench.workload("C2", 0), labels=["Cooperative"] * 4 + ["Byzantine"], attack=("gauss", 0.3))
+    trs = {r: Trainer(**dict(cfg, aggregation=[r] * 4 + ["clip"])) for r in ("clip", "gmed", "mkrum")}
+    ms = {k: [] for k in trs}
+    for r in range(timed_rounds + 1):
+        for k, tr in trs.items():
+            tr.rollout_block()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            a.record()
+            tr.update_round()
+            b.record()
+            torch.cuda.synchronize()
+            if r > 0:
+                ms[k].append(a.elapsed_time(b))
+    out = {k: dict(median_ms=float(np.median(v)), rounds_ms=v) for k, v in ms.items()}
+    for k in ("gmed", "mkrum"):
+        out[f"{k}_added_ms"] = out[k]["median_ms"] - out["clip"]["median_ms"]
+    out["n_envs"] = cfg["n_envs"]
+    out["aggregation_launches_per_round"] = trs["gmed"].n_epochs
+    return out
+
+
+def byzantine_weight(tr, b=4):
+    """Mean weight the receivers of agent b gave its message in the last epoch (critic and TR nets)."""
+    ws = []
+    for j, w in tr.neighbour_weights().items():
+        for k, node in enumerate(tr.in_nodes[j]):
+            if node == b:
+                ws.extend(w[:, k].tolist())
+    return float(np.mean(ws)) if ws else None
+
+
 z = np.load(os.path.join(ROOT, "tests", "golden", "ref_learning.npz"))
 runs = [str(r) for r in z["runs"] if str(r).startswith("malicious/H1/")]
 name, power = card()
 result = dict(card=name, power_limit_w=power, n_blocks=n_blocks, n_envs=n_envs, timing=timing(), cells=[])
 print(f"{name}, power limit {power} W: update round {result['timing']['Faulty']['median_ms']:.2f} ms (Faulty) vs "
       f"{result['timing']['Byzantine']['median_ms']:.2f} ms (Byzantine)", flush=True)
+vector = any(r in VECTOR for r in RULES)
+if vector:
+    result["rule_timing"] = rt = rule_timing()
+    print(f"update round with agent 4 Byzantine: clip {rt['clip']['median_ms']:.2f} ms, gmed {rt['gmed']['median_ms']:.2f} ms "
+          f"({rt['gmed_added_ms']:+.3f}), mkrum {rt['mkrum']['median_ms']:.2f} ms ({rt['mkrum_added_ms']:+.3f})", flush=True)
 for rule in RULES:
     for attack in ATTACKS:
-        team, est = [], []
+        team, est, byz = [], [], []
         for tag in runs:
             _, _, ss = tag.split("/")
             labels = [str(x) for x in z[f"{tag}/labels"]]
@@ -97,20 +144,32 @@ for rule in RULES:
                 tr.update_round()
                 t.append(float(rr[:, :4].mean())); e.append(float(ee[:, :4].mean()))
             team.append(float(np.mean(t[-tail:]))); est.append(float(np.mean(e[-tail:])))
+            byz.append(byzantine_weight(tr))
         cell = dict(rule=rule, attack=attack[0], param=attack[1], seeds=len(runs), team=float(np.mean(team)),
                     est=float(np.mean(est)), team_per_seed=team, est_per_seed=est)
+        if vector:
+            cell["byz_weight"] = float(np.mean(byz)) if rule in VECTOR else None
         result["cells"].append(cell)
-        print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}", flush=True)
+        print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}"
+              + (f"  weight of agent 4 {cell['byz_weight']:.3f}" if cell.get("byz_weight") is not None else ""), flush=True)
 
 os.makedirs(out_dir, exist_ok=True)
 json.dump(result, open(os.path.join(out_dir, "attack_sweep.json"), "w"))
 with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
     f.write(f"{name}, power limit {power} W; {len(runs)} seeds, {n_blocks} blocks x 50 episodes, {n_envs} environments; "
-            "means of the last 500 episodes\n\n| rule | attack | team return | critic estimate |\n|---|---|---|---|\n")
+            "means of the last 500 episodes\n\n| rule | attack | team return | critic estimate |"
+            + (" weight of agent 4 |\n|---|---|---|---|---|\n" if vector else "\n|---|---|---|---|\n"))
     for c in result["cells"]:
-        f.write(f"| {c['rule']} | {c['attack']} {c['param']} | {c['team']:.2f} | {c['est']:.2f} |\n")
+        f.write(f"| {c['rule']} | {c['attack']} {c['param']} | {c['team']:.2f} | {c['est']:.2f} |"
+                + ((f" {c['byz_weight']:.3f} |" if c["byz_weight"] is not None else " - |") if vector else "") + "\n")
     t = result["timing"]
     f.write(f"\nC2 update round at {t['n_envs']} environments (median of {timed_rounds}, alternated): "
             f"{t['Faulty']['median_ms']:.2f} ms with agent 4 Faulty, {t['Byzantine']['median_ms']:.2f} ms Byzantine (gauss), "
             f"{t['added_ms']:+.2f} ms\n")
+    if vector:
+        rt = result["rule_timing"]
+        f.write(f"\nC2 update round at {rt['n_envs']} environments, agent 4 Byzantine (gauss), every cooperative agent on one "
+                f"rule (median of {timed_rounds}, alternated): clip {rt['clip']['median_ms']:.2f} ms, gmed "
+                f"{rt['gmed']['median_ms']:.2f} ms ({rt['gmed_added_ms']:+.3f} ms), mkrum {rt['mkrum']['median_ms']:.2f} ms "
+                f"({rt['mkrum_added_ms']:+.3f} ms)\n")
 print(open(os.path.join(out_dir, "attack_sweep.md")).read())
