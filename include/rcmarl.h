@@ -155,6 +155,55 @@ typedef struct {
 } rcmarl_attack_job;
 int rcmarl_attack(const rcmarl_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* Byzantine messages scaled to the receiver's honest spread (rcmarl_adaptive_attack): the min-max and min-sum attacks of
+ * Shejwalkar & Houmansadr, "Manipulating the Byzantine" (NDSS 2021), under the threat model of rcmarl_attack.  They push
+ * the message as far along a direction d as one distance constraint over the honest set allows; they do not adapt to the
+ * receiver's rule or H.  All arithmetic is fp32.  Over the honest rows v_1 .. v_n (n = n_honest, in list order, repeats
+ * included, v_k = msgs + honest[k] * msg_stride) with P = job.n:
+ *   mu, sigma   exactly as rcmarl_attack computes them (same summation order);
+ *   d           UV:  d = -mu / ||mu||, ||mu|| = sqrt(sum_p mu_p^2); d = 0 if ||mu|| is 0 or not finite
+ *               STD: d = -sigma
+ *               SGN: d_p = -sign(mu_p), sign(0) = 0
+ *   e_k = sum_p (mu_p - v_k,p)^2,  b_k = sum_p (mu_p - v_k,p) d_p,  a = sum_p d_p^2,  D_kl = sum_p (v_k,p - v_l,p)^2;
+ * each sum is taken by one warp (lane-strided fmaf partials, then the fixed xor butterfly), and a value of e_k, a, D_kl
+ * or ||mu||^2 that is not finite counts as +inf.
+ *   MINMAX  c = max_{k<l} D_kl (0 for n = 1); gamma_k = root(a, b_k, e_k, c); gamma = max(0, min_k gamma_k).  In exact
+ *           arithmetic {g >= 0 : max_k ||mu + g d - v_k||^2 <= c} = [0, gamma] (it holds 0 because e_k <= c).
+ *   MINSUM  c = max_k sum_{l != k} D_kl (summed in index order); gamma = root(n a, sum_k b_k, sum_k e_k, c) with the
+ *           sums in index order and n a one fp32 product.  In exact arithmetic {g >= 0 : sum_k ||mu + g d - v_k||^2 <= c}
+ *           = [0, gamma].
+ * root(A, b, e, c) is the largest root of A g^2 + 2 b g + e = c in a form free of cancellation: with m = c - e and
+ * R = sqrtf(fmaxf(fmaf(b, b, A * m), 0)), it is (-b + R) / A if b <= 0 and m / (b + R) otherwise; it is 0 when m <= 0.
+ * gamma = 0 when a = 0, when c, a, some e_k or some b_k is not finite, or when the result is not finite.  The output is
+ *   t = scale * gamma,   dst[p] = t == 0 ? mu_p : fmaf(t, d_p, mu_p),
+ * so scale = 1 is the paper's attack and scale = 0 is bitwise rcmarl_attack's ALIE at z = 0.  gamma_out (optional, one
+ * float) receives gamma.  The paper finds gamma by halving a step from an initial guess until the constraint holds; the
+ * closed form is the supremum that search converges to.
+ * One CTA per job, the honest rows, mu and d staged in shared memory, fixed summation orders, no atomics: bitwise
+ * reproducible, independent of the job order and of how jobs are split over launches.  Refused (RCMARL_ERR_ARG, nothing
+ * launched, dst and gamma_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_honest outside
+ * 1..RCMARL_MAX_NEIGHBOURS, a negative honest index, an unknown kind or dev, a scale that is not finite or is < 0,
+ * (n_honest + 2) * n > RCMARL_ADAPTIVE_MAX_FLOATS (the staging bound: 16 honest rows, mu and d of up to 1536
+ * parameters), a dst or gamma_out that overlaps an honest row of any job of the launch, and two written ranges (dsts,
+ * gamma_outs) of the launch that overlap.  NaN inputs are not supported. */
+#define RCMARL_ADAPTIVE_MAX_FLOATS (18 * 1536)
+typedef enum { RCMARL_ADAPT_MINMAX = 0, RCMARL_ADAPT_MINSUM = 1 } rcmarl_adaptive_kind;
+typedef enum { RCMARL_DEV_UV = 0, RCMARL_DEV_STD = 1, RCMARL_DEV_SGN = 2 } rcmarl_adaptive_dev;
+typedef struct {
+    float* dst;                 /* the crafted message (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    float* gamma_out;           /* optional [1]: gamma */
+    int32_t n;                  /* parameters crafted: dst[0:n] from msgs[honest[k]][0:n] */
+    int32_t n_honest;
+    int32_t honest[RCMARL_MAX_NEIGHBOURS];
+    int32_t kind;               /* rcmarl_adaptive_kind */
+    int32_t dev;                /* rcmarl_adaptive_dev */
+    float scale;                /* s >= 0; 1 is the paper's attack */
+    int32_t reserved;
+} rcmarl_adaptive_attack_job;
+int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* Distance-based resilient aggregation of whole messages (rcmarl_vector_aggregate).  The rules above are coordinate-wise;
  * these compare the in-neighbours' messages as vectors.  One job: its n = n_in messages x_k = msgs + in_nodes[k] *
  * msg_stride, k = 0 .. n-1 (k = 0 is the receiver's own; repeats in in_nodes count), each of P = job.n packed

@@ -11,6 +11,8 @@
 //   attack_kernel   Byzantine messages crafted per receiver (ALIE / IPM / Gaussian, rcmarl_attack)
 //   vector_agg_kernel  distance-based rules over whole messages (Krum, multi-Krum, self-centred clipping, geometric
 //                   median; rcmarl_vector_aggregate)
+//   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
+//                   (rcmarl_adaptive_attack)
 //   consensus, sgd/adam apply, reward mix: the small glue kernels.
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
@@ -546,6 +548,129 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
     }
 }
 
+// Min-max / min-sum Byzantine messages (rcmarl_adaptive_attack, include/rcmarl.h): one CTA of 256 threads per job.  The
+// honest rows are staged in shared memory, then mu and d (one thread per coordinate, mu and sigma as attack_kernel).
+// Every distance and inner product is summed by ONE warp as in warp_sqdist, so its value does not depend on which warp
+// takes it; gamma is solved on one thread and the output takes one thread per coordinate.
+struct AdaptiveParams { rcmarl_adaptive_attack_job jobs[RCMARL_MAX_JOBS]; };
+constexpr int ADA_THREADS = 256;
+
+// sum_p x_p y_p of two shared-memory vectors of n floats, in every lane of the calling warp
+__device__ __forceinline__ float warp_dot(const float* x, const float* y, int n, int lane) {
+    float s = 0.f;
+    for (int p = lane; p < n; p += 32) s = fmaf(x[p], y[p], s);
+    return warp_sum(s);
+}
+
+// the largest root of A g^2 + 2 b g + e = c, cancellation-free; 0 when c - e <= 0
+__device__ __forceinline__ float adaptive_root(float A, float b, float e, float c) {
+    const float m = c - e;
+    if (!(m > 0.f)) return 0.f;
+    const float R = sqrtf(fmaxf(fmaf(b, b, A * m), 0.f));
+    return b <= 0.f ? (-b + R) / A : m / (b + R);
+}
+
+__global__ void __launch_bounds__(ADA_THREADS) adaptive_attack_kernel(const __grid_constant__ AdaptiveParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];    // D_kl, k != l
+    __shared__ float ek[MAXN], bk[MAXN];
+    __shared__ float scal[2];              // a; UV: ||mu||^2, then gamma
+    const rcmarl_adaptive_attack_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nh = job.n_honest;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    constexpr int NW = ADA_THREADS / 32;
+    float* xs = smem;                              // [n_honest][n]
+    float* mu = smem + (int64_t)nh * n;            // [n]
+    float* d = mu + n;                             // [n]
+    for (int k = 0; k < nh; ++k) {
+        const float* src = job.msgs + (int64_t)job.honest[k] * job.msg_stride;
+        for (int p = tid; p < n; p += ADA_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        float s = 0.f;
+        for (int k = 0; k < nh; ++k) s += xs[k * n + p];
+        const float m = s / (float)nh;
+        mu[p] = m;
+        if (job.dev == RCMARL_DEV_STD) {
+            float q = 0.f;
+            for (int k = 0; k < nh; ++k) q = fmaf(xs[k * n + p] - m, xs[k * n + p] - m, q);
+            d[p] = -sqrtf(q / (float)nh);
+        } else if (job.dev == RCMARL_DEV_SGN) {
+            d[p] = m > 0.f ? -1.f : (m < 0.f ? 1.f : 0.f);
+        }
+    }
+    __syncthreads();
+    if (job.dev == RCMARL_DEV_UV) {
+        if (warp == 0) {
+            const float q = warp_dot(mu, mu, n, lane);
+            if (lane == 0) scal[1] = isfinite(q) ? sqrtf(q) : INFINITY;
+        }
+        __syncthreads();
+        const float nrm = scal[1];
+        const bool zero = nrm == 0.f || !isfinite(nrm);
+        for (int p = tid; p < n; p += ADA_THREADS) d[p] = zero ? 0.f : -mu[p] / nrm;
+        __syncthreads();
+    }
+    // warp tasks: the unordered pairs k < l, then e_k and b_k for each k, then a
+    const int n_pairs = nh * (nh - 1) / 2;
+    for (int t = warp; t < n_pairs + nh + 1; t += NW) {
+        if (t < n_pairs) {
+            int k = 0, r = t;
+            while (r >= nh - 1 - k) { r -= nh - 1 - k; ++k; }
+            const int l = k + 1 + r;
+            const float v = warp_sqdist(xs + k * n, xs + l * n, n, lane);
+            if (lane == 0) { dist[k * MAXN + l] = v; dist[l * MAXN + k] = v; }
+        } else if (t < n_pairs + nh) {
+            const int k = t - n_pairs;
+            const float* v = xs + k * n;
+            const float e = warp_sqdist(mu, v, n, lane);
+            float s = 0.f;
+            for (int p = lane; p < n; p += 32) s = fmaf(mu[p] - v[p], d[p], s);
+            s = warp_sum(s);
+            if (lane == 0) { ek[k] = e; bk[k] = s; }
+        } else {
+            const float q = warp_dot(d, d, n, lane);
+            if (lane == 0) scal[0] = isfinite(q) ? q : INFINITY;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const float a = scal[0];
+        bool ok = a > 0.f && isfinite(a);
+        for (int k = 0; k < nh; ++k) ok = ok && isfinite(ek[k]) && isfinite(bk[k]);
+        float g = 0.f;
+        if (job.kind == RCMARL_ADAPT_MINMAX) {
+            float c = 0.f;
+            for (int k = 0; k < nh; ++k)
+                for (int l = k + 1; l < nh; ++l) c = fmaxf(c, dist[k * MAXN + l]);
+            if (ok && isfinite(c)) {
+                g = INFINITY;
+                for (int k = 0; k < nh; ++k) g = fminf(g, adaptive_root(a, bk[k], ek[k], c));
+                g = fmaxf(0.f, g);
+            }
+        } else {
+            float c = 0.f, sb = 0.f, se = 0.f;
+            for (int k = 0; k < nh; ++k) {
+                float s = 0.f;
+                for (int l = 0; l < nh; ++l)
+                    if (l != k) s += dist[k * MAXN + l];
+                c = fmaxf(c, s);
+                sb += bk[k];
+                se += ek[k];
+            }
+            if (ok && isfinite(c)) g = adaptive_root((float)nh * a, sb, se, c);
+        }
+        if (!isfinite(g)) g = 0.f;
+        scal[1] = g;
+        if (job.gamma_out) *job.gamma_out = g;
+    }
+    __syncthreads();
+    const float t = job.scale * scal[1];
+    for (int p = tid; p < n; p += ADA_THREADS) job.dst[p] = t == 0.f ? mu[p] : fmaf(t, d[p], mu[p]);
+}
+
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
 __global__ void __launch_bounds__(256) sgd_kernel(const __grid_constant__ SgdParams P) {
     const rcmarl_sgd_job& job = P.jobs[blockIdx.y];
@@ -1023,6 +1148,30 @@ static void float_range(const float* base, int64_t row, int64_t stride, int64_t 
     last = first + (uintptr_t)(n * (int64_t)sizeof(float));
 }
 
+// true if a written range [w0, w1) overlaps another written range or a read range [r0, r1)
+static bool writes_overlap(const uintptr_t* w0, const uintptr_t* w1, int n_w, const uintptr_t* r0, const uintptr_t* r1,
+                           int n_r) {
+    for (int a = 0; a < n_w; ++a) {
+        for (int b = a + 1; b < n_w; ++b)
+            if (w0[a] < w1[b] && w0[b] < w1[a]) return true;
+        for (int r = 0; r < n_r; ++r)
+            if (w0[a] < r1[r] && r0[r] < w1[a]) return true;
+    }
+    return false;
+}
+
+// Lift a kernel's dynamic shared-memory limit to `bytes`, once per device (opted: that kernel's flags), before its first
+// launch there, independent of any other launch.
+static int opt_in_smem(const void* kernel, int bytes, bool (&opted)[64]) {
+    int dev = 0;
+    RC_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64 || !opted[dev]) {
+        RC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        if (dev >= 0 && dev < 64) opted[dev] = true;
+    }
+    return RCMARL_OK;
+}
+
 int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     VectorParams P;
@@ -1054,24 +1203,56 @@ int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* str
         for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
             float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
     }
-    for (int a = 0; a < n_w; ++a) {
-        for (int b = a + 1; b < n_w; ++b)
-            if (w0[a] < w1[b] && w0[b] < w1[a]) return RCMARL_ERR_ARG;
-        for (int r = 0; r < n_r; ++r)
-            if (w0[a] < r1[r] && r0[r] < w1[a]) return RCMARL_ERR_ARG;
-    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
     // The kernel also has static shared memory, so the default 48 KB limit applies to static + dynamic: opt in to the
     // largest staging size, once per device, before the first launch there (independent of any other launch).
     static bool opted[64] = {};
-    int dev = 0;
-    RC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !opted[dev]) {
-        RC_CUDA(cudaFuncSetAttribute(vector_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(sizeof(float) * RCMARL_VECTOR_MAX_FLOATS)));
-        if (dev >= 0 && dev < 64) opted[dev] = true;
-    }
+    if (int e = opt_in_smem((const void*)vector_agg_kernel, (int)(sizeof(float) * RCMARL_VECTOR_MAX_FLOATS), opted)) return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     vector_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    AdaptiveParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_adaptive_attack_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_honest; ++k)
+            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (q.kind < RCMARL_ADAPT_MINMAX || q.kind > RCMARL_ADAPT_MINSUM || q.dev < RCMARL_DEV_UV || q.dev > RCMARL_DEV_SGN)
+            return RCMARL_ERR_ARG;
+        if (!std::isfinite(q.scale) || q.scale < 0.f) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_honest + 2) * q.n;
+        if (floats > RCMARL_ADAPTIVE_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate: no written range (a dst, a gamma_out) may overlap an honest row of any job of the launch
+    // or another written range
+    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (jobs[j].gamma_out) {
+            float_range(jobs[j].gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < jobs[j].n_honest; ++k, ++n_r)
+            float_range(jobs[j].msgs, jobs[j].honest[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    // the staging bound is above the default 48 KB of dynamic shared memory
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)adaptive_attack_kernel, (int)(sizeof(float) * RCMARL_ADAPTIVE_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    adaptive_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

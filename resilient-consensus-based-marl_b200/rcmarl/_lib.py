@@ -31,6 +31,12 @@ VECTOR_RULES = {"krum": VEC_KRUM, "mkrum": VEC_MKRUM, "scclip": VEC_SCCLIP, "gme
 GMED_ITERS = 8
 GMED_NU = 1e-6
 VECTOR_MAX_FLOATS = 48 * 1024
+ADAPT_MINMAX, ADAPT_MINSUM = 0, 1                 # rcmarl_adaptive_kind
+DEV_UV, DEV_STD, DEV_SGN = 0, 1, 2                # rcmarl_adaptive_dev
+# min-max / min-sum attacks (rcmarl_adaptive_attack): name -> (kind, dev); the parameter is the scale s >= 0
+ADAPTIVE_ATTACKS = {f"{k}_{d}": (kind, dev) for k, kind in (("minmax", ADAPT_MINMAX), ("minsum", ADAPT_MINSUM))
+                    for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+ADAPTIVE_MAX_FLOATS = 18 * 1536
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -54,6 +60,12 @@ class AttackJob(C.Structure):
 class VectorJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("weights_out", c_fp), ("n", C.c_int32),
                 ("n_in", C.c_int32), ("H", C.c_int32), ("rule", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS)]
+
+
+class AdaptiveAttackJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("gamma_out", c_fp), ("n", C.c_int32),
+                ("n_honest", C.c_int32), ("honest", C.c_int32 * MAX_NEIGHBOURS), ("kind", C.c_int32), ("dev", C.c_int32),
+                ("scale", C.c_float), ("reserved", C.c_int32)]
 
 
 class ValueJob(C.Structure):
@@ -109,6 +121,7 @@ SYMBOLS = [
     ("rcmarl_consensus_hidden", C.c_int, [C.POINTER(ConsensusJob), C.c_int, c_fp]),
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
@@ -202,19 +215,27 @@ def check_vector_rule(rule, H, n_in):
     return VECTOR_RULES[rule]
 
 
+def is_adaptive_attack(name):
+    """True for the name of a min-max / min-sum attack (rcmarl_adaptive_attack): "minmax_uv", ..., "minsum_sgn"."""
+    return isinstance(name, str) and name in ADAPTIVE_ATTACKS
+
+
 def check_attack(attack):
-    """(name, param) -> (rcmarl_attack_kind, float param); raise RcmarlError unless the name is known and the parameter
-    finite (and, for "gauss", s >= 0), as rcmarl_attack requires (include/rcmarl.h)."""
+    """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
+    "gauss" and the adaptive attacks also >= 0), as rcmarl_attack / rcmarl_adaptive_attack require (include/rcmarl.h).
+    kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss", and the pair (rcmarl_adaptive_kind,
+    rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the paper's attack)."""
     try:
         name, param = attack
         param = float(param)
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
-    if not isinstance(name, str) or name not in ATTACKS:
-        raise RcmarlError(f"unknown attack {name!r}: expected one of {sorted(ATTACKS)}")
-    if not math.isfinite(param) or (name == "gauss" and param < 0):
-        raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if name == "gauss" else "") + f", got {param}")
-    return ATTACKS[name], param
+    if not isinstance(name, str) or (name not in ATTACKS and name not in ADAPTIVE_ATTACKS):
+        raise RcmarlError(f"unknown attack {name!r}: expected one of {sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS)}")
+    nonneg = name == "gauss" or name in ADAPTIVE_ATTACKS
+    if not math.isfinite(param) or (nonneg and param < 0):
+        raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
+    return (ADAPTIVE_ATTACKS[name] if name in ADAPTIVE_ATTACKS else ATTACKS[name]), param
 
 
 def param_count(d_in, n_out):

@@ -295,6 +295,31 @@ def attack(jobs):
     L.check(L.lib().rcmarl_attack(a, len(a), _stream()), "rcmarl_attack")
 
 
+def adaptive_attack_job(dst, msgs, msg_stride, n, honest, attack, scale, gamma_out=None):
+    """attack: min-max / min-sum attack name ("minmax_uv", ..., "minsum_sgn") or a (rcmarl_adaptive_kind,
+    rcmarl_adaptive_dev) pair of ids (include/rcmarl.h); scale: s >= 0.  Names are checked here, ids and limits by the
+    library."""
+    j = L.AdaptiveAttackJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.gamma_out = ptr(gamma_out)
+    j.n_honest = len(honest)
+    for k, v in enumerate(honest[:L.MAX_NEIGHBOURS]):
+        j.honest[k] = v
+    if isinstance(attack, str):
+        if not L.is_adaptive_attack(attack):
+            raise L.RcmarlError(f"unknown adaptive attack {attack!r}: expected one of {sorted(L.ADAPTIVE_ATTACKS)}")
+        attack = L.ADAPTIVE_ATTACKS[attack]
+    j.kind, j.dev = int(attack[0]), int(attack[1])
+    j.scale = scale
+    j._keep = (dst, msgs, gamma_out)
+    return j
+
+
+def adaptive_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.AdaptiveAttackJob, jobs)
+    L.check(L.lib().rcmarl_adaptive_attack(a, len(a), _stream()), "rcmarl_adaptive_attack")
+
+
 def vector_job(dst, msgs, msg_stride, n, in_nodes, H, rule, weights_out=None):
     """rule: distance-based rule name ("krum", "mkrum", "scclip", "gmed") or rcmarl_vector_rule id (include/rcmarl.h).
     Names are checked here, ids and limits by the library."""
