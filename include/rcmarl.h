@@ -204,6 +204,64 @@ typedef struct {
 } rcmarl_adaptive_attack_job;
 int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* Rule-aware Byzantine messages (rcmarl_tailored_attack): the AGR-tailored attack of Shejwalkar & Houmansadr (NDSS 2021,
+ * section IV; compare Fang et al., USENIX Security 2020).  Threat model: that of rcmarl_attack, extended -- the attacker
+ * also knows the receiver j's aggregation rule, its H and every real message j hears.  One job is one (attacker,
+ * receiver j, net).  All arithmetic is fp32.
+ *   Slots.  k = 0 .. n_in-1 in in_nodes[j] order, slot 0 the receiver's own message.  slots[k] >= 0 is a real slot, the
+ *           row msgs + slots[k] * msg_stride, read as it is (an honest agent, or a Malicious, Greedy or Faulty one);
+ *           slots[k] = -1 is a crafted slot: a Byzantine in-neighbour of j, which the attacker models as sending the
+ *           same message m as itself (repeats count).  Bit k of honest_mask marks slot k as a member of the honest set
+ *           S_j; its rows, in slot order, are the honest rows of rcmarl_adaptive_attack.
+ *   Search. mu, d and gamma_mm are exactly those of rcmarl_adaptive_attack for MINMAX and direction dev over S_j (the
+ *           same device code and summation orders).  Gamma = scale * gamma_mm, and Gamma = 0 if that fp32 product is
+ *           not finite (a huge scale: every candidate is then mu); for i = 0 .. K (K =
+ *           RCMARL_TAILORED_STEPS) the candidate gamma_i = (Gamma * i) / K (fp32, in that order) and its message
+ *             m(gamma_i)_p = gamma_i == 0 ? mu_p : fmaf(gamma_i, d_p, mu_p);
+ *           x(gamma_i) is the slot list with every crafted slot set to m(gamma_i).
+ *   Objective.  O_i = sum_p (R_j(x(gamma_i))_p - mu_p)^2, summed by one warp (lane-strided fmaf partials, then the fixed
+ *           xor butterfly); a sum that is not finite counts as -inf.  R_j is the receiver's rule with H:
+ *             family COORD (rule: rcmarl_agg_rule): resilient aggregation of the n_in slot values of every packed
+ *               parameter, own = slot 0, as rcmarl_consensus_hidden computes it.  That is exact for the hidden layers;
+ *               for the head it is the attacker's model only (the receiver combines its head through per-row
+ *               estimates in rcmarl_team, which the attacker does not model);
+ *             family VECTOR (rule: rcmarl_vector_rule): exactly the output of rcmarl_vector_aggregate on x(gamma_i).
+ *   Output. i* = argmax_i O_i, ties to the smaller i, and i* = 0 if every O_i is -inf; dst[p] = m(gamma_i*)_p and
+ *           gamma_out (optional, one float) receives gamma_i*.
+ * Hence scale = 0 is bitwise rcmarl_attack's ALIE at z = 0 (mu); at scale = 1, gamma_K = gamma_mm, so the message does
+ * at least as much damage to its target rule as the min-max message in the same direction (up to the rounding of O);
+ * and a plain-mean receiver (COORD CLIP, H = 0) whose real slots are all honest has R_j - mu = gamma (n_crafted / n_in) d,
+ * so O rises strictly with i when a = ||d||^2 > 0 and gamma_mm > 0, and the output is the min-max message at the scale.
+ * (A real slot that is not honest adds a constant offset to R_j - mu, and O may fall before it rises.)
+ * One CTA per job: the real slots, mu, d, the candidate and one work row staged in shared memory, fixed summation
+ * orders, no atomics -- bitwise reproducible, independent of the job order and of how jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst and gamma_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null dst
+ * or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, no crafted slot, no honest slot, a crafted slot marked honest,
+ * a honest_mask bit at or past n_in, a slot below -1, an unknown family, rule or dev, an H the rule refuses for n_in
+ * (the checks of rcmarl_consensus_hidden and rcmarl_vector_aggregate), a scale that is not finite or is < 0,
+ * (n_in + 3) * n > RCMARL_TAILORED_MAX_FLOATS (the staging bound: 15 real slots, mu, d, the candidate and the work row
+ * of up to 1536 parameters), a dst or gamma_out that overlaps a real slot's row of any job of the launch, and two
+ * written ranges (dsts, gamma_outs) of the launch that overlap.  NaN inputs are not supported. */
+#define RCMARL_TAILORED_STEPS 32
+#define RCMARL_TAILORED_MAX_FLOATS (19 * 1536)
+typedef enum { RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1 } rcmarl_tailored_family;
+typedef struct {
+    float* dst;                 /* the crafted message (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    float* gamma_out;           /* optional [1]: gamma_i* */
+    int32_t n;                  /* parameters per message */
+    int32_t n_in;
+    int32_t slots[RCMARL_MAX_NEIGHBOURS];   /* a message row, or -1 for a crafted slot */
+    uint32_t honest_mask;       /* bit k: slot k is in the honest set */
+    int32_t family;             /* rcmarl_tailored_family */
+    int32_t rule;               /* rcmarl_agg_rule (COORD) or rcmarl_vector_rule (VECTOR) */
+    int32_t H;
+    int32_t dev;                /* rcmarl_adaptive_dev */
+    float scale;                /* s >= 0: the search range is [0, s * gamma_mm] */
+} rcmarl_tailored_attack_job;
+int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* Distance-based resilient aggregation of whole messages (rcmarl_vector_aggregate).  The rules above are coordinate-wise;
  * these compare the in-neighbours' messages as vectors.  One job: its n = n_in messages x_k = msgs + in_nodes[k] *
  * msg_stride, k = 0 .. n-1 (k = 0 is the receiver's own; repeats in in_nodes count), each of P = job.n packed

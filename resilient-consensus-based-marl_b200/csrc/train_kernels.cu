@@ -13,6 +13,7 @@
 //                   median; rcmarl_vector_aggregate)
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
+//   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
 //   consensus, sgd/adam apply, reward mix: the small glue kernels.
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
@@ -393,31 +394,32 @@ __device__ __forceinline__ float warp_sqdist(const float* a, const float* b, int
     return isfinite(s) ? s : INFINITY;
 }
 
-__global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_constant__ VectorParams P) {
+// The messages of a job staged one after another in shared memory: message k at xs + k * n.
+struct StagedRows {
+    const float* xs;
+    int n;
+    __device__ __forceinline__ const float* operator()(int k) const { return xs + k * n; }
+    __device__ __forceinline__ float at(int k, int p) const { return xs[k * n + p]; }
+};
+
+// The body of rcmarl_vector_aggregate over nin messages row(0) .. row(nin - 1) of n floats in shared memory: writes the
+// aggregate to out[0:n] and leaves w_k in wt (the caller synchronises before reading either).  z is a shared work row
+// of n floats (GMED's iterate) and may be out itself: the last Weiszfeld step reads only the messages and wt.  Shared
+// scratch: dist [MAXN * MAXN] (KRUM / MKRUM: D_kl; SCCLIP: d_k in dist[k]), wt [MAXN] (KRUM / MKRUM: w_k; SCCLIP: c_k;
+// GMED: beta_k), score [MAXN], total (GMED: sum beta).  Called by the whole CTA of VEC_THREADS threads; Row maps a
+// message index to its staged row.
+template <class Row>
+__device__ __forceinline__ void vector_rule(const Row& row, int n, int nin, int H, int rule, float* z, float* out,
+                                            float* dist, float* wt, float* score, float& total) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
-    extern __shared__ __align__(16) float smem[];
-    __shared__ float dist[MAXN * MAXN];    // KRUM / MKRUM: D_kl; SCCLIP: d_k in dist[k]
-    __shared__ float wt[MAXN];             // KRUM / MKRUM: w_k; SCCLIP: c_k; GMED: beta_k
-    __shared__ float score[MAXN];
-    __shared__ float total;                // GMED: sum beta
-    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
-    const int n = job.n, nin = job.n_in, H = job.H, rule = job.rule;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     constexpr int NW = VEC_THREADS / 32;
-    float* xs = smem;                              // [n_in][n]
-    float* z = smem + (int64_t)nin * n;            // GMED iterate [n]
-    for (int k = 0; k < nin; ++k) {
-        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
-        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
-    }
-    __syncthreads();
-
     if (rule == RCMARL_VEC_KRUM || rule == RCMARL_VEC_MKRUM) {
         for (int t = warp; t < nin * (nin - 1) / 2; t += NW) {       // unordered pairs k < l
             int k = 0, r = t;
             while (r >= nin - 1 - k) { r -= nin - 1 - k; ++k; }
             const int l = k + 1 + r;
-            const float d = warp_sqdist(xs + k * n, xs + l * n, n, lane);
+            const float d = warp_sqdist(row(k), row(l), n, lane);
             if (lane == 0) { dist[k * MAXN + l] = d; dist[l * MAXN + k] = d; }
         }
         __syncthreads();
@@ -462,12 +464,12 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
         for (int p = tid; p < n; p += VEC_THREADS) {
             float s = 0.f;
             for (int k = 0; k < nin; ++k)
-                if (wt[k] != 0.f) s += xs[k * n + p];
-            job.dst[p] = s / fm;
+                if (wt[k] != 0.f) s += row.at(k, p);
+            out[p] = s / fm;
         }
     } else if (rule == RCMARL_VEC_SCCLIP) {
         for (int k = 1 + warp; k < nin; k += NW) {
-            const float d = sqrtf(warp_sqdist(xs + k * n, xs, n, lane));
+            const float d = sqrtf(warp_sqdist(row(k), row(0), n, lane));
             if (lane == 0) dist[k] = d;
         }
         __syncthreads();
@@ -489,13 +491,13 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
         __syncthreads();
         const float fn = (float)nin;
         for (int p = tid; p < n; p += VEC_THREADS) {
-            const float x0 = xs[p];
+            const float x0 = row.at(0, p);
             float s = 0.f;
             for (int k = 1; k < nin; ++k) {
                 const float c = wt[k];
-                if (c != 0.f) s = fmaf(c, xs[k * n + p] - x0, s);
+                if (c != 0.f) s = fmaf(c, row.at(k, p) - x0, s);
             }
-            job.dst[p] = x0 + s / fn;
+            out[p] = x0 + s / fn;
         }
         __syncthreads();                                              // every c_k read
         if (tid == 0) {
@@ -510,13 +512,13 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
         for (int p = tid; p < n; p += VEC_THREADS) {
             float v[MAXN];
 #pragma unroll
-            for (int k = 0; k < MAXN; ++k) v[k] = k < nin ? xs[k * n + p] : 0.f;
+            for (int k = 0; k < MAXN; ++k) v[k] = k < nin ? row.at(k, p) : 0.f;
             z[p] = resilient_mean_small<MAXN>(v, nin, (nin - 1) / 2, RCMARL_AGG_TRIM);
         }
         for (int it = 0; it < RCMARL_GMED_ITERS; ++it) {
             __syncthreads();                                          // z complete
             for (int k = warp; k < nin; k += NW) {
-                const float d = sqrtf(warp_sqdist(xs + k * n, z, n, lane));
+                const float d = sqrtf(warp_sqdist(row(k), z, n, lane));
                 if (lane == 0) wt[k] = isfinite(d) ? 1.f / fmaxf(d, RCMARL_GMED_NU) : 0.f;
             }
             __syncthreads();
@@ -527,21 +529,41 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
                 total = s;
             }
             __syncthreads();
-            const float S = total;
-            float* out = it == RCMARL_GMED_ITERS - 1 ? job.dst : z;
+            const float St = total;
+            float* o = it == RCMARL_GMED_ITERS - 1 ? out : z;
             for (int p = tid; p < n; p += VEC_THREADS) {
                 float s = 0.f;
                 for (int k = 0; k < nin; ++k) {
                     const float b = wt[k];
-                    if (b != 0.f) s = fmaf(b, xs[k * n + p], s);
+                    if (b != 0.f) s = fmaf(b, row.at(k, p), s);
                 }
-                out[p] = s / S;
+                o[p] = s / St;
             }
         }
         __syncthreads();                                              // every beta_k read
         if (tid == 0)
             for (int k = 0; k < nin; ++k) wt[k] = wt[k] / total;
     }
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];
+    __shared__ float wt[MAXN];
+    __shared__ float score[MAXN];
+    __shared__ float total;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    float* xs = smem;                              // [n_in][n]
+    float* z = smem + (int64_t)nin * n;            // GMED iterate [n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    vector_rule(StagedRows{xs, n}, n, nin, job.H, job.rule, z, job.dst, dist, wt, score, total);
     if (job.weights_out) {
         __syncthreads();
         if (tid < nin) job.weights_out[tid] = wt[tid];
@@ -570,39 +592,32 @@ __device__ __forceinline__ float adaptive_root(float A, float b, float e, float 
     return b <= 0.f ? (-b + R) / A : m / (b + R);
 }
 
-__global__ void __launch_bounds__(ADA_THREADS) adaptive_attack_kernel(const __grid_constant__ AdaptiveParams P) {
+// mu, d and gamma of rcmarl_adaptive_attack (kind, dev) over the nh honest rows xs[k * n .. k * n + n) staged in shared
+// memory: writes mu[0:n] and d[0:n] and calls finish(gamma) on thread 0 (the caller synchronises before reading any of
+// them).  Shared scratch: dist [MAXN * MAXN] (D_kl, k != l), ek, bk [MAXN], scal [2] (a; UV: ||mu||).  Called by the
+// whole CTA of ADA_THREADS threads after the rows are staged.
+template <class Finish>
+__device__ __forceinline__ void adaptive_gamma(const float* xs, int nh, int n, const int& kind, const int& dev, float* mu,
+                                               float* d, float* dist, float* ek, float* bk, float* scal,
+                                               const Finish& finish) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
-    extern __shared__ __align__(16) float smem[];
-    __shared__ float dist[MAXN * MAXN];    // D_kl, k != l
-    __shared__ float ek[MAXN], bk[MAXN];
-    __shared__ float scal[2];              // a; UV: ||mu||^2, then gamma
-    const rcmarl_adaptive_attack_job& job = P.jobs[blockIdx.x];
-    const int n = job.n, nh = job.n_honest;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     constexpr int NW = ADA_THREADS / 32;
-    float* xs = smem;                              // [n_honest][n]
-    float* mu = smem + (int64_t)nh * n;            // [n]
-    float* d = mu + n;                             // [n]
-    for (int k = 0; k < nh; ++k) {
-        const float* src = job.msgs + (int64_t)job.honest[k] * job.msg_stride;
-        for (int p = tid; p < n; p += ADA_THREADS) xs[k * n + p] = __ldg(src + p);
-    }
-    __syncthreads();
     for (int p = tid; p < n; p += ADA_THREADS) {
         float s = 0.f;
         for (int k = 0; k < nh; ++k) s += xs[k * n + p];
         const float m = s / (float)nh;
         mu[p] = m;
-        if (job.dev == RCMARL_DEV_STD) {
+        if (dev == RCMARL_DEV_STD) {
             float q = 0.f;
             for (int k = 0; k < nh; ++k) q = fmaf(xs[k * n + p] - m, xs[k * n + p] - m, q);
             d[p] = -sqrtf(q / (float)nh);
-        } else if (job.dev == RCMARL_DEV_SGN) {
+        } else if (dev == RCMARL_DEV_SGN) {
             d[p] = m > 0.f ? -1.f : (m < 0.f ? 1.f : 0.f);
         }
     }
     __syncthreads();
-    if (job.dev == RCMARL_DEV_UV) {
+    if (dev == RCMARL_DEV_UV) {
         if (warp == 0) {
             const float q = warp_dot(mu, mu, n, lane);
             if (lane == 0) scal[1] = isfinite(q) ? sqrtf(q) : INFINITY;
@@ -641,7 +656,7 @@ __global__ void __launch_bounds__(ADA_THREADS) adaptive_attack_kernel(const __gr
         bool ok = a > 0.f && isfinite(a);
         for (int k = 0; k < nh; ++k) ok = ok && isfinite(ek[k]) && isfinite(bk[k]);
         float g = 0.f;
-        if (job.kind == RCMARL_ADAPT_MINMAX) {
+        if (kind == RCMARL_ADAPT_MINMAX) {
             float c = 0.f;
             for (int k = 0; k < nh; ++k)
                 for (int l = k + 1; l < nh; ++l) c = fmaxf(c, dist[k * MAXN + l]);
@@ -663,12 +678,126 @@ __global__ void __launch_bounds__(ADA_THREADS) adaptive_attack_kernel(const __gr
             if (ok && isfinite(c)) g = adaptive_root((float)nh * a, sb, se, c);
         }
         if (!isfinite(g)) g = 0.f;
+        finish(g);
+    }
+}
+
+__global__ void __launch_bounds__(ADA_THREADS) adaptive_attack_kernel(const __grid_constant__ AdaptiveParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];    // D_kl, k != l
+    __shared__ float ek[MAXN], bk[MAXN];
+    __shared__ float scal[2];              // a; UV: ||mu||^2, then gamma
+    const rcmarl_adaptive_attack_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nh = job.n_honest;
+    const int tid = threadIdx.x;
+    float* xs = smem;                              // [n_honest][n]
+    float* mu = smem + (int64_t)nh * n;            // [n]
+    float* d = mu + n;                             // [n]
+    for (int k = 0; k < nh; ++k) {
+        const float* src = job.msgs + (int64_t)job.honest[k] * job.msg_stride;
+        for (int p = tid; p < n; p += ADA_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    adaptive_gamma(xs, nh, n, job.kind, job.dev, mu, d, dist, ek, bk, scal, [&](float g) {
         scal[1] = g;
         if (job.gamma_out) *job.gamma_out = g;
-    }
+    });
     __syncthreads();
     const float t = job.scale * scal[1];
     for (int p = tid; p < n; p += ADA_THREADS) job.dst[p] = t == 0.f ? mu[p] : fmaf(t, d[p], mu[p]);
+}
+
+// Rule-aware Byzantine messages (rcmarl_tailored_attack, include/rcmarl.h): one CTA of 256 threads per job.  The real
+// slots are staged in shared memory, the honest ones first (in slot order, so that adaptive_gamma sees exactly the rows
+// rcmarl_adaptive_attack would), then mu, d, the candidate row and one work row.  Every crafted slot maps to the
+// candidate row, so the receiver's rule (resilient_mean_small per coordinate, or vector_rule) runs unchanged on the slot
+// list x(gamma_i), once per candidate; its output goes to the work row and one warp sums the objective.
+struct TailoredParams { rcmarl_tailored_attack_job jobs[RCMARL_MAX_JOBS]; };
+static_assert(ADA_THREADS == VEC_THREADS, "one CTA runs both the adaptive and the vector rule bodies");
+
+// The slot list of a tailored job: slot k at xs + off[k].
+struct SlotRows {
+    const float* xs;
+    const int* off;
+    __device__ __forceinline__ const float* operator()(int k) const { return xs + off[k]; }
+    __device__ __forceinline__ float at(int k, int p) const { return xs[off[k] + p]; }
+};
+
+// (at most one CTA per job and 117 KB of staging per CTA: the register budget of one CTA per SM keeps it free of spills)
+__global__ void __launch_bounds__(ADA_THREADS, 1) tailored_attack_kernel(const __grid_constant__ TailoredParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];
+    __shared__ float ek[MAXN], bk[MAXN], wt[MAXN], score[MAXN];
+    __shared__ float scal[2], total, best_o;
+    __shared__ int off[MAXN], best_i;
+    const rcmarl_tailored_attack_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    int nh = 0, nr = 0;                            // honest slots, real slots
+    for (int k = 0; k < nin; ++k) {
+        nh += (job.honest_mask >> k) & 1u;
+        nr += job.slots[k] >= 0 ? 1 : 0;
+    }
+    float* xs = smem;                              // [nr][n]: the honest slots, then the other real slots
+    float* mu = smem + (int64_t)nr * n;            // [n]
+    float* d = mu + n;                             // [n]
+    float* cand = d + n;                           // [n]: m(gamma_i), every crafted slot
+    float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
+    if (tid == 0) {
+        int h = 0, o = nh;
+        for (int k = 0; k < nin; ++k)
+            off[k] = job.slots[k] < 0 ? (int)(cand - xs) : ((job.honest_mask >> k) & 1u ? h++ : o++) * n;
+        best_o = -INFINITY;
+        best_i = 0;
+    }
+    __syncthreads();
+    for (int k = 0; k < nin; ++k) {
+        if (job.slots[k] < 0) continue;
+        const float* src = job.msgs + (int64_t)job.slots[k] * job.msg_stride;
+        float* row = xs + off[k];
+        for (int p = tid; p < n; p += ADA_THREADS) row[p] = __ldg(src + p);
+    }
+    __syncthreads();
+    constexpr int kind = RCMARL_ADAPT_MINMAX;
+    adaptive_gamma(xs, nh, n, kind, job.dev, mu, d, dist, ek, bk, scal, [&](float g) { scal[1] = g; });
+    __syncthreads();
+    const float prod = job.scale * scal[1];
+    const float range = isfinite(prod) ? prod : 0.f;   // Gamma = s * gamma_mm; 0 if that overflows (dst = mu)
+    const SlotRows rows{xs, off};
+    for (int i = 0; i <= RCMARL_TAILORED_STEPS; ++i) {
+        const float g = range * (float)i / (float)RCMARL_TAILORED_STEPS;
+        for (int p = tid; p < n; p += ADA_THREADS) cand[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
+        __syncthreads();                                              // x(gamma_i) complete; the last objective read
+        if (job.family == RCMARL_TAILOR_COORD) {
+            for (int p = tid; p < n; p += ADA_THREADS) {
+                float v[MAXN];
+#pragma unroll
+                for (int k = 0; k < MAXN; ++k) v[k] = k < nin ? rows.at(k, p) : 0.f;
+                z[p] = resilient_mean_small<MAXN>(v, nin, job.H, job.rule);
+            }
+        } else {
+            vector_rule(rows, n, nin, job.H, job.rule, z, z, dist, wt, score, total);
+        }
+        __syncthreads();                                              // R_j(x(gamma_i)) complete
+        if (warp == 0) {                                              // O_i = sum_p (R_p - mu_p)^2, one warp
+            float s = 0.f;
+            for (int p = lane; p < n; p += 32) {
+                const float e = z[p] - mu[p];
+                s = fmaf(e, e, s);
+            }
+            s = warp_sum(s);
+            if (lane == 0 && isfinite(s) && s > best_o) {             // ties to the smaller i; not finite: -inf
+                best_o = s;
+                best_i = i;
+            }
+        }
+    }
+    __syncthreads();
+    const float g = range * (float)best_i / (float)RCMARL_TAILORED_STEPS;
+    if (tid == 0 && job.gamma_out) *job.gamma_out = g;
+    for (int p = tid; p < n; p += ADA_THREADS) job.dst[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
 }
 
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
@@ -1253,6 +1382,68 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs, int n_jobs, v
         return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     adaptive_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+// the receiver model of a tailored job: a known family and rule, and an H that rule allows for n_in messages (the
+// checks of rcmarl_consensus_hidden and rcmarl_vector_aggregate)
+static bool bad_tailored_rule(const rcmarl_tailored_attack_job& q) {
+    if (q.H < 0 || q.H >= q.n_in) return true;
+    if (q.family == RCMARL_TAILOR_COORD) return bad_rule(q.rule, q.H, q.n_in);
+    if (q.family != RCMARL_TAILOR_VECTOR || q.rule < RCMARL_VEC_KRUM || q.rule > RCMARL_VEC_GMED) return true;
+    return (q.rule == RCMARL_VEC_KRUM || q.rule == RCMARL_VEC_MKRUM) && q.n_in < q.H + 3;
+}
+
+int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    TailoredParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_tailored_attack_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.honest_mask >> q.n_in) return RCMARL_ERR_ARG;            // a bit past the slot list
+        int n_crafted = 0;
+        for (int k = 0; k < q.n_in; ++k) {
+            if (q.slots[k] < -1) return RCMARL_ERR_ARG;
+            if (q.slots[k] == -1) {
+                if ((q.honest_mask >> k) & 1u) return RCMARL_ERR_ARG;  // a crafted slot marked honest
+                ++n_crafted;
+            }
+        }
+        if (n_crafted == 0 || q.honest_mask == 0u) return RCMARL_ERR_ARG;
+        if (bad_tailored_rule(q) || q.dev < RCMARL_DEV_UV || q.dev > RCMARL_DEV_SGN) return RCMARL_ERR_ARG;
+        if (!std::isfinite(q.scale) || q.scale < 0.f) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_in + 3) * q.n;
+        if (floats > RCMARL_TAILORED_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate: no written range (a dst, a gamma_out) may overlap a real slot's row of any job of the
+    // launch or another written range
+    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (jobs[j].gamma_out) {
+            float_range(jobs[j].gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < jobs[j].n_in; ++k)
+            if (jobs[j].slots[k] >= 0) {
+                float_range(jobs[j].msgs, jobs[j].slots[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
+                ++n_r;
+            }
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    // the staging bound is above the default 48 KB of dynamic shared memory
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)tailored_attack_kernel, (int)(sizeof(float) * RCMARL_TAILORED_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    tailored_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

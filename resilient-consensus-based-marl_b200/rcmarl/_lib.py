@@ -37,6 +37,10 @@ DEV_UV, DEV_STD, DEV_SGN = 0, 1, 2                # rcmarl_adaptive_dev
 ADAPTIVE_ATTACKS = {f"{k}_{d}": (kind, dev) for k, kind in (("minmax", ADAPT_MINMAX), ("minsum", ADAPT_MINSUM))
                     for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
 ADAPTIVE_MAX_FLOATS = 18 * 1536
+TAILOR_COORD, TAILOR_VECTOR = 0, 1                # rcmarl_tailored_family
+# rule-aware attacks (rcmarl_tailored_attack): candidate steps K and the staging bound; the names are TAILORED_ATTACKS
+TAILORED_STEPS = 32
+TAILORED_MAX_FLOATS = 19 * 1536
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -66,6 +70,12 @@ class AdaptiveAttackJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("gamma_out", c_fp), ("n", C.c_int32),
                 ("n_honest", C.c_int32), ("honest", C.c_int32 * MAX_NEIGHBOURS), ("kind", C.c_int32), ("dev", C.c_int32),
                 ("scale", C.c_float), ("reserved", C.c_int32)]
+
+
+class TailoredAttackJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("gamma_out", c_fp), ("n", C.c_int32),
+                ("n_in", C.c_int32), ("slots", C.c_int32 * MAX_NEIGHBOURS), ("honest_mask", C.c_uint32),
+                ("family", C.c_int32), ("rule", C.c_int32), ("H", C.c_int32), ("dev", C.c_int32), ("scale", C.c_float)]
 
 
 class ValueJob(C.Structure):
@@ -122,6 +132,7 @@ SYMBOLS = [
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
+    ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
@@ -220,22 +231,42 @@ def is_adaptive_attack(name):
     return isinstance(name, str) and name in ADAPTIVE_ATTACKS
 
 
+class TailoredKind(int):
+    """The kind check_attack gives a rule-aware attack: its rcmarl_adaptive_dev, as a type of its own so that it is
+    told apart from the rcmarl_attack_kind ids and the adaptive (kind, dev) pairs."""
+
+    def __repr__(self):
+        return f"TailoredKind({int(self)})"
+
+
+TAILORED_ATTACKS = {f"tailored_{d}": TailoredKind(dev) for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+
+
+def is_tailored_attack(name):
+    """True for the name of a rule-aware attack (rcmarl_tailored_attack): "tailored_uv", "tailored_std", "tailored_sgn"."""
+    return isinstance(name, str) and name in TAILORED_ATTACKS
+
+
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss" and the adaptive attacks also >= 0), as rcmarl_attack / rcmarl_adaptive_attack require (include/rcmarl.h).
-    kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss", and the pair (rcmarl_adaptive_kind,
-    rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the paper's attack)."""
+    "gauss", the adaptive and the tailored attacks also >= 0), as rcmarl_attack / rcmarl_adaptive_attack /
+    rcmarl_tailored_attack require (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and
+    "gauss", the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s
+    (1 is the paper's attack), and the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, whose parameter is
+    the range multiplier s."""
     try:
         name, param = attack
         param = float(param)
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
-    if not isinstance(name, str) or (name not in ATTACKS and name not in ADAPTIVE_ATTACKS):
-        raise RcmarlError(f"unknown attack {name!r}: expected one of {sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS)}")
-    nonneg = name == "gauss" or name in ADAPTIVE_ATTACKS
+    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS}
+    if not isinstance(name, str) or name not in known:
+        raise RcmarlError(f"unknown attack {name!r}: expected one of "
+                          f"{sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS)}")
+    nonneg = name == "gauss" or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
-    return (ADAPTIVE_ATTACKS[name] if name in ADAPTIVE_ATTACKS else ATTACKS[name]), param
+    return known[name], param
 
 
 def param_count(d_in, n_out):

@@ -320,6 +320,41 @@ def adaptive_attack(jobs):
     L.check(L.lib().rcmarl_adaptive_attack(a, len(a), _stream()), "rcmarl_adaptive_attack")
 
 
+def tailored_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack, scale, gamma_out=None):
+    """slots: the receiver's slot list (in_nodes order, own first), a message row or -1 for a crafted slot; honest: the
+    slot indices of the honest set; rule: the receiver's rule name (coordinate-wise "clip", "trim", "wmsr" or
+    distance-based "krum", "mkrum", "scclip", "gmed") or a (rcmarl_tailored_family, rule id) pair; attack: "tailored_uv",
+    "tailored_std", "tailored_sgn" or an rcmarl_adaptive_dev id; scale: the range multiplier s >= 0.  Names are checked
+    here, ids and limits by the library."""
+    j = L.TailoredAttackJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.gamma_out = ptr(gamma_out)
+    j.n_in = len(slots)
+    for k, v in enumerate(slots[:L.MAX_NEIGHBOURS]):
+        j.slots[k] = v
+    bad = [k for k in honest if not (isinstance(k, (int, np.integer)) and 0 <= k < len(slots))]
+    if bad:
+        raise L.RcmarlError(f"honest slot indices {bad} are outside the slot list of {len(slots)}")
+    j.honest_mask = sum(1 << int(k) for k in set(honest))
+    if isinstance(rule, str):
+        fam = L.TAILOR_VECTOR if L.is_vector_rule(rule) else L.TAILOR_COORD
+        rule = (fam, L.VECTOR_RULES[rule] if fam == L.TAILOR_VECTOR else L.agg_rule(rule))
+    j.family, j.rule, j.H = int(rule[0]), int(rule[1]), H
+    if isinstance(attack, str):
+        if not L.is_tailored_attack(attack):
+            raise L.RcmarlError(f"unknown tailored attack {attack!r}: expected one of {sorted(L.TAILORED_ATTACKS)}")
+        attack = L.TAILORED_ATTACKS[attack]
+    j.dev = int(attack)
+    j.scale = scale
+    j._keep = (dst, msgs, gamma_out)
+    return j
+
+
+def tailored_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.TailoredAttackJob, jobs)
+    L.check(L.lib().rcmarl_tailored_attack(a, len(a), _stream()), "rcmarl_tailored_attack")
+
+
 def vector_job(dst, msgs, msg_stride, n, in_nodes, H, rule, weights_out=None):
     """rule: distance-based rule name ("krum", "mkrum", "scclip", "gmed") or rcmarl_vector_rule id (include/rcmarl.h).
     Names are checked here, ids and limits by the library."""

@@ -108,8 +108,8 @@ class Trainer:
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
         self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
-        # gamma of each adaptive attack of the last epoch: row q = adapt_pairs[q], columns critic, TR
-        self.att_gamma = torch.zeros(len(self.adapt_pairs), 2, **f32) if self.adapt_pairs else None
+        # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
+        self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         self.adam_m = torch.zeros(NA, self.PA, **f32)
         self.adam_v = torch.zeros(NA, self.PA, **f32)
         self.adam_t = [0] * NA
@@ -190,6 +190,11 @@ class Trainer:
         # the pairs whose attacker runs a min-max / min-sum attack (rcmarl_adaptive_attack; check_attack gives its kind
         # as a (kind, dev) pair): their messages are crafted by a launch of their own
         self.adapt_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs) if isinstance(self.attack[b][0], tuple)]
+        # the pairs whose attacker runs a rule-aware attack (rcmarl_tailored_attack, kind L.TailoredKind): a launch of
+        # their own too, after the adaptive one
+        self.tailor_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                             if isinstance(self.attack[b][0], L.TailoredKind)]
+        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs
 
     def _receiver_nodes(self, j):
         """in_nodes[j] with each Byzantine neighbour replaced by the message row crafted for receiver j."""
@@ -207,14 +212,21 @@ class Trainer:
         return {i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(self.vec_agents)}
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum attack: float32 [2]}: the gamma of the message b
-        crafted for j in the last epoch of the last update round (include/rcmarl.h, rcmarl_adaptive_attack); entry 0 for
-        the critic, 1 for the team-reward net."""
-        if not self.adapt_pairs:
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum or a tailored attack: float32 [2]}: the gamma of
+        the message b crafted for j in the last epoch of the last update round (include/rcmarl.h, rcmarl_adaptive_attack;
+        for a tailored attack gamma_i*, rcmarl_tailored_attack); entry 0 for the critic, 1 for the team-reward net."""
+        if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
         self.d2h_bytes += g.nbytes
-        return {self.byz_pairs[e][:2]: g[q].copy() for q, e in enumerate(self.adapt_pairs)}
+        return {self.byz_pairs[e][:2]: g[q].copy() for q, e in enumerate(self.gamma_pairs)}
+
+    def _tailored_slots(self, j):
+        """(slots, honest) of receiver j for rcmarl_tailored_attack: _receiver_nodes(j) with every Byzantine pair row
+        replaced by -1 (a crafted slot), and the indices of the cooperative slots."""
+        slots = [-1 if r >= self.NA else r for r in self._receiver_nodes(j)]
+        honest = [k for k, i in enumerate(self.in_nodes[j]) if self.labels[i] == COOP]
+        return slots, honest
 
     def _try_peer_comm(self):
         """Set up the peer-memory exchange on every rank, or on none: the ranks agree (MIN all-reduce of a success
@@ -421,12 +433,21 @@ class Trainer:
 
         # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
         # (the min-max / min-sum pairs in a job list of their own, with the gamma of each message)
-        att_jobs, ada_jobs = [], []
+        # (and the tailored pairs in a third, against their receiver's own rule and H)
+        att_jobs, ada_jobs, tail_jobs = [], [], []
         ada_row = {e: q for q, e in enumerate(self.adapt_pairs)}
+        tail_row = {e: len(self.adapt_pairs) + q for q, e in enumerate(self.tailor_pairs)}
         for e, (b, j, honest) in enumerate(self.byz_pairs):
             kind, param = self.attack[b]
+            if e in tail_row:
+                slots, hon = self._tailored_slots(j)
+                rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
+                        else (L.TAILOR_COORD, self.aggregation[j]))
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
-                if e in ada_row:
+                if e in tail_row:
+                    tail_jobs.append(ops.tailored_attack_job(msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind,
+                                                             param, gamma_out=self.att_gamma[tail_row[e], t:t + 1]))
+                elif e in ada_row:
                     ada_jobs.append(ops.adaptive_attack_job(msgs[NA + e], msgs, P, P, honest, kind, param,
                                                             gamma_out=self.att_gamma[ada_row[e], t:t + 1]))
                 else:
@@ -435,6 +456,8 @@ class Trainer:
         att_groups = [ops.job_array(L.AttackJob, att_jobs[g:g + L.MAX_JOBS]) for g in range(0, len(att_jobs), L.MAX_JOBS)]
         ada_groups = [ops.job_array(L.AdaptiveAttackJob, ada_jobs[g:g + L.MAX_JOBS])
                       for g in range(0, len(ada_jobs), L.MAX_JOBS)]
+        tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(tail_jobs), L.MAX_JOBS)]
 
         # distance-based aggregates over the messages each receiver hears (crafted Byzantine ones included): at most 16
         # cooperative agents x 2 nets, so one launch per epoch
@@ -470,6 +493,9 @@ class Trainer:
                 self.launches += 1
             for g in ada_groups:                                           # no epoch dependence: no job changes
                 ops.adaptive_attack(g)
+                self.launches += 1
+            for g in tail_groups:                                          # no epoch dependence either
+                ops.tailored_attack(g)
                 self.launches += 1
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)

@@ -7,14 +7,17 @@ of it, means of the last 500 episodes, over the seeds; for a distance-based rule
 agent 4 gave its crafted message in the last epoch of the last round (Trainer.neighbour_weights, both nets), over the
 seeds.  The attack list (by default alie 1.0, ipm 0.5, gauss 0.3) may also name the min-max / min-sum attacks
 (rcmarl_adaptive_attack: minmax_uv, minmax_std, minmax_sgn, minsum_uv, minsum_std, minsum_sgn, scale 1 = the paper's
-attack); an entry is a name or name:param.  For those the table also reports the mean gamma of agent 4's messages in the
-last epoch of the last round (Trainer.attack_gammas, both nets and every receiver), over the seeds.
+attack) and the rule-aware attacks tuned against each receiver's own rule and H (rcmarl_tailored_attack: tailored_uv,
+tailored_std, tailored_sgn, range multiplier 2 by default); an entry is a name or name:param.  For those the table also
+reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in the last epoch of the last round
+(Trainer.attack_gammas, both nets and every receiver), over the seeds.
 
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
 alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
-minmax_std against the same round on gauss, alternated the same way.
+minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
+tailored_std (every cooperative agent on clip) against gauss.
 
     python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
                                  [rules=clip,trim,wmsr] [attacks=alie,ipm,gauss]
@@ -34,7 +37,7 @@ import bench                                   # noqa: E402
 import torch                                   # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
-PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3}
+PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0}
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -42,6 +45,7 @@ out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_ou
 RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
 VECTOR = ("krum", "mkrum", "scclip", "gmed")
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
+TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
 ATTACKS = tuple((a.split(":")[0], float(a.split(":")[1]) if ":" in a else PARAMS.get(a, 1.0))
                 for a in (sys.argv[6] if len(sys.argv) > 6 else "alie,ipm,gauss").split(","))
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
@@ -107,11 +111,11 @@ def rule_timing():
     return out
 
 
-def adaptive_timing():
-    """ms per update round (median over rounds) with agent 4 Byzantine on gauss and on minmax_std, at the benchmark's C2
+def adaptive_timing(attack="minmax_std"):
+    """ms per update round (median over rounds) with agent 4 Byzantine on gauss and on `attack`, at the benchmark's C2
     shape, the two trainers alternated round by round."""
     cfg = dict(bench.workload("C2", 0), labels=["Cooperative"] * 4 + ["Byzantine"])
-    trs = {a: Trainer(**dict(cfg, attack=(a, PARAMS.get(a, 1.0)))) for a in ("gauss", "minmax_std")}
+    trs = {a: Trainer(**dict(cfg, attack=(a, PARAMS.get(a, 1.0)))) for a in ("gauss", attack)}
     ms = {k: [] for k in trs}
     for r in range(timed_rounds + 1):
         for k, tr in trs.items():
@@ -125,13 +129,13 @@ def adaptive_timing():
             if r > 0:
                 ms[k].append(a.elapsed_time(b))
     out = {k: dict(median_ms=float(np.median(v)), rounds_ms=v) for k, v in ms.items()}
-    out["minmax_std_added_ms"] = out["minmax_std"]["median_ms"] - out["gauss"]["median_ms"]
+    out[f"{attack}_added_ms"] = out[attack]["median_ms"] - out["gauss"]["median_ms"]
     out["n_envs"] = cfg["n_envs"]
     return out
 
 
 def mean_gamma(tr):
-    """Mean gamma of the adaptive messages of the last epoch (critic and TR nets, every receiver)."""
+    """Mean gamma of the adaptive and tailored messages of the last epoch (critic and TR nets, every receiver)."""
     g = [x for v in tr.attack_gammas().values() for x in v.tolist()]
     return float(np.mean(g)) if g else None
 
@@ -153,15 +157,20 @@ result = dict(card=name, power_limit_w=power, n_blocks=n_blocks, n_envs=n_envs, 
 print(f"{name}, power limit {power} W: update round {result['timing']['Faulty']['median_ms']:.2f} ms (Faulty) vs "
       f"{result['timing']['Byzantine']['median_ms']:.2f} ms (Byzantine)", flush=True)
 vector = any(r in VECTOR for r in RULES)
-adaptive = any(a in ADAPTIVE for a, _ in ATTACKS)
+adaptive = any(a in ADAPTIVE + TAILORED for a, _ in ATTACKS)
+tailored = any(a in TAILORED for a, _ in ATTACKS)
 if vector:
     result["rule_timing"] = rt = rule_timing()
     print(f"update round with agent 4 Byzantine: clip {rt['clip']['median_ms']:.2f} ms, gmed {rt['gmed']['median_ms']:.2f} ms "
           f"({rt['gmed_added_ms']:+.3f}), mkrum {rt['mkrum']['median_ms']:.2f} ms ({rt['mkrum_added_ms']:+.3f})", flush=True)
-if adaptive:
+if any(a in ADAPTIVE for a, _ in ATTACKS):
     result["adaptive_timing"] = at = adaptive_timing()
     print(f"update round with agent 4 Byzantine: gauss {at['gauss']['median_ms']:.2f} ms, minmax_std "
           f"{at['minmax_std']['median_ms']:.2f} ms ({at['minmax_std_added_ms']:+.3f})", flush=True)
+if tailored:
+    result["tailored_timing"] = tt = adaptive_timing("tailored_std")
+    print(f"update round with agent 4 Byzantine: gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std "
+          f"{tt['tailored_std']['median_ms']:.2f} ms ({tt['tailored_std_added_ms']:+.3f})", flush=True)
 for rule in RULES:
     for attack in ATTACKS:
         team, est, byz, gam = [], [], [], []
@@ -192,7 +201,7 @@ for rule in RULES:
         if vector:
             cell["byz_weight"] = float(np.mean(byz)) if rule in VECTOR else None
         if adaptive:
-            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE else None
+            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED else None
         result["cells"].append(cell)
         print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}"
               + (f"  weight of agent 4 {cell['byz_weight']:.3f}" if cell.get("byz_weight") is not None else "")
@@ -219,9 +228,14 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
                 f"rule (median of {timed_rounds}, alternated): clip {rt['clip']['median_ms']:.2f} ms, gmed "
                 f"{rt['gmed']['median_ms']:.2f} ms ({rt['gmed_added_ms']:+.3f} ms), mkrum {rt['mkrum']['median_ms']:.2f} ms "
                 f"({rt['mkrum_added_ms']:+.3f} ms)\n")
-    if adaptive:
+    if "adaptive_timing" in result:
         at = result["adaptive_timing"]
         f.write(f"\nC2 update round at {at['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
                 f"gauss {at['gauss']['median_ms']:.2f} ms, minmax_std {at['minmax_std']['median_ms']:.2f} ms "
                 f"({at['minmax_std_added_ms']:+.3f} ms)\n")
+    if tailored:
+        tt = result["tailored_timing"]
+        f.write(f"\nC2 update round at {tt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
+                f"gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std {tt['tailored_std']['median_ms']:.2f} ms "
+                f"({tt['tailored_std_added_ms']:+.3f} ms)\n")
 print(open(os.path.join(out_dir, "attack_sweep.md")).read())

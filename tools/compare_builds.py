@@ -1,0 +1,87 @@
+"""Compare the outputs of the distance-based rules (rcmarl_vector_aggregate) and the min-max / min-sum attacks
+(rcmarl_adaptive_attack) between two builds of librcmarl.so, bit for bit.  Their kernels share their rule bodies with
+tailored_attack_kernel (vector_rule, adaptive_gamma in csrc/train_kernels.cu), so a change there may change their
+register allocation and SASS; this shows whether it changed anything they compute.
+
+Each build runs in its own process (RCMARL_LIB selects the library) on the same inputs: 24 messages of 1421 parameters
+around a common centre, four of them 1e3 times larger and one holding 1e30; every vector rule at n_in 1 .. 16 (H drawn
+per job, repeated in-nodes) with the weights, and every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
+gamma), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a build
+from before rcmarl_tailored_attack existed loads too.
+
+    python tools/compare_builds.py LIB_A LIB_B [out_dir]     -> prints whether every output is bitwise equal
+    (e.g. build the parent commit with `git archive HEAD~1 | tar -x -C DIR && make -C DIR/resilient-consensus-based-marl_b200/csrc`)
+"""
+import os
+import subprocess
+import sys
+import tempfile
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+CHILD = r'''
+import ctypes as C, sys
+import numpy as np, torch
+sys.path[:0] = [sys.argv[2]]
+from rcmarl import _lib as L, ops
+lib = C.CDLL(L.LIB_PATH)
+L.SYMBOLS[:] = [s for s in L.SYMBOLS if hasattr(lib, s[0])]       # an older build lacks the newer entry points
+rs = np.random.RandomState(77)
+P = 1421
+PC = (661, 761, 1101, 1421)
+X = (rs.randn(P) + rs.randn(24, P) * rs.uniform(0.05, 1, size=(24, 1))).astype(np.float32)
+X[20:] *= 1e3
+X[23, 5] = 1e30
+msgs = torch.as_tensor(X).cuda()
+outs = []
+for rule in ("krum", "mkrum", "scclip", "gmed"):
+    jobs, dsts, ws = [], [], []
+    for n_in in range(1, 17):
+        krum = rule in ("krum", "mkrum")
+        if krum and n_in < 3:
+            continue
+        H = int(rs.randint(0, n_in - 2 if krum else n_in))
+        d = torch.full((P,), float("nan"), device="cuda")
+        w = torch.full((16,), float("nan"), device="cuda")
+        nodes = [int(x) for x in rs.choice(24, size=n_in)]
+        jobs.append(ops.vector_job(d, msgs, P, PC[n_in % 4], nodes, H, rule, weights_out=w))
+        dsts.append(d)
+        ws.append(w)
+    ops.vector_aggregate(jobs)
+    outs += [d.cpu().numpy() for d in dsts] + [w.cpu().numpy() for w in ws]
+for a in ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn"):
+    jobs, dsts = [], []
+    for nh in range(1, 17):
+        d = torch.full((P + 1,), float("nan"), device="cuda")
+        honest = [int(x) for x in rs.choice(20, size=nh)]
+        jobs.append(ops.adaptive_attack_job(d[:P], msgs, P, PC[nh % 4], honest, a, 1.5, gamma_out=d[P:]))
+        dsts.append(d)
+    ops.adaptive_attack(jobs)
+    outs += [d.cpu().numpy() for d in dsts]
+np.savez(sys.argv[1], *outs)
+'''
+
+
+def dump(lib, path):
+    env = dict(os.environ, RCMARL_LIB=os.path.abspath(lib))
+    subprocess.check_call([sys.executable, "-c", CHILD, path, os.path.join(ROOT, "resilient-consensus-based-marl_b200")],
+                          env=env)
+    return np.load(path)
+
+
+def main():
+    if len(sys.argv) < 3:
+        sys.exit(__doc__)
+    out_dir = sys.argv[3] if len(sys.argv) > 3 else tempfile.mkdtemp()
+    a = dump(sys.argv[1], os.path.join(out_dir, "outputs_a.npz"))
+    b = dump(sys.argv[2], os.path.join(out_dir, "outputs_b.npz"))
+    diff = [k for k in a.files if a[k].tobytes() != b[k].tobytes()]
+    print(f"{len(a.files)} output arrays (vector_aggregate outputs and weights, adaptive_attack messages and gamma): "
+          + ("bitwise equal" if not diff and a.files == b.files else f"{len(diff)} differ: {diff[:8]}"))
+    sys.exit(1 if diff or a.files != b.files else 0)
+
+
+if __name__ == "__main__":
+    main()
