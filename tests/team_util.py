@@ -55,20 +55,21 @@ def loop_team(name):
                 desired=np.array([[1, 2], [3, 5], [0, 0]]), nrow=4, ncol=6, H=1, fast_lr=0.01)
 
 
-def oracle_agents(labels, w, H, fast, gamma, slow_lr=0.002):
-    """fp64 oracle agents; a malicious agent without a critic_local net starts it from its critic (as Trainer does)."""
+def oracle_agents(labels, w, H, fast, gamma, slow_lr=0.002, dtype=np.float64):
+    """Oracle agents (fp64 by default); a malicious agent without a critic_local net starts it from its critic (as
+    Trainer does)."""
     ags = []
     for i, lab in enumerate(labels):
         a, c, t = w[i][0], w[i][1], w[i][2]
         if lab == C:
-            ags.append(O.RPBCACOracleAgent(a, c, t, slow_lr, fast[i], gamma, H=H[i], dtype=np.float64))
+            ags.append(O.RPBCACOracleAgent(a, c, t, slow_lr, fast[i], gamma, H=H[i], dtype=dtype))
         elif lab == M:
             ags.append(O.MaliciousOracleAgent(a, c, t, slow_lr, fast[i], gamma,
-                                              critic_local_w=w[i][3] if len(w[i]) > 3 else None, dtype=np.float64))
+                                              critic_local_w=w[i][3] if len(w[i]) > 3 else None, dtype=dtype))
         elif lab == G:
-            ags.append(O.GreedyOracleAgent(a, c, t, slow_lr, fast[i], gamma, dtype=np.float64))
+            ags.append(O.GreedyOracleAgent(a, c, t, slow_lr, fast[i], gamma, dtype=dtype))
         else:
-            ags.append(O.FaultyOracleAgent(a, c, t, slow_lr, gamma, dtype=np.float64))
+            ags.append(O.FaultyOracleAgent(a, c, t, slow_lr, gamma, dtype=dtype))
     return ags
 
 
