@@ -79,11 +79,18 @@ int64_t rcmarl_param_count(int d_in, int n_out); /* packed length of one network
 int64_t rcmarl_workspace_bytes(int n_jobs, int max_params);
 
 /* How a one-wave grid of `sm_count` CTAs is split over `n_jobs` jobs that sweep `n_rows` buffer rows:
- * ctas_host[j] = CTAs of job j (kinds_host[j] = RCMARL_IN_*).  balanced = 0: equal shares, the plan of rcmarl_grad;
- * 1: shares sized by each job's cost per row, the plan of rcmarl_minibatch_fit (with n_rows = one mini-batch).
+ * ctas_host[j] = CTAs of job j (kinds_host[j] = RCMARL_IN_*).  balanced = 0: equal shares; 1: shares sized by each
+ * job's cost per row, the plan of rcmarl_grad and of rcmarl_minibatch_fit (with n_rows = one mini-batch).
  * Host arithmetic only (no device needed); exposed for tests and for sizing experiments. */
 int rcmarl_grad_grid_plan(int n_agents, const int32_t* kinds_host, int n_jobs, int loss_mode, int64_t n_rows, int balanced,
                           int sm_count, int32_t* ctas_host);
+
+/* The weight-gradient tile map of the fit kernels for a network of d_in inputs and n_out outputs ((10|15|32|48, 1) or
+ * (10|32, RCMARL_N_ACTIONS)).  info[6] = {tiles, activation entries per tile, delta entries per tile, row groups per
+ * warp, phase-2 warp-FFMA per 64-row chunk, first packed parameter accumulated outside the tiles (all later ones are)};
+ * params[t * rows * cols + ii * cols + jj] = packed parameter index of element (ii, jj) of tile t, -1 for padding
+ * (cap = capacity of params).  Host arithmetic only; exposed for tests. */
+int rcmarl_grad_tile_map(int d_in, int n_out, int32_t* info, int32_t* params, int64_t cap);
 
 /* ---------------------------------------------------------------------------
  * K4 / C5.  Coordinate-wise clipped ("winsorised") mean over the neighbour axis,

@@ -9,62 +9,95 @@
 //   phase 1 (forward + backward-data): every lane carries R = 2 buffer rows, so each broadcast weight quad
 //            (uniform LDS.128, 2 wavefronts) feeds 8 FFMA;
 //   phase 2 (weight gradients = sum over rows of outer products): the per-row activation / delta vectors are
-//            staged in a warp-private shared-memory tile and every lane owns one 8x8 register tile of the
-//            gradient (4 LDS.128 = 16 wavefronts per 64 FFMA); lanes are split into row groups so that
-//            NG x (number of tiles) <= 32 lanes are busy.  Accumulators stay in registers across ALL rows of the
-//            CTA; the output-layer gradient of the scalar nets is accumulated per lane in phase 1.
-// Reductions are fixed-order (lane -> warp -> CTA partial -> reduce_kernel): bitwise reproducible.
+//            staged in a warp-private shared-memory tile and every lane owns one TA x TD register tile of the
+//            gradient (TileLayout); lanes are split into row groups so that NG x (number of tiles) <= 32 lanes are
+//            busy.  Accumulators stay in registers across ALL rows of the CTA; the output-layer gradient of the
+//            scalar nets is accumulated per lane in phase 1.
+// Reductions are fixed-order (lane -> row group -> warp -> CTA partial -> reduce_kernel): bitwise reproducible.
 #pragma once
 #include "common.cuh"
 
 namespace rcmarl {
 
-__host__ __device__ constexpr int round8(int n) { return (n + 7) & ~7; }
+__host__ __device__ constexpr int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// Phase-2 tile shape of a network: TA activation entries x TD delta entries per lane.  The activation vectors are
+// [x(DIN), 1] and [h1(20), 1] (the "1" carries the bias gradient), the delta vectors are 20 wide.  A tile of
+// TA x TD costs TA*TD FFMA per step and the warp takes 64 / NG steps per chunk, so the phase-2 issue is
+// TA*TD / NG warp-FFMA per buffer row (DESIGN.md 4.2):
+//   critic (DIN 10): 11 x 4  -> [x, 1] is one block, [h1, 1] two (1 pad entry); 15 tiles, NG 2: 22 per row
+//   team reward (DIN 15): 8 x 7 -> [x, 1] two blocks, [h1, 1] three (3 pad entries), deltas 3 x 7 (1 pad); 15 tiles,
+//                         NG 2: 28 per row
+//   everything else (the actor, the 16-agent nets): 8 x 8 as before (the 8 x 8 shape gave 32 per row for both
+//   n_agents = 5 scalar nets).
+// Both shapes load 4 LDS.128 per step, as the 8 x 8 one does, so the shared-memory wavefronts per row do not grow.
+__host__ __device__ constexpr int tile_rows(int din, int nout) { return (nout == 1 && din == 10) ? 11 : 8; }
+__host__ __device__ constexpr int tile_cols(int din, int nout) {
+    return nout != 1 ? 8 : (din == 10 ? 4 : (din == 15 ? 7 : 8));
+}
 
 template <int DIN, int NOUT>
 struct TileLayout {
     static constexpr bool L3T = (NOUT > 1);             // output-layer gradient through tiles (actor) or per lane
-    static constexpr int LA1 = round8(DIN + 1);         // [x .. , 1, 0 pad]
+    static constexpr int TA = tile_rows(DIN, NOUT);     // activation entries per tile
+    static constexpr int TD = tile_cols(DIN, NOUT);     // delta entries per tile
+    // every vector is stored as blocks of TA (TD) entries, each padded to a 16-byte multiple so that a tile's block
+    // is SA / 4 (SD / 4) aligned LDS.128
+    static constexpr int SA = round4(TA), SD = round4(TD);
+    static constexpr int BA1 = ceil_div(DIN + 1, TA);   // blocks of [x .., 1]
+    static constexpr int BA2 = ceil_div(HID + 1, TA);   // blocks of [h1(20), 1] (and [h2(20), 1])
+    static constexpr int BD = ceil_div(HID, TD);        // blocks of delta1 / delta2
+    static constexpr int BD3 = ceil_div(NOUT, TD);      // blocks of dLoss/dlogits
     static constexpr int OA1 = 0;
-    static constexpr int OA2 = LA1;                     // [h1(20), 1, 0, 0, 0]
-    static constexpr int OA3 = OA2 + 24;                // [h2(20), 1, 0, 0, 0]   (only if L3T)
-    static constexpr int OD1 = OA3 + (L3T ? 24 : 0);    // delta1 (20) + 4 zeros
-    static constexpr int OD2 = OD1 + 24;                // delta2 (20) + 4 zeros
-    static constexpr int OD3 = OD2 + 24;                // dLoss/dlogits (NOUT) + zeros (only if L3T)
-    static constexpr int RAW = OD3 + (L3T ? 8 : 0);
+    static constexpr int OA2 = OA1 + BA1 * SA;
+    static constexpr int OA3 = OA2 + BA2 * SA;          // (only if L3T)
+    static constexpr int OD1 = OA3 + (L3T ? BA2 * SA : 0);
+    static constexpr int OD2 = OD1 + BD * SD;
+    static constexpr int OD3 = OD2 + BD * SD;           // (only if L3T)
+    static constexpr int RAW = OD3 + (L3T ? BD3 * SD : 0);
     // row stride: odd number of 16-byte units => conflict-free float4 stores within a quarter-warp
     static constexpr int RS = ((RAW / 4) % 2 == 0) ? RAW + 4 : RAW;
-    static constexpr int NT1 = (LA1 / 8) * 3;
-    static constexpr int NT2 = 9;
-    static constexpr int NT3 = L3T ? 3 : 0;
-    static constexpr int NT = NT1 + NT2 + NT3;          // 8x8 tiles covering all weight gradients
+    static constexpr int NT1 = BA1 * BD;
+    static constexpr int NT2 = BA2 * BD;
+    static constexpr int NT3 = L3T ? BA2 * BD3 : 0;
+    static constexpr int NT = NT1 + NT2 + NT3;          // tiles covering all weight gradients
     static_assert(NT <= 32, "tile count exceeds a warp");
     static constexpr int NG = 32 / NT;                  // row groups processed concurrently by one warp
     static constexpr int ROWS = 64;                     // rows per warp chunk (R = 2 per lane)
+    static_assert(ROWS % NG == 0, "every row group takes the same number of steps");
+    static constexpr int NACC = TA * TD;                // accumulators per lane
+    static constexpr int ACC_STRIDE = round4(NACC);     // per-lane slot of the CTA reduction buffer
+    static constexpr int PH2_FFMA = (ROWS / NG) * NACC; // phase-2 warp-FFMA per 64-row chunk
+
+    // entry of a vector held in slot s when it is stored in blocks of tb entries (padded to round4(tb) slots),
+    // -1 for a block's padding slot.  Entries past the vector's end are padding too (callers check).
+    __host__ __device__ static constexpr int slot_entry(int s, int tb) {
+        return (s % round4(tb)) < tb ? (s / round4(tb)) * tb + s % round4(tb) : -1;
+    }
 
     __device__ static __forceinline__ void tile_offsets(int t, int& aoff, int& doff) {
         if (t < NT1) {
-            aoff = OA1 + 8 * (t / 3); doff = OD1 + 8 * (t % 3);
+            aoff = OA1 + SA * (t / BD); doff = OD1 + SD * (t % BD);
         } else if (t < NT1 + NT2) {
-            t -= NT1; aoff = OA2 + 8 * (t / 3); doff = OD2 + 8 * (t % 3);
+            t -= NT1; aoff = OA2 + SA * (t / BD); doff = OD2 + SD * (t % BD);
         } else {
-            t -= NT1 + NT2; aoff = OA3 + 8 * t; doff = OD3;
+            t -= NT1 + NT2; aoff = OA3 + SA * (t / BD3); doff = OD3 + SD * (t % BD3);
         }
     }
-    // packed-parameter index of element (ii, jj) of tile t, -1 for padding
-    __device__ static __forceinline__ int tile_param(int t, int ii, int jj) {
+    // packed-parameter index of element (ii, jj) of tile t (ii < TA, jj < TD), -1 for padding
+    __host__ __device__ static int tile_param(int t, int ii, int jj) {
         if (t < NT1) {
-            const int i = 8 * (t / 3) + ii, j = 8 * (t % 3) + jj;
+            const int i = TA * (t / BD) + ii, j = TD * (t % BD) + jj;
             if (j >= HID) return -1;
             return i < DIN ? i * HID + j : (i == DIN ? off_b1(DIN) + j : -1);
         } else if (t < NT1 + NT2) {
             t -= NT1;
-            const int i = 8 * (t / 3) + ii, j = 8 * (t % 3) + jj;
+            const int i = TA * (t / BD) + ii, j = TD * (t % BD) + jj;
             if (j >= HID) return -1;
             return i < HID ? off_W2(DIN) + i * HID + j : (i == HID ? off_b2(DIN) + j : -1);
         } else if (t < NT) {
             t -= NT1 + NT2;
-            const int i = 8 * t + ii, o = jj;
+            const int i = TA * (t / BD3) + ii, o = TD * (t % BD3) + jj;
             if (o >= NOUT) return -1;
             return i < HID ? off_W3(DIN) + i * NOUT + o : (i == HID ? off_b3(DIN, NOUT) + o : -1);
         }
@@ -98,9 +131,13 @@ constexpr int grad_warps() {
 }
 
 // Relative cost of one buffer row for a job (FMA issue slots per lane-row): phase 1 (forward, output layer, backward-data)
-// plus phase 2 (the NT 8x8 tiles are spread over NG row groups, so a 64-row chunk takes 64 / NG tile steps of 64 FMA).
+// plus phase 2 as an 8x8 tiling would issue it (NT 8x8 tiles spread over NG row groups, so a 64-row chunk takes 64 / NG
+// tile steps of 64 FMA).  The model predates the per-network tile shapes of TileLayout and is kept as it is: with the
+// shipped shapes' phase-2 counts (22 and 28 per row instead of 32) the 132-SM plans would move from [17, 16] to
+// [18, 15] per team-reward / critic pair and from [43, 46, 43] to [40, 52, 40] for a mini-batch step; that shift is not
+// measured yet (DESIGN.md 4.2).
 __host__ __device__ constexpr int grad_row_cost(int din, int nout) {
-    const int la1 = round8(din + 1);
+    const int la1 = (din + 8) & ~7;                  // [x, 1] rounded up to 8x8 tiles
     const int nt = (la1 / 8) * 3 + 9 + (nout > 1 ? 3 : 0);
     const int ng = 32 / nt;
     return din * HID + 2 * HID * HID + 2 * HID * nout + 2048 / ng;
@@ -159,9 +196,29 @@ struct GradCore {
     uint32_t phase;
     // phase-2 assignment of this lane: tile `tile`, row group `grp`
     int grp, aoff, doff;
-    f2 acc[32];                            // 8x8 tile, packed as pairs over the delta index
+    float acc[L::NACC];                    // TA x TD tile, row-major over (activation, delta)
     float g3[L::L3T ? 1 : HID + 1];       // scalar nets: output-layer gradient per lane [W3(20) | b3]
     float loss;
+
+    // Store v[0 .. N) (and a constant 1 as entry N when ONE) into NSLOT slots at dst, in blocks of TB entries
+    // (L::slot_entry).  VARYING = true writes the quads that hold at least one entry of v (once per chunk); false writes
+    // the quads of constants only (once, write_pads).
+    template <int N, bool ONE, int TB, int NSLOT, bool VARYING>
+    __device__ __forceinline__ static void put_vec(float* dst, const float (&v)[N]) {
+#pragma unroll
+        for (int q = 0; q < NSLOT / 4; ++q) {
+            bool varying = false;
+            float w[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int e = L::slot_entry(4 * q + u, TB);
+                const bool in = e >= 0 && e < N;
+                varying |= in;
+                w[u] = in ? v[in ? e : 0] : ((ONE && e == N) ? 1.f : 0.f);
+            }
+            if (varying == VARYING) st4(dst + 4 * q, w[0], w[1], w[2], w[3]);
+        }
+    }
 
     // shared-memory carve-up + mbarrier init; nothing here touches global memory (may run before pdl_wait)
     __device__ __forceinline__ void setup(float* smem) {
@@ -183,27 +240,29 @@ struct GradCore {
         L::tile_offsets(tile, aoff, doff);
     }
 
-    // the constant columns of this lane's two tile rows ([.., 1, 0 pad] of the activations, zero pad of the deltas)
-    // never change: write them once instead of once per chunk (saves 3-4 of 22 STS.128 per row).  Must be repeated after
-    // cta_reduce (which reuses the tiles).
+    // the constant quads of this lane's two tile rows ([.., 1, 0 pad] of the activations, zero pad of the deltas)
+    // never change: write them once instead of once per chunk.  Must be repeated after cta_reduce (which reuses the
+    // tiles).
     __device__ __forceinline__ void write_pads() {
+        const float zx[DIN] = {}, zh[HID] = {}, zo[NOUT] = {};
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             float* rowp = wt + (lane + 32 * r) * L::RS;
-#pragma unroll
-            for (int q = 0; q < L::LA1 / 4; ++q)
-                if (4 * q >= DIN) st4(rowp + L::OA1 + 4 * q, 4 * q == DIN ? 1.f : 0.f, 0.f, 0.f, 0.f);
-            st4(rowp + L::OA2 + 20, 1.f, 0.f, 0.f, 0.f);
-            if constexpr (L::L3T) st4(rowp + L::OA3 + 20, 1.f, 0.f, 0.f, 0.f);
-            st4(rowp + L::OD1 + 20, 0.f, 0.f, 0.f, 0.f);
-            st4(rowp + L::OD2 + 20, 0.f, 0.f, 0.f, 0.f);
+            put_vec<DIN, true, L::TA, L::BA1 * L::SA, false>(rowp + L::OA1, zx);
+            put_vec<HID, true, L::TA, L::BA2 * L::SA, false>(rowp + L::OA2, zh);
+            if constexpr (L::L3T) {
+                put_vec<HID, true, L::TA, L::BA2 * L::SA, false>(rowp + L::OA3, zh);
+                put_vec<NOUT, false, L::TD, L::BD3 * L::SD, false>(rowp + L::OD3, zo);
+            }
+            put_vec<HID, false, L::TD, L::BD * L::SD, false>(rowp + L::OD1, zh);
+            put_vec<HID, false, L::TD, L::BD * L::SD, false>(rowp + L::OD2, zh);
         }
         __syncwarp();
     }
 
     __device__ __forceinline__ void zero_acc() {
 #pragma unroll
-        for (int e = 0; e < 32; ++e) acc[e] = pack2(0.f, 0.f);
+        for (int e = 0; e < L::NACC; ++e) acc[e] = 0.f;
 #pragma unroll
         for (int j = 0; j < (L::L3T ? 1 : HID + 1); ++j) g3[j] = 0.f;
         loss = 0.f;
@@ -281,28 +340,15 @@ struct GradCore {
                 }
                 dense20_rows<DIN, R>(sw, sw + off_b1(DIN), x, h1);
 #pragma unroll
-                for (int r = 0; r < R; ++r) {
-                    float* a1 = wt + (lane + 32 * r) * L::RS + L::OA1;
-#pragma unroll
-                    for (int q = 0; q < L::LA1 / 4; ++q) {
-                        if (4 * q >= DIN) continue;                       // constant columns: write_pads()
-                        float v[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const int k = 4 * q + u;
-                            v[u] = k < DIN ? x[r][k < DIN ? k : 0] : (k == DIN ? 1.f : 0.f);
-                        }
-                        st4(a1 + 4 * q, v[0], v[1], v[2], v[3]);
-                    }
-                }
+                for (int r = 0; r < R; ++r)
+                    put_vec<DIN, true, L::TA, L::BA1 * L::SA, true>(wt + (lane + 32 * r) * L::RS + L::OA1, x[r]);
             }
             dense20_rows<HID, R>(sw + off_W2(DIN), sw + off_b2(DIN), h1, h2);
             float d2[R][HID];
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 float* rowp = wt + (lane + 32 * r) * L::RS;
-#pragma unroll
-                for (int q = 0; q < 5; ++q) st4(rowp + L::OA2 + 4 * q, h1[r][4 * q], h1[r][4 * q + 1], h1[r][4 * q + 2], h1[r][4 * q + 3]);
+                put_vec<HID, true, L::TA, L::BA2 * L::SA, true>(rowp + L::OA2, h1[r]);
                 const float tgt = live[r] ? __ldg(job.target + row[r] * job.target_stride) : 0.f;
                 if constexpr (NOUT == 1) {
                     // Keras MSE (Appendix A.2): dLoss/dout = 2 (out - y) / B; the 2/B is applied by the caller
@@ -326,10 +372,8 @@ struct GradCore {
                     loss = fmaf(tgt, (mx + lse) - la, loss);
 #pragma unroll
                     for (int o = 0; o < NACT; ++o) g[o] = (p[o] - (o == a ? 1.f : 0.f)) * tgt;
-#pragma unroll
-                    for (int q = 0; q < 5; ++q) st4(rowp + L::OA3 + 4 * q, h2[r][4 * q], h2[r][4 * q + 1], h2[r][4 * q + 2], h2[r][4 * q + 3]);
-                    st4(rowp + L::OD3, g[0], g[1], g[2], g[3]);
-                    st4(rowp + L::OD3 + 4, g[4], 0.f, 0.f, 0.f);
+                    put_vec<HID, true, L::TA, L::BA2 * L::SA, true>(rowp + L::OA3, h2[r]);
+                    put_vec<NOUT, false, L::TD, L::BD3 * L::SD, true>(rowp + L::OD3, g);
 #pragma unroll
                     for (int j = 0; j < HID; ++j) {
                         float s = 0.f;
@@ -338,21 +382,34 @@ struct GradCore {
                         d2[r][j] = s * lrelu_grad_from_out(h2[r][j]);
                     }
                 }
-#pragma unroll
-                for (int q = 0; q < 5; ++q) st4(rowp + L::OD2 + 4 * q, d2[r][4 * q], d2[r][4 * q + 1], d2[r][4 * q + 2], d2[r][4 * q + 3]);
+                put_vec<HID, false, L::TD, L::BD * L::SD, true>(rowp + L::OD2, d2[r]);
             }
-            // delta1[i] = (W2[i][:] . delta2) * lrelu'(z1[i]) for both rows; each W2 quad feeds 8 FFMA
+            // delta1[i] = (W2[i][:] . delta2) * lrelu'(z1[i]) for both rows; each W2 quad feeds 8 FFMA.  Computed one
+            // stored quad (TD-blocked slot layout) at a time; quads of padding only are left to write_pads().
             f2 d2p[R][HID / 2];
 #pragma unroll
             for (int r = 0; r < R; ++r)
 #pragma unroll
                 for (int j = 0; j < HID / 2; ++j) d2p[r][j] = pack2(d2[r][2 * j], d2[r][2 * j + 1]);
 #pragma unroll
-            for (int q = 0; q < 5; ++q) {
+            for (int q = 0; q < L::BD * L::SD / 4; ++q) {
+                bool varying = false;
+#pragma unroll
+                for (int ii = 0; ii < 4; ++ii) {
+                    const int i = L::slot_entry(4 * q + ii, L::TD);
+                    varying |= i >= 0 && i < HID;
+                }
+                if (!varying) continue;
                 float d1[R][4];
 #pragma unroll
                 for (int ii = 0; ii < 4; ++ii) {
-                    const int i = 4 * q + ii;
+                    const int e = L::slot_entry(4 * q + ii, L::TD);
+                    if (e < 0 || e >= HID) {
+#pragma unroll
+                        for (int r = 0; r < R; ++r) d1[r][ii] = 0.f;
+                        continue;
+                    }
+                    const int i = e;
                     f2 s[R];
 #pragma unroll
                     for (int r = 0; r < R; ++r) s[r] = pack2(0.f, 0.f);
@@ -379,23 +436,26 @@ struct GradCore {
             }
         }
         __syncwarp();
-        // ---------------- phase 2: 8x8 register tile per lane, NG rows per step ----------------
+        // ---------------- phase 2: TA x TD register tile per lane, NG rows per step ----------------
         constexpr int kPh2Unroll = 4;
 #pragma unroll kPh2Unroll
         for (int it = 0; it < L::ROWS / L::NG; ++it) {
             const float* rp = wt + (it * L::NG + grp) * L::RS;
-            const float4 a0 = *reinterpret_cast<const float4*>(rp + aoff);
-            const float4 a1 = *reinterpret_cast<const float4*>(rp + aoff + 4);
-            const float4 d0 = *reinterpret_cast<const float4*>(rp + doff);
-            const float4 d1 = *reinterpret_cast<const float4*>(rp + doff + 4);
-            const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const f2 d[4] = {pack2(d0.x, d0.y), pack2(d0.z, d0.w), pack2(d1.x, d1.y), pack2(d1.z, d1.w)};
+            float a[L::SA], d[L::SD];
 #pragma unroll
-            for (int ii = 0; ii < 8; ++ii) {
-                const f2 aa = pack2(a[ii], a[ii]);
-#pragma unroll
-                for (int jp = 0; jp < 4; ++jp) acc[ii * 4 + jp] = fma2(aa, d[jp], acc[ii * 4 + jp]);
+            for (int q = 0; q < L::SA / 4; ++q) {
+                const float4 v = *reinterpret_cast<const float4*>(rp + aoff + 4 * q);
+                a[4 * q] = v.x; a[4 * q + 1] = v.y; a[4 * q + 2] = v.z; a[4 * q + 3] = v.w;
             }
+#pragma unroll
+            for (int q = 0; q < L::SD / 4; ++q) {
+                const float4 v = *reinterpret_cast<const float4*>(rp + doff + 4 * q);
+                d[4 * q] = v.x; d[4 * q + 1] = v.y; d[4 * q + 2] = v.z; d[4 * q + 3] = v.w;
+            }
+#pragma unroll
+            for (int ii = 0; ii < L::TA; ++ii)
+#pragma unroll
+                for (int jj = 0; jj < L::TD; ++jj) acc[ii * L::TD + jj] = fmaf(a[ii], d[jj], acc[ii * L::TD + jj]);
         }
         __syncwarp();
     }
@@ -408,18 +468,19 @@ struct GradCore {
     template <class ST>
     __device__ __forceinline__ void cta_reduce(ST store) {
     __syncthreads();
-    float* red = tiles;                               // [GRAD_WARPS][32][64]
+    constexpr int AS = L::ACC_STRIDE;
+    float* red = tiles;                               // [GRAD_WARPS][32][AS]
     {
-        float4* dst = reinterpret_cast<float4*>(red + (warp * 32 + lane) * 64);
+        float4* dst = reinterpret_cast<float4*>(red + (warp * 32 + lane) * AS);
 #pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            float4 v;
-            unpack2(acc[2 * q], v.x, v.y);
-            unpack2(acc[2 * q + 1], v.z, v.w);
-            dst[q] = v;
+        for (int q = 0; q < AS / 4; ++q) {
+            float v[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) v[u] = 4 * q + u < L::NACC ? acc[4 * q + u < L::NACC ? 4 * q + u : 0] : 0.f;
+            dst[q] = make_float4(v[0], v[1], v[2], v[3]);
         }
     }
-    float* red3 = red + GRAD_WARPS * 32 * 64;         // [GRAD_WARPS][HID + 2]: lane-private layer-3 sums + loss
+    float* red3 = red + GRAD_WARPS * 32 * AS;         // [GRAD_WARPS][HID + 2]: lane-private layer-3 sums + loss
     loss = warp_sum(loss);
     if (lane == 0) red3[warp * (HID + 2) + HID + 1] = loss;
     if constexpr (!L::L3T) {
@@ -430,14 +491,14 @@ struct GradCore {
         }
     }
     __syncthreads();
-    for (int q = threadIdx.x; q < L::NT * 64; q += blockDim.x) {
-        const int t = q >> 6, e = q & 63;
-        const int idx = L::tile_param(t, e >> 3, e & 7);
+    for (int q = threadIdx.x; q < L::NT * L::NACC; q += blockDim.x) {
+        const int t = q / L::NACC, e = q % L::NACC;
+        const int idx = L::tile_param(t, e / L::TD, e % L::TD);
         if (idx >= 0) {
             float s = 0.f;
             for (int w = 0; w < GRAD_WARPS; ++w)
 #pragma unroll
-                for (int g = 0; g < L::NG; ++g) s += red[(w * 32 + g * L::NT + t) * 64 + e];
+                for (int g = 0; g < L::NG; ++g) s += red[(w * 32 + g * L::NT + t) * AS + e];
             store(idx, s);
         }
     }
@@ -497,7 +558,7 @@ template <int NA, int DIN, int NOUT, int NW>
 constexpr int grad_smem_floats() {
     using L = TileLayout<DIN, NOUT>;
     constexpr int tiles = NW * L::ROWS * L::RS;
-    constexpr int red = NW * 32 * 64 + NW * (HID + 2);
+    constexpr int red = NW * 32 * L::ACC_STRIDE + NW * (HID + 2);
     static_assert(tiles >= red, "the CTA reduction buffer reuses the tile region");
     constexpr int stage = (grad_use_tma(NA) ? NW * L::ROWS * 3 * NA : 0) + 2 * NW + 8;   // staged rows + one mbarrier per warp
     return round4(param_count(DIN, NOUT)) + tiles + stage + 16;

@@ -942,11 +942,13 @@ static int grid_y_for(int64_t work_items, int n_jobs, int ctas_per_sm) {
 
 // Shares of a one-wave grid over n jobs: g[j] = CTAs of job j; pure host arithmetic (also behind rcmarl_grad_grid_plan
 // for the CPU tests).
-//   balanced = false (rcmarl_grad): equal shares, floor(SMs / n_jobs) CTAs per job.  All jobs then sweep the same rows in
-//     lock-step, which keeps the buffer rows they share in L2.
-//   balanced = true (rcmarl_minibatch_fit, whose chains read different rows): shares sized by cost.  A job's cost per row
-//     depends on its network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks; greedy: the job that
-//     currently finishes last gets the next CTA.
+//   balanced = false: equal shares, floor(SMs / n_jobs) CTAs per job (leaves SMs % n_jobs SMs idle, and the cheaper
+//     jobs' CTAs idle at the end of the launch).
+//   balanced = true (rcmarl_grad, rcmarl_minibatch_fit): shares sized by cost.  A job's cost per row depends on its
+//     network (grad_row_cost) and a CTA works in rounds of `gw` 64-row chunks; greedy: the job that currently finishes
+//     last gets the next CTA.  The fit kernels do ~2 000 FMA per 64-byte buffer row, so the full-batch launch reads its
+//     rows at ~15 % of HBM bandwidth even with no L2 reuse between jobs; sweeping the jobs in lock-step (equal shares)
+//     was measured slower than these shares (C2 fit launch 12.34 -> 12.05 ms on an H100 SXM, DESIGN.md 4.2).
 static void plan_shares(int n, const int* cost, int64_t nchunks, int gw, int sms, bool balanced, int* g) {
     int64_t units = (nchunks + gw - 1) / gw;
     if (units < 1) units = 1;
@@ -991,6 +993,18 @@ static int plan_grid(int n, const int* cost, int64_t nchunks, int gw, bool balan
 static int grad_job_cost(int na, int kind, int loss_mode) {
     if (loss_mode == RCMARL_LOSS_CE) return grad_row_cost(2 * na, NACT);
     return grad_row_cost(kind == RCMARL_IN_SA ? 3 * na : 2 * na, 1);
+}
+
+// host copy of TileLayout<DIN, NOUT> behind rcmarl_grad_tile_map
+template <int DIN, int NOUT>
+static int grad_tile_map(int32_t* info, int32_t* params, int64_t cap) {
+    using L = TileLayout<DIN, NOUT>;
+    info[0] = L::NT; info[1] = L::TA; info[2] = L::TD; info[3] = L::NG; info[4] = L::PH2_FFMA;
+    info[5] = L::L3T ? param_count(DIN, NOUT) : off_W3(DIN);
+    if (cap < (int64_t)L::NT * L::NACC) return RCMARL_ERR_ARG;
+    for (int t = 0; t < L::NT; ++t)
+        for (int e = 0; e < L::NACC; ++e) params[t * L::NACC + e] = L::tile_param(t, e / L::TD, e % L::TD);
+    return RCMARL_OK;
 }
 
 
@@ -1040,6 +1054,20 @@ int rcmarl_grad_grid_plan(int n_agents, const int32_t* kinds_host, int n_jobs, i
     return RCMARL_OK;
 }
 
+int rcmarl_grad_tile_map(int d_in, int n_out, int32_t* info, int32_t* params, int64_t cap) {
+    if (!info || !params) return RCMARL_ERR_ARG;
+    if (n_out == 1) {
+        if (d_in == 10) return grad_tile_map<10, 1>(info, params, cap);
+        if (d_in == 15) return grad_tile_map<15, 1>(info, params, cap);
+        if (d_in == 32) return grad_tile_map<32, 1>(info, params, cap);
+        if (d_in == 48) return grad_tile_map<48, 1>(info, params, cap);
+    } else if (n_out == NACT) {
+        if (d_in == 10) return grad_tile_map<10, NACT>(info, params, cap);
+        if (d_in == 32) return grad_tile_map<32, NACT>(info, params, cap);
+    }
+    return RCMARL_ERR_ARG;
+}
+
 int rcmarl_values(const rcmarl_rows* rows, const rcmarl_value_job* jobs, int n_jobs, void* stream) {
     if (int e = check_rows(rows)) return e;
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
@@ -1081,14 +1109,16 @@ int rcmarl_grad(const rcmarl_rows* rows, const rcmarl_grad_job* jobs, int n_jobs
         Q.n[j] = n + 1;
         if (n + 1 > maxn) maxn = n + 1;
     }
-    // equal CTA shares; each warp of a CTA takes one 64-row chunk per sweep
+    // CTA shares by cost; each warp of a CTA takes one 64-row chunk per sweep
+    int cost[RCMARL_MAX_JOBS];
+    for (int j = 0; j < n_jobs; ++j) cost[j] = grad_job_cost(NA, jobs[j].kind, loss_mode);
     const bool ce = loss_mode == RCMARL_LOSS_CE;
     const int cpc = NA == 5 ? (ce ? grad_warps<5, RCMARL_LOSS_CE>() : grad_warps<5, RCMARL_LOSS_MSE>())
                             : (ce ? grad_warps<16, RCMARL_LOSS_CE>() : grad_warps<16, RCMARL_LOSS_MSE>());
     P.partial = (float*)ws;
     P.n_jobs = n_jobs;
     P.stride = maxn;
-    const int n_ctas = plan_grid(n_jobs, nullptr, (rows->n_rows + 63) / 64, cpc, false, P.cta_first);
+    const int n_ctas = plan_grid(n_jobs, cost, (rows->n_rows + 63) / 64, cpc, true, P.cta_first);
     if ((int64_t)n_ctas * maxn * (int64_t)sizeof(float) > ws_bytes) return RCMARL_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
     const int e = NA == 5 ? (ce ? launch_grad<5, RCMARL_LOSS_CE>(P, n_ctas, st) : launch_grad<5, RCMARL_LOSS_MSE>(P, n_ctas, st))
@@ -1146,7 +1176,7 @@ int rcmarl_minibatch_fit(const rcmarl_rows* rows, const rcmarl_grad_job* gjobs, 
     }
     const int cpc = NA == 5 ? grad_warps<5, RCMARL_LOSS_MSE>() : grad_warps<16, RCMARL_LOSS_MSE>();
     const int64_t n_rows_mb = (int64_t)(n_times < mb_times ? n_times : mb_times) * rows->n_envs;
-    // CTA shares by cost (the chains do not share rows in L2 the way the lock-step full-batch jobs do).  A mapping with every
+    // CTA shares by cost, as in rcmarl_grad.  A mapping with every
     // CTA serving every chain in turn (reduction of a chain hidden behind the other chains' turns) was measured
     // slower and removed.
     const int n_ctas = plan_grid(n_jobs, cost, (n_rows_mb + 63) / 64, cpc, true, P.cta_first);

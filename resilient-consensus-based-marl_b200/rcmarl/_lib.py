@@ -127,6 +127,7 @@ SYMBOLS = [
     ("rcmarl_workspace_bytes", C.c_int64, [C.c_int, C.c_int]),
     ("rcmarl_grad_grid_plan", C.c_int, [C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(C.c_int32)]),
+    ("rcmarl_grad_tile_map", C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int64]),
     ("rcmarl_clip_mean", C.c_int, [c_fp, C.c_int, C.c_int64, C.c_int64, C.c_int, c_fp, c_fp]),
     ("rcmarl_consensus_hidden", C.c_int, [C.POINTER(ConsensusJob), C.c_int, c_fp]),
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
