@@ -315,6 +315,40 @@ typedef struct {
 } rcmarl_vector_job;
 int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
+/* Spectral resilient aggregation of whole messages (rcmarl_dnc_aggregate): the divide-and-conquer (DnC) rule of
+ * Shejwalkar & Houmansadr, "Manipulating the Byzantine" (NDSS 2021, section VI, Algorithm 2), which removes the messages
+ * that lie furthest along the top principal direction of the centred messages.  It takes rcmarl_vector_job with
+ * rule = RCMARL_SPECTRAL_DNC; its n = n_in messages x_0 .. x_{n-1} (x_0 the receiver's own; repeats in in_nodes count)
+ * each hold P = job.n packed parameters.
+ *   Flagged  F = the rows holding +-inf; U = every other row, in index order, m = |U|.  If m = 0: out = x_0, w = e_0.
+ *   Centre   in fp64 from the fp32 inputs: mu_p = (sum_{k in U, index order} x_k,p) / m,  c_k = x_k - mu (k in U),
+ *            G_kl = sum_p c_k,p c_l,p (each G_kl summed by one warp: lane-strided fma partials, then the fixed xor
+ *            butterfly).  fp64 holds the square of any finite fp32 value, so only +-inf needs flagging.
+ *   Scores   lambda = the largest eigenvalue of G and u its unit eigenvector, by cyclic Jacobi in fp64 (rows p < q
+ *            in order; a rotation is skipped, and G_pq set to 0, when 100 |G_pq| is below the rounding of |G_pp| and
+ *            of |G_qq|; at most RCMARL_DNC_SWEEPS sweeps, ending early after a sweep without a rotation); lambda is
+ *            the largest diagonal entry (ties to the lower index).  score_k = lambda u_k^2 = <c_k, v>^2 for k in U (v
+ *            the top right singular vector of the centred rows, the paper's outlier score); score_k = +inf for k in F.
+ *   Removal  max(|F|, H) rows are removed: every row of F, then the H - |F| highest scores of U (equal scores: the
+ *            higher index first).  I = the kept rows.
+ *   Output   out = (sum_{k in I, index order} x_k) / |I| in fp32 (as multi-Krum's), w_k = 1/|I| on I, 0 elsewhere;
+ *            weights_out receives w when it is not NULL.
+ * 0 <= H < n_in; H = 0 gives the plain mean, and the rule may remove the receiver's own message.  Every coordinate is
+ * used in one iteration that removes H rows (the paper's b = P, niters = 1 and c = 1, with H as its bound m on the
+ * number of malicious messages): with every coordinate, each further iteration would pick the same rows.  When lambda is repeated or nearly so, u (and
+ * so the selection) is not unique: which of the candidate directions the Jacobi sweep returns is fixed, but it is not
+ * a property of the messages.  NaN inputs are not supported.  One CTA per job, fixed summation orders, no atomics:
+ * bitwise reproducible, independent of the job order and of how jobs are split over launches.  dst[0:n] = out.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst and weights_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null
+ * dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, a rule other than RCMARL_SPECTRAL_DNC,
+ * H outside [0, n_in), (n_in + 2) * n > RCMARL_DNC_MAX_FLOATS (the staging bound: the fp32 messages and the fp64 mean
+ * are staged in shared memory), a dst or weights_out that overlaps an in-node row of any job of the launch, and two
+ * written ranges (dsts, weights_outs) of the launch that overlap. */
+#define RCMARL_DNC_SWEEPS 32
+#define RCMARL_DNC_MAX_FLOATS (48 * 1024)
+typedef enum { RCMARL_SPECTRAL_DNC = 0 } rcmarl_spectral_rule;
+int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

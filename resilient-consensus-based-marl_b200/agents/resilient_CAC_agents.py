@@ -5,7 +5,8 @@ Same constructor and method names, argument meaning and mutation conventions as 
   *_update_local            return (message copy, loss) and leave the agent's own networks untouched (:113,120)
   resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166), or
                                  their trimmed / W-MSR mean with aggregation="trim" / "wmsr", or the hidden layers
-                                 of a distance-based aggregate ("krum", "mkrum", "scclip", "gmed") of whole messages
+                                 of a distance-based ("krum", "mkrum", "scclip", "gmed") or divide-and-conquer
+                                 ("dnc") aggregate of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
@@ -29,8 +30,8 @@ class RPBCAC_agent():
         self.H = H
         # resilient aggregation rule of every consensus step: "clip" (the reference's), "trim" or "wmsr"
         # (include/rcmarl.h, rcmarl_agg_rule), or a distance-based rule over whole messages: "krum", "mkrum", "scclip"
-        # or "gmed" (rcmarl_vector_rule)
-        if not L.is_vector_rule(aggregation):
+        # or "gmed" (rcmarl_vector_rule), or the spectral rule "dnc" (divide-and-conquer, rcmarl_dnc_aggregate)
+        if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation)):
             L.agg_rule(aggregation)
         self.aggregation = aggregation
         self.n_actions = self.actor.output_shape[1]
@@ -46,7 +47,7 @@ class RPBCAC_agent():
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
         v = v.reshape(v.shape[0], -1)
-        if L.is_vector_rule(self.aggregation):    # the rows as whole vectors: out = sum_k w_k v_k
+        if self._whole_messages():                # the rows as whole vectors: out = sum_k w_k v_k
             out = self._with_aggregate(v)[-1]
         elif L.agg_rule(self.aggregation) == L.AGG_CLIP:
             out = ops.clip_mean(v, self.H)
@@ -57,18 +58,28 @@ class RPBCAC_agent():
                                                     self.aggregation)])
         return Tensor(out.reshape(shape))
 
+    def _whole_messages(self):
+        """True if the rule aggregates whole messages (a distance-based rule or dnc)."""
+        return L.is_vector_rule(self.aggregation) or L.is_spectral_rule(self.aggregation)
+
     def _with_aggregate(self, stack):
-        """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based rule."""
+        """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based or
+        dnc rule."""
         n, P = stack.shape
-        L.check_vector_rule(self.aggregation, self.H, n)
         out = torch.cat([stack, torch.empty(1, P, dtype=stack.dtype, device=stack.device)])
-        ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
+        if L.is_spectral_rule(self.aggregation):
+            L.check_spectral_rule(self.H, n)
+            ops.dnc_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, L.SPECTRAL_DNC)])
+        else:
+            L.check_vector_rule(self.aggregation, self.H, n)
+            ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
         return out
 
     def _consensus_inputs(self, stack):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
-        distance-based rule's aggregate becomes the single in-node under clip, which returns it exactly, as in Trainer."""
-        if L.is_vector_rule(self.aggregation):
+        distance-based or dnc rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
+        Trainer."""
+        if self._whole_messages():
             return self._with_aggregate(stack), [stack.shape[0]], 0, "clip"
         return stack, list(range(stack.shape[0])), self.H, self.aggregation
 

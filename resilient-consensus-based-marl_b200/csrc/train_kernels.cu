@@ -11,6 +11,8 @@
 //   attack_kernel   Byzantine messages crafted per receiver (ALIE / IPM / Gaussian, rcmarl_attack)
 //   vector_agg_kernel  distance-based rules over whole messages (Krum, multi-Krum, self-centred clipping, geometric
 //                   median; rcmarl_vector_aggregate)
+//   dnc_agg_kernel  divide-and-conquer: removes the messages furthest along the top principal direction
+//                   (rcmarl_dnc_aggregate)
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
@@ -568,6 +570,149 @@ __global__ void __launch_bounds__(VEC_THREADS) vector_agg_kernel(const __grid_co
         __syncthreads();
         if (tid < nin) job.weights_out[tid] = wt[tid];
     }
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// Divide-and-conquer (rcmarl_dnc_aggregate, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The fp32
+// messages and the fp64 mean of the unflagged ones are staged in shared memory; every Gram entry is summed by ONE warp
+// (lane-strided fp64 fma partials, then the fixed xor butterfly), so its value does not depend on which warp takes it.
+// The Jacobi eigen-solve runs on warp 0, one lane per row of the m x m matrix, with every lane computing each rotation
+// identically; scores, selection and weights also run on warp 0, and the output takes one thread per coordinate.
+__global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ double A[MAXN * MAXN];              // G, reduced in place by the Jacobi rotations
+    __shared__ double V[MAXN * MAXN];              // the accumulated rotations: column c is the eigenvector of A[c][c]
+    __shared__ int ulist[MAXN];                    // U in index order
+    __shared__ int flagged[MAXN];
+    __shared__ float wt[MAXN];
+    __shared__ int m_s;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    double* mu = reinterpret_cast<double*>(smem);  // [n]
+    float* xs = smem + 2 * (int64_t)n;             // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    for (int k = warp; k < nin; k += NW) {
+        bool inf = false;
+        for (int p = lane; p < n; p += 32) inf |= isinf(xs[k * n + p]);
+        inf = __any_sync(0xffffffffu, inf);
+        if (lane == 0) flagged[k] = inf ? 1 : 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int m = 0;
+        for (int k = 0; k < nin; ++k)
+            if (!flagged[k]) ulist[m++] = k;
+        m_s = m;
+    }
+    __syncthreads();
+    const int m = m_s;
+    if (m > 0) {
+        const double inv_m = 1.0 / (double)m;
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            double s = 0.0;
+            for (int a = 0; a < m; ++a) s += (double)xs[ulist[a] * n + p];
+            mu[p] = s * inv_m;
+        }
+        __syncthreads();
+        for (int t = warp; t < m * (m + 1) / 2; t += NW) {          // pairs a <= b of U positions
+            int a = 0, r = t;
+            while (r >= m - a) { r -= m - a; ++a; }
+            const int b = a + r;
+            const float* xa = xs + ulist[a] * n;
+            const float* xb = xs + ulist[b] * n;
+            double s = 0.0;
+            for (int p = lane; p < n; p += 32) s = fma((double)xa[p] - mu[p], (double)xb[p] - mu[p], s);
+            s = warp_sum_f64(s);
+            if (lane == 0) { A[a * MAXN + b] = s; A[b * MAXN + a] = s; }
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const int k = lane;
+            if (k < m)
+                for (int c = 0; c < m; ++c) V[k * MAXN + c] = c == k ? 1.0 : 0.0;
+            __syncwarp();
+            for (int sweep = 0; sweep < RCMARL_DNC_SWEEPS; ++sweep) {
+                bool rotated = false;
+                for (int p = 0; p < m - 1; ++p) {
+                    for (int q = p + 1; q < m; ++q) {
+                        const double apq = A[p * MAXN + q], app = A[p * MAXN + p], aqq = A[q * MAXN + q];
+                        const double g = 100.0 * fabs(apq);
+                        __syncwarp();                               // every lane has read them
+                        if (apq == 0.0 || (fabs(app) + g == fabs(app) && fabs(aqq) + g == fabs(aqq))) {
+                            if (k == 0) { A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0; }
+                            __syncwarp();
+                            continue;
+                        }
+                        rotated = true;
+                        const double theta = (aqq - app) / (2.0 * apq);
+                        const double tt = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + hypot(theta, 1.0));
+                        const double c = 1.0 / sqrt(fma(tt, tt, 1.0)), s = tt * c;
+                        if (k < m && k != p && k != q) {
+                            const double akp = A[k * MAXN + p], akq = A[k * MAXN + q];
+                            const double nkp = c * akp - s * akq, nkq = s * akp + c * akq;
+                            A[k * MAXN + p] = nkp; A[p * MAXN + k] = nkp;
+                            A[k * MAXN + q] = nkq; A[q * MAXN + k] = nkq;
+                        } else if (k == p) {
+                            A[p * MAXN + p] = app - tt * apq;
+                            A[q * MAXN + q] = aqq + tt * apq;
+                            A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0;
+                        }
+                        if (k < m) {
+                            const double vkp = V[k * MAXN + p], vkq = V[k * MAXN + q];
+                            V[k * MAXN + p] = c * vkp - s * vkq;
+                            V[k * MAXN + q] = s * vkp + c * vkq;
+                        }
+                        __syncwarp();
+                    }
+                }
+                if (!rotated) break;
+            }
+            // lambda = the largest diagonal entry (ties to the lower index), score of U position a = lambda * u_a^2
+            int top = 0;
+            for (int c = 1; c < m; ++c)
+                if (A[c * MAXN + c] > A[top * MAXN + top]) top = c;
+            const double lambda = A[top * MAXN + top];
+            // U position of lane k's row (k < nin), or -1 if flagged; its score
+            int pos = -1;
+            for (int a = 0; a < m; ++a)
+                if (ulist[a] == k) pos = a;
+            double sc = INFINITY;
+            if (pos >= 0) {
+                const double u = V[pos * MAXN + top];
+                sc = lambda * (u * u);
+            }
+            // rows above k in the removal order: a higher score, or an equal one at a higher index (F is all +inf)
+            const int n_flag = nin - m, n_rm = max(n_flag, job.H);
+            int above = 0;
+            for (int l = 0; l < nin; ++l) {
+                const double sl = __shfl_sync(0xffffffffu, sc, l);
+                if (l != k && l < nin) above += (sl > sc || (sl == sc && l > k)) ? 1 : 0;
+            }
+            if (k < nin) wt[k] = above < n_rm ? 0.f : 1.f / (float)(nin - n_rm);
+        }
+    } else if (tid < nin) {
+        wt[tid] = tid == 0 ? 1.f : 0.f;                              // every row flagged: out = x_0
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = |I| (1 when every row is flagged)
+        float s = 0.f, cnt = 0.f;
+        for (int k = 0; k < nin; ++k)
+            if (wt[k] != 0.f) { s += xs[k * n + p]; cnt += 1.f; }
+        job.dst[p] = s / cnt;
+    }
+    if (job.weights_out && tid < nin) job.weights_out[tid] = wt[tid];
 }
 
 // Min-max / min-sum Byzantine messages (rcmarl_adaptive_attack, include/rcmarl.h): one CTA of 256 threads per job.  The
@@ -1369,6 +1514,45 @@ int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* str
     if (int e = opt_in_smem((const void*)vector_agg_kernel, (int)(sizeof(float) * RCMARL_VECTOR_MAX_FLOATS), opted)) return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     vector_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.rule != RCMARL_SPECTRAL_DNC || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_in + 2) * q.n;
+        if (floats > RCMARL_DNC_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate: no written range (a dst, a weights_out) may overlap an in-node row of any job of the
+    // launch or another written range
+    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (jobs[j].weights_out) {
+            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
+            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)dnc_agg_kernel, (int)(sizeof(float) * RCMARL_DNC_MAX_FLOATS), opted)) return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    dnc_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

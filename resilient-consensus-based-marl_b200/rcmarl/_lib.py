@@ -41,6 +41,10 @@ TAILOR_COORD, TAILOR_VECTOR = 0, 1                # rcmarl_tailored_family
 # rule-aware attacks (rcmarl_tailored_attack): candidate steps K and the staging bound; the names are TAILORED_ATTACKS
 TAILORED_STEPS = 32
 TAILORED_MAX_FLOATS = 19 * 1536
+SPECTRAL_DNC = 0                                  # rcmarl_spectral_rule
+SPECTRAL_RULES = {"dnc": SPECTRAL_DNC}
+DNC_SWEEPS = 32
+DNC_MAX_FLOATS = 48 * 1024
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -132,6 +136,7 @@ SYMBOLS = [
     ("rcmarl_consensus_hidden", C.c_int, [C.POINTER(ConsensusJob), C.c_int, c_fp]),
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -225,6 +230,19 @@ def check_vector_rule(rule, H, n_in):
         raise RcmarlError(f"aggregation {rule!r} with H={H} needs 0 <= H < n_in" + (" and n_in >= H + 3" if krum else "")
                           + f" (n_in={n_in}, at most {MAX_NEIGHBOURS})")
     return VECTOR_RULES[rule]
+
+
+def is_spectral_rule(rule):
+    """True for the name of a spectral rule (rcmarl_spectral_rule): "dnc"."""
+    return isinstance(rule, str) and rule in SPECTRAL_RULES
+
+
+def check_spectral_rule(H, n_in):
+    """Raise RcmarlError unless DnC (rcmarl_dnc_aggregate, include/rcmarl.h) allows H out of n_in messages:
+    1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  Returns the rcmarl_spectral_rule id."""
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
+        raise RcmarlError(f"aggregation 'dnc' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
+    return SPECTRAL_DNC
 
 
 def is_adaptive_attack(name):

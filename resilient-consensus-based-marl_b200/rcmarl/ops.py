@@ -378,6 +378,12 @@ def vector_aggregate(jobs):
     L.check(L.lib().rcmarl_vector_aggregate(a, len(a), _stream()), "rcmarl_vector_aggregate")
 
 
+def dnc_aggregate(jobs):
+    """rcmarl_dnc_aggregate over rcmarl_vector_job jobs (vector_job(..., rule=L.SPECTRAL_DNC, ...))."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_dnc_aggregate(a, len(a), _stream()), "rcmarl_dnc_aggregate")
+
+
 def reward_mix(r, agents, out=None, scale=1.0):
     """r: [rows, n_agents]; out[row] = scale * sum_k r[row, agents[k]] / len(agents) in list order."""
     n_rows, n_agents = r.shape

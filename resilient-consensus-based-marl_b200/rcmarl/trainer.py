@@ -61,17 +61,30 @@ class Trainer:
         # A distance-based rule ("krum", "mkrum", "scclip", "gmed") aggregates whole messages into one extra message row
         # per such agent; its consensus and team jobs then read that row as their only in-node under clip, which returns
         # it exactly (the projection target phi.W3 + b3 is linear in the head).
+        # The spectral rule "dnc" (divide-and-conquer) does the same through a launch of its own.
         self.vector_rule = [L.VECTOR_RULES[a] if L.is_vector_rule(a) else None for a in agg] + [None] * (NA - n_real)
-        self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) else L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
+        self.dnc = [L.is_spectral_rule(a) for a in agg] + [False] * (NA - n_real)
+        self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) or L.is_spectral_rule(a) else L.agg_rule(a) for a in agg] \
+            + [L.AGG_CLIP] * (NA - n_real)
         for i in self.coop:
             if self.vector_rule[i] is not None:
                 L.check_vector_rule(agg[i], self.H[i], len(self.in_nodes[i]))
+            elif self.dnc[i]:
+                L.check_spectral_rule(self.H[i], len(self.in_nodes[i]))
             else:
                 L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
         self._init_attacks(attack)
-        # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows
+        for e in self.tailor_pairs:                # rcmarl_tailored_attack does not model the DnC rule
+            b, j, _ = self.byz_pairs[e]
+            if self.dnc[j]:
+                raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose rule 'dnc' "
+                                    "the tailored attack does not model")
+        # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
+        # that of each cooperative agent on dnc
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
         self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
+        self.dnc_agents = [i for i in self.coop if self.dnc[i]]
+        self.dnc_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + q for q, i in enumerate(self.dnc_agents)}
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -102,12 +115,14 @@ class Trainer:
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
-        # vec_row[i] the aggregate of cooperative agent i's distance-based rule
-        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents)
+        # vec_row[i] / dnc_row[i] the aggregate of cooperative agent i's distance-based / dnc rule
+        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
         self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
+        # ... and of each dnc aggregate: row 2q critic, 2q + 1 TR of dnc_agents[q]
+        self.dnc_weights = torch.zeros(2 * len(self.dnc_agents), L.MAX_NEIGHBOURS, **f32) if self.dnc_agents else None
         # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         self.adam_m = torch.zeros(NA, self.PA, **f32)
@@ -202,14 +217,17 @@ class Trainer:
         return [row.get(k, k) for k in self.in_nodes[j]]
 
     def neighbour_weights(self):
-        """{cooperative agent i with a distance-based rule: float32 [2, n_in]}: the weight w_k its rule gave each
-        in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in the
-        last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net."""
-        if not self.vec_agents:
-            return {}
-        w = self.vec_weights.cpu().numpy()
-        self.d2h_bytes += w.nbytes
-        return {i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(self.vec_agents)}
+        """{cooperative agent i with a distance-based or the dnc rule: float32 [2, n_in]}: the weight w_k its rule gave
+        each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in
+        the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net."""
+        out = {}
+        for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights)):
+            if not agents:
+                continue
+            w = weights.cpu().numpy()
+            self.d2h_bytes += w.nbytes
+            out.update({i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(agents)})
+        return out
 
     def attack_gammas(self):
         """{(attacker b, cooperative receiver j) of a min-max / min-sum or a tailored attack: float32 [2]}: the gamma of
@@ -418,8 +436,8 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            if i in self.vec_row:                  # the aggregate as the single in-node: clip returns it exactly
-                nodes, H, rule = [self.vec_row[i]], 0, L.AGG_CLIP
+            if i in self.vec_row or i in self.dnc_row:   # the aggregate as the single in-node: clip returns it exactly
+                nodes, H, rule = [self.vec_row.get(i, self.dnc_row.get(i))], 0, L.AGG_CLIP
             else:
                 nodes, H, rule = self._receiver_nodes(i), self.H[i], self.aggregation[i]
             cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
@@ -468,6 +486,14 @@ class Trainer:
                 vec_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], self.vector_rule[i],
                                                weights_out=self.vec_weights[2 * q + t]))
         vec_jobs = ops.job_array(L.VectorJob, vec_jobs) if vec_jobs else None
+        # the dnc aggregates likewise, in one launch of their own
+        dnc_jobs = []
+        for q, i in enumerate(self.dnc_agents):
+            nodes, row = self._receiver_nodes(i), self.dnc_row[i]
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                dnc_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], L.SPECTRAL_DNC,
+                                               weights_out=self.dnc_weights[2 * q + t]))
+        dnc_jobs = ops.job_array(L.VectorJob, dnc_jobs) if dnc_jobs else None
 
         for epoch in range(self.n_epochs):                                 # :100
             # ---------------- I) local updates (:105-121)
@@ -499,6 +525,9 @@ class Trainer:
                 self.launches += 1
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)
+                self.launches += 1
+            if dnc_jobs is not None:
+                ops.dnc_aggregate(dnc_jobs)
                 self.launches += 1
             # ---------------- II) resilient consensus (:125-145)
             if coop:

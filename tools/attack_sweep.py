@@ -1,21 +1,22 @@
 """Byzantine attacks against each resilient aggregation rule on the C2 team: 4 cooperative agents (H = 1) and agent 4
-Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (by default clip, trim, wmsr; any of the coordinate rules and
-the distance-based krum, mkrum, scclip, gmed) x attack (alie, ipm, gauss) over the learning harness's seeds
+Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (by default clip, trim, wmsr; any of the coordinate rules,
+the distance-based krum, mkrum, scclip, gmed and the divide-and-conquer dnc) x attack (alie, ipm, gauss) over the learning harness's seeds
 (tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed; agent 4 keeps its weights
 and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the cooperative critics' estimate
-of it, means of the last 500 episodes, over the seeds; for a distance-based rule also the mean weight the receivers of
+of it, means of the last 500 episodes, over the seeds; for a distance-based rule or dnc also the mean weight the receivers of
 agent 4 gave its crafted message in the last epoch of the last round (Trainer.neighbour_weights, both nets), over the
 seeds.  The attack list (by default alie 1.0, ipm 0.5, gauss 0.3) may also name the min-max / min-sum attacks
 (rcmarl_adaptive_attack: minmax_uv, minmax_std, minmax_sgn, minsum_uv, minsum_std, minsum_sgn, scale 1 = the paper's
 attack) and the rule-aware attacks tuned against each receiver's own rule and H (rcmarl_tailored_attack: tailored_uv,
 tailored_std, tailored_sgn, range multiplier 2 by default); an entry is a name or name:param.  For those the table also
 reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in the last epoch of the last round
-(Trainer.attack_gammas, both nets and every receiver), over the seeds.
+(Trainer.attack_gammas, both nets and every receiver), over the seeds.  The tailored attacks do not model dnc: those
+cells are marked refused.
 
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
-alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
+and when it names dnc, on clip and dnc (all of them when it names both), alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
 tailored_std (every cooperative agent on clip) against gauss.
 
@@ -35,6 +36,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "resilient-consensus-based-marl_b200"))
 import bench                                   # noqa: E402
 import torch                                   # noqa: E402
+from rcmarl._lib import RcmarlError            # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
 PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0}
@@ -44,6 +46,7 @@ timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
 out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_out")
 RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
 VECTOR = ("krum", "mkrum", "scclip", "gmed")
+WHOLE = VECTOR + ("dnc",)                       # the rules that report neighbour weights
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
 TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
 ATTACKS = tuple((a.split(":")[0], float(a.split(":")[1]) if ":" in a else PARAMS.get(a, 1.0))
@@ -86,11 +89,17 @@ def timing():
     return out
 
 
+def timed_rules():
+    """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc if listed."""
+    return (("clip",) + (("gmed", "mkrum") if any(r in VECTOR for r in RULES) else ())
+            + (("dnc",) if "dnc" in RULES else ()))
+
+
 def rule_timing():
-    """ms per update round (median over rounds) with agent 4 Byzantine (gauss) and every cooperative agent on clip, gmed
-    and mkrum, at the benchmark's C2 shape, the three trainers alternated round by round."""
+    """ms per update round (median over rounds) with agent 4 Byzantine (gauss) and every cooperative agent on each of
+    timed_rules(), at the benchmark's C2 shape, the trainers alternated round by round."""
     cfg = dict(bench.workload("C2", 0), labels=["Cooperative"] * 4 + ["Byzantine"], attack=("gauss", 0.3))
-    trs = {r: Trainer(**dict(cfg, aggregation=[r] * 4 + ["clip"])) for r in ("clip", "gmed", "mkrum")}
+    trs = {r: Trainer(**dict(cfg, aggregation=[r] * 4 + ["clip"])) for r in timed_rules()}
     ms = {k: [] for k in trs}
     for r in range(timed_rounds + 1):
         for k, tr in trs.items():
@@ -104,10 +113,10 @@ def rule_timing():
             if r > 0:
                 ms[k].append(a.elapsed_time(b))
     out = {k: dict(median_ms=float(np.median(v)), rounds_ms=v) for k, v in ms.items()}
-    for k in ("gmed", "mkrum"):
+    for k in timed_rules()[1:]:
         out[f"{k}_added_ms"] = out[k]["median_ms"] - out["clip"]["median_ms"]
     out["n_envs"] = cfg["n_envs"]
-    out["aggregation_launches_per_round"] = trs["gmed"].n_epochs
+    out["aggregation_launches_per_round"] = trs["clip"].n_epochs
     return out
 
 
@@ -156,13 +165,19 @@ name, power = card()
 result = dict(card=name, power_limit_w=power, n_blocks=n_blocks, n_envs=n_envs, timing=timing(), cells=[])
 print(f"{name}, power limit {power} W: update round {result['timing']['Faulty']['median_ms']:.2f} ms (Faulty) vs "
       f"{result['timing']['Byzantine']['median_ms']:.2f} ms (Byzantine)", flush=True)
-vector = any(r in VECTOR for r in RULES)
+vector = any(r in WHOLE for r in RULES)
+
+
+def timing_line(rt):
+    return ", ".join([f"clip {rt['clip']['median_ms']:.2f} ms"] + [f"{k} {rt[k]['median_ms']:.2f} ms ({rt[k + '_added_ms']:+.3f} ms)"
+                                                               for k in timed_rules()[1:]])
+
+
 adaptive = any(a in ADAPTIVE + TAILORED for a, _ in ATTACKS)
 tailored = any(a in TAILORED for a, _ in ATTACKS)
 if vector:
     result["rule_timing"] = rt = rule_timing()
-    print(f"update round with agent 4 Byzantine: clip {rt['clip']['median_ms']:.2f} ms, gmed {rt['gmed']['median_ms']:.2f} ms "
-          f"({rt['gmed_added_ms']:+.3f}), mkrum {rt['mkrum']['median_ms']:.2f} ms ({rt['mkrum_added_ms']:+.3f})", flush=True)
+    print(f"update round with agent 4 Byzantine: {timing_line(rt)}", flush=True)
 if any(a in ADAPTIVE for a, _ in ATTACKS):
     result["adaptive_timing"] = at = adaptive_timing()
     print(f"update round with agent 4 Byzantine: gauss {at['gauss']['median_ms']:.2f} ms, minmax_std "
@@ -174,6 +189,7 @@ if tailored:
 for rule in RULES:
     for attack in ATTACKS:
         team, est, byz, gam = [], [], [], []
+        refused = None
         for tag in runs:
             _, _, ss = tag.split("/")
             labels = [str(x) for x in z[f"{tag}/labels"]]
@@ -185,9 +201,13 @@ for rule in RULES:
                     nets_i.append([z[f"{tag}/agent{i}/n{n}_k{k}"] for k in range(6)])
                     n += 1
                 w.append(nets_i[:3])
-            tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
-                         desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=rule, attack=attack,
-                         **bench.HYPER)
+            try:
+                tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
+                             desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=rule,
+                             attack=attack, **bench.HYPER)
+            except RcmarlError as ex:                   # e.g. a tailored attack against dnc
+                refused = str(ex)
+                break
             t, e = [], []
             for _ in range(n_blocks):
                 ee, rr = tr.rollout_block()
@@ -196,10 +216,15 @@ for rule in RULES:
             team.append(float(np.mean(t[-tail:]))); est.append(float(np.mean(e[-tail:])))
             byz.append(byzantine_weight(tr))
             gam.append(mean_gamma(tr))
+        if refused is not None:
+            cell = dict(rule=rule, attack=attack[0], param=attack[1], refused=refused)
+            result["cells"].append(cell)
+            print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: refused ({refused})", flush=True)
+            continue
         cell = dict(rule=rule, attack=attack[0], param=attack[1], seeds=len(runs), team=float(np.mean(team)),
                     est=float(np.mean(est)), team_per_seed=team, est_per_seed=est)
         if vector:
-            cell["byz_weight"] = float(np.mean(byz)) if rule in VECTOR else None
+            cell["byz_weight"] = float(np.mean(byz)) if rule in WHOLE else None
         if adaptive:
             cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED else None
         result["cells"].append(cell)
@@ -215,6 +240,10 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
             + (" weight of agent 4 |" if vector else "") + (" gamma |" if adaptive else "")
             + "\n|---|---|---|---|" + ("---|" if vector else "") + ("---|" if adaptive else "") + "\n")
     for c in result["cells"]:
+        if "refused" in c:
+            f.write(f"| {c['rule']} | {c['attack']} {c['param']} | refused | refused |" + (" - |" if vector else "")
+                    + (" - |" if adaptive else "") + "\n")
+            continue
         f.write(f"| {c['rule']} | {c['attack']} {c['param']} | {c['team']:.2f} | {c['est']:.2f} |"
                 + ((f" {c['byz_weight']:.3f} |" if c["byz_weight"] is not None else " - |") if vector else "")
                 + ((f" {c['gamma']:.3f} |" if c["gamma"] is not None else " - |") if adaptive else "") + "\n")
@@ -225,9 +254,7 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
     if vector:
         rt = result["rule_timing"]
         f.write(f"\nC2 update round at {rt['n_envs']} environments, agent 4 Byzantine (gauss), every cooperative agent on one "
-                f"rule (median of {timed_rounds}, alternated): clip {rt['clip']['median_ms']:.2f} ms, gmed "
-                f"{rt['gmed']['median_ms']:.2f} ms ({rt['gmed_added_ms']:+.3f} ms), mkrum {rt['mkrum']['median_ms']:.2f} ms "
-                f"({rt['mkrum_added_ms']:+.3f} ms)\n")
+                f"rule (median of {timed_rounds}, alternated): {timing_line(rt)}\n")
     if "adaptive_timing" in result:
         at = result["adaptive_timing"]
         f.write(f"\nC2 update round at {at['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
