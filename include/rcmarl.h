@@ -349,6 +349,33 @@ int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void
 typedef enum { RCMARL_SPECTRAL_DNC = 0 } rcmarl_spectral_rule;
 int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
+/* Nearest-neighbour mixing (rcmarl_nnm_mix): the pre-aggregation step of Allouah, Farhadkhani, Guerraoui, Gupta, Pinot
+ * & Stephan, "Fixing by Mixing: A Recipe for Optimal Byzantine ML under Heterogeneity" (AISTATS 2023).  It replaces each
+ * message a receiver hears by the mean of its n - H nearest received messages (itself among them); the receiver's own
+ * rule then runs on the mixed messages.  It takes rcmarl_vector_job with rule = RCMARL_MIX_NNM; its n = n_in messages
+ * x_0 .. x_{n-1} (x_0 the receiver's own; repeats in in_nodes count) each hold P = job.n packed parameters.  In fp32:
+ *   D_kl     for k != l exactly as rcmarl_vector_aggregate computes it (each pair k < l summed by one warp, lane-strided
+ *            partials, then the fixed xor butterfly); a distance that is not finite counts as +inf.  D_kk = 0, not
+ *            computed (a row holding +-inf gives no NaN).
+ *   N_k      order l by (D_kl, then l != k, then l) -- the own row first among equal distances, then the lower index --
+ *            and take the first n - H, less every l with D_kl = +inf.  N_k always holds k.
+ *   Output   mixed_k = (sum_{l in N_k, index order} x_l) / |N_k|: an fp32 sum from 0, then one division by
+ *            (float)|N_k| (multi-Krum's arithmetic), written to dst + k * msg_stride for k = 0 .. n-1.  weights_out,
+ *            when not NULL, receives M row-major [n_in][n_in]: M_kl = 1/|N_k| for l in N_k, 0 elsewhere.
+ * 0 <= H < n_in.  H = 0 with every distance finite gives every row multi-Krum's output at H = 0 (the plain mean); H =
+ * n - 1 passes every row through.  A row at non-finite distance from every other row (+-inf, 1e30) passes through and
+ * no finite row mixes it in, so at most H poisoned inputs give at most H poisoned mixed rows.  NaN inputs are not
+ * supported.  One CTA per job, fixed summation orders, no atomics: bitwise reproducible, independent of the job order
+ * and of how jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, every dst row and weights_out untouched): n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, a rule
+ * other than RCMARL_MIX_NNM, H outside [0, n_in), n_in * n > RCMARL_NNM_MAX_FLOATS (the messages are staged in shared
+ * memory), a written range (the n_in dst rows, the n_in^2 weights) that overlaps an in-node row of any job of the
+ * launch, and two written ranges of the launch that overlap. */
+#define RCMARL_NNM_MAX_FLOATS (48 * 1024)
+typedef enum { RCMARL_MIX_NNM = 0 } rcmarl_mixing_rule;
+int rcmarl_nnm_mix(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

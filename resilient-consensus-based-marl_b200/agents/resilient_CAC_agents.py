@@ -8,6 +8,8 @@ Same constructor and method names, argument meaning and mutation conventions as 
                                  of a distance-based ("krum", "mkrum", "scclip", "gmed") or divide-and-conquer
                                  ("dnc") aggregate of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
+                                 With mixing="nnm", every consensus step first replaces each received message by the
+                                 mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
 Tensors may be NumPy arrays, torch tensors or facade Tensors; they are moved to the GPU.  Calling these methods one
@@ -22,7 +24,7 @@ from rcmarl import nets, ops
 
 
 class RPBCAC_agent():
-    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip"):
+    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip", mixing=None):
         self.actor = actor
         self.critic = critic
         self.TR = team_reward
@@ -34,6 +36,10 @@ class RPBCAC_agent():
         if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation)):
             L.agg_rule(aggregation)
         self.aggregation = aggregation
+        # pre-aggregation mixing of the received messages: None or "nnm" (rcmarl_mixing_rule)
+        if mixing is not None:
+            L.check_mixing(mixing, 0, 1)
+        self.mixing = mixing
         self.n_actions = self.actor.output_shape[1]
         self.fast_lr = fast_lr
         self.slow_lr = slow_lr
@@ -46,7 +52,7 @@ class RPBCAC_agent():
     def _resilient_aggregation(self, values_innodes):
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
-        v = v.reshape(v.shape[0], -1)
+        v = self._mixed(v.reshape(v.shape[0], -1).contiguous())
         if self._whole_messages():                # the rows as whole vectors: out = sum_k w_k v_k
             out = self._with_aggregate(v)[-1]
         elif L.agg_rule(self.aggregation) == L.AGG_CLIP:
@@ -57,6 +63,16 @@ class RPBCAC_agent():
             ops.consensus_hidden([ops.consensus_job(out, v, v.shape[1], v.shape[1], list(range(v.shape[0])), self.H,
                                                     self.aggregation)])
         return Tensor(out.reshape(shape))
+
+    def _mixed(self, stack):
+        """[n, P] device stack (own = row 0) -> its n nearest-neighbour mixed rows if the agent mixes, else the stack."""
+        if self.mixing is None:
+            return stack
+        n, P = stack.shape
+        L.check_mixing(self.mixing, self.H, n)
+        out = torch.empty_like(stack)
+        ops.nnm_mix([ops.vector_job(out, stack, P, P, list(range(n)), self.H, L.MIX_NNM)])
+        return out
 
     def _whole_messages(self):
         """True if the rule aggregates whole messages (a distance-based rule or dnc)."""
@@ -78,7 +94,8 @@ class RPBCAC_agent():
     def _consensus_inputs(self, stack):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
         distance-based or dnc rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
-        Trainer."""
+        Trainer.  An agent that mixes does so first."""
+        stack = self._mixed(stack)
         if self._whole_messages():
             return self._with_aggregate(stack), [stack.shape[0]], 0, "clip"
         return stack, list(range(stack.shape[0])), self.H, self.aggregation

@@ -13,6 +13,7 @@
 //                   median; rcmarl_vector_aggregate)
 //   dnc_agg_kernel  divide-and-conquer: removes the messages furthest along the top principal direction
 //                   (rcmarl_dnc_aggregate)
+//   nnm_mix_kernel  nearest-neighbour mixing: each message becomes the mean of its n - H nearest (rcmarl_nnm_mix)
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
@@ -713,6 +714,68 @@ __global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_const
         job.dst[p] = s / cnt;
     }
     if (job.weights_out && tid < nin) job.weights_out[tid] = wt[tid];
+}
+
+// Nearest-neighbour mixing (rcmarl_nnm_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The n_in
+// messages are staged in shared memory and every distance of a pair k < l is summed by ONE warp with warp_sqdist, as in
+// vector_rule, so D_kl is bitwise Krum's.  The selections N_k run on warp 0, one lane per k, with rank counts over
+// registers, and are kept as bit masks; the output takes one thread per coordinate and adds each N_k in index order.
+__global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    static_assert(MAXN * MAXN <= VEC_THREADS, "one thread per entry of M");
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];
+    __shared__ unsigned sel[MAXN];                 // N_k: bit l set for l in N_k
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float* xs = smem;                              // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    for (int t = warp; t < nin * (nin - 1) / 2; t += NW) {           // unordered pairs k < l
+        int k = 0, r = t;
+        while (r >= nin - 1 - k) { r -= nin - 1 - k; ++k; }
+        const int l = k + 1 + r;
+        const float d = warp_sqdist(xs + k * n, xs + l * n, n, lane);
+        if (lane == 0) { dist[k * MAXN + l] = d; dist[l * MAXN + k] = d; }
+    }
+    __syncthreads();
+    if (warp == 0 && lane < nin) {
+        const int k = lane, m = nin - job.H;
+        float v[MAXN];
+#pragma unroll
+        for (int l = 0; l < MAXN; ++l) v[l] = (l < nin && l != k) ? dist[k * MAXN + l] : 0.f;
+        unsigned mask = 0u;
+#pragma unroll
+        for (int l = 0; l < MAXN; ++l) {              // rank of l in the order (D_kl, l != k, l)
+            int r = 0;
+#pragma unroll
+            for (int q = 0; q < MAXN; ++q)
+                if (q < nin && q != l) r += (v[q] < v[l] || (v[q] == v[l] && (q == k || (l != k && q < l)))) ? 1 : 0;
+            if (l < nin && r < m && v[l] < INFINITY) mask |= 1u << l;
+        }
+        sel[k] = mask;
+    }
+    __syncthreads();
+    for (int k = 0; k < nin; ++k) {
+        const unsigned mask = sel[k];
+        const float cnt = (float)__popc(mask);
+        float* dst = job.dst + (int64_t)k * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            float s = 0.f;
+            for (int l = 0; l < nin; ++l)
+                if ((mask >> l) & 1u) s += xs[l * n + p];
+            dst[p] = s / cnt;
+        }
+    }
+    if (job.weights_out && tid < nin * nin) {
+        const unsigned mask = sel[tid / nin];
+        job.weights_out[tid] = ((mask >> (tid % nin)) & 1u) ? 1.f / (float)__popc(mask) : 0.f;
+    }
 }
 
 // Min-max / min-sum Byzantine messages (rcmarl_adaptive_attack, include/rcmarl.h): one CTA of 256 threads per job.  The
@@ -1553,6 +1616,45 @@ int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream
     if (int e = opt_in_smem((const void*)dnc_agg_kernel, (int)(sizeof(float) * RCMARL_DNC_MAX_FLOATS), opted)) return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     dnc_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_nnm_mix(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.rule != RCMARL_MIX_NNM || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)q.n_in * q.n;
+        if (floats > RCMARL_NNM_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate, with n_in dst rows per job: no written range (a dst row, a weights_out) may overlap an
+    // in-node row of any job of the launch or another written range
+    constexpr int MAX_W = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1), MAX_R = RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS;
+    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
+        if (q.weights_out) {
+            float_range(q.weights_out, 0, 0, (int64_t)q.n_in * q.n_in, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < q.n_in; ++k, ++n_r)
+            float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)nnm_mix_kernel, (int)(sizeof(float) * RCMARL_NNM_MAX_FLOATS), opted)) return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    nnm_mix_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

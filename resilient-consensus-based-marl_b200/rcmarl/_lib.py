@@ -45,6 +45,9 @@ SPECTRAL_DNC = 0                                  # rcmarl_spectral_rule
 SPECTRAL_RULES = {"dnc": SPECTRAL_DNC}
 DNC_SWEEPS = 32
 DNC_MAX_FLOATS = 48 * 1024
+MIX_NNM = 0                                       # rcmarl_mixing_rule
+MIXING_RULES = {"nnm": MIX_NNM}
+NNM_MAX_FLOATS = 48 * 1024
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -137,6 +140,7 @@ SYMBOLS = [
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -243,6 +247,17 @@ def check_spectral_rule(H, n_in):
     if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
         raise RcmarlError(f"aggregation 'dnc' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
     return SPECTRAL_DNC
+
+
+def check_mixing(name, H, n_in):
+    """Raise RcmarlError unless `name` names a pre-aggregation mixing rule (rcmarl_mixing_rule: "nnm") that allows H
+    out of n_in messages (rcmarl_nnm_mix, include/rcmarl.h): 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  Returns
+    the rcmarl_mixing_rule id."""
+    if not isinstance(name, str) or name not in MIXING_RULES:
+        raise RcmarlError(f"unknown mixing rule {name!r}: expected None or one of {sorted(MIXING_RULES)}")
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
+        raise RcmarlError(f"mixing {name!r} with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
+    return MIXING_RULES[name]
 
 
 def is_adaptive_attack(name):

@@ -384,6 +384,13 @@ def dnc_aggregate(jobs):
     L.check(L.lib().rcmarl_dnc_aggregate(a, len(a), _stream()), "rcmarl_dnc_aggregate")
 
 
+def nnm_mix(jobs):
+    """rcmarl_nnm_mix over rcmarl_vector_job jobs (vector_job(dst, ..., rule=L.MIX_NNM, weights_out=[n_in * n_in])):
+    mixed row k goes to dst + k * msg_stride."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_nnm_mix(a, len(a), _stream()), "rcmarl_nnm_mix")
+
+
 def reward_mix(r, agents, out=None, scale=1.0):
     """r: [rows, n_agents]; out[row] = scale * sum_k r[row, agents[k]] / len(agents) in list order."""
     n_rows, n_agents = r.shape

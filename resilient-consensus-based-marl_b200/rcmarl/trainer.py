@@ -29,7 +29,7 @@ class Trainer:
                  common_reward=False, mu=0.1, seed=0, device=None, rank=0, world=1, group=None,
                  perm_source=None, local_steps=5, mb_epochs=10, mb_times=32, actor_mb_times=200,
                  capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip",
-                 attack=None):
+                 attack=None, mixing=None):
         L.lib()
         # Any team size up to 16 (main.py:26): the kernels are instantiated for 5 and 16 agents, a team of n_real agents
         # runs on the next instantiation with the extra agent slots zero (inputs and W1 rows, rcmarl/nets.py) -- exactly the
@@ -73,18 +73,41 @@ class Trainer:
                 L.check_spectral_rule(self.H[i], len(self.in_nodes[i]))
             else:
                 L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
+        # Nearest-neighbour mixing ("nnm") before a cooperative agent's rule: its n_in received messages become n_in
+        # mixed message rows (rcmarl_nnm_mix), which its rule then reads in their place with the same H
+        mix = [mixing] * n_real if mixing is None or isinstance(mixing, str) else list(mixing)
+        if len(mix) != n_real:
+            raise L.RcmarlError("mixing must be None, one mixing rule or one entry per agent")
+        self.mixing = [None] * NA
+        for i in range(n_real):
+            if mix[i] is None:
+                continue
+            if i in self.coop:
+                L.check_mixing(mix[i], self.H[i], len(self.in_nodes[i]))
+                self.mixing[i] = mix[i]
+            else:                                  # only cooperative agents aggregate: the name alone is checked
+                L.check_mixing(mix[i], 0, 1)
         self._init_attacks(attack)
-        for e in self.tailor_pairs:                # rcmarl_tailored_attack does not model the DnC rule
+        for e in self.tailor_pairs:                # rcmarl_tailored_attack models neither the DnC rule nor mixing
             b, j, _ = self.byz_pairs[e]
             if self.dnc[j]:
                 raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose rule 'dnc' "
                                     "the tailored attack does not model")
+            if self.mixing[j] is not None:
+                raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose mixing "
+                                    f"{self.mixing[j]!r} the tailored attack does not model")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
         # that of each cooperative agent on dnc
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
         self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
         self.dnc_agents = [i for i in self.coop if self.dnc[i]]
         self.dnc_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + q for q, i in enumerate(self.dnc_agents)}
+        # then the n_in mixed rows of each cooperative agent that mixes: mixed row k at mix_row[i] + k
+        self.mix_agents = [i for i in self.coop if self.mixing[i] is not None]
+        self.mix_row, row = {}, NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
+        for i in self.mix_agents:
+            self.mix_row[i] = row
+            row += len(self.in_nodes[i])
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -115,14 +138,18 @@ class Trainer:
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
-        # vec_row[i] / dnc_row[i] the aggregate of cooperative agent i's distance-based / dnc rule
-        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
+        # vec_row[i] / dnc_row[i] the aggregate of cooperative agent i's distance-based / dnc rule; mix_row[i] + k its
+        # mixed message k
+        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) \
+            + sum(len(self.in_nodes[i]) for i in self.mix_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
         self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
         # ... and of each dnc aggregate: row 2q critic, 2q + 1 TR of dnc_agents[q]
         self.dnc_weights = torch.zeros(2 * len(self.dnc_agents), L.MAX_NEIGHBOURS, **f32) if self.dnc_agents else None
+        # mixing matrix M (row-major [n_in][n_in]) of each agent that mixes: row 2q critic, 2q + 1 TR of mix_agents[q]
+        self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
         # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         self.adam_m = torch.zeros(NA, self.PA, **f32)
@@ -216,10 +243,17 @@ class Trainer:
         row = {b: self.NA + e for e, (b, r, _) in enumerate(self.byz_pairs) if r == j}
         return [row.get(k, k) for k in self.in_nodes[j]]
 
+    def _rule_nodes(self, j):
+        """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, else _receiver_nodes(j)."""
+        if self.mixing[j] is None:
+            return self._receiver_nodes(j)
+        return list(range(self.mix_row[j], self.mix_row[j] + len(self.in_nodes[j])))
+
     def neighbour_weights(self):
         """{cooperative agent i with a distance-based or the dnc rule: float32 [2, n_in]}: the weight w_k its rule gave
         each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in
-        the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net."""
+        the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.  For an agent that
+        mixes, the rule weighs the mixed messages, and the entry is the effective weight w M of each in-neighbour."""
         out = {}
         for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights)):
             if not agents:
@@ -227,6 +261,25 @@ class Trainer:
             w = weights.cpu().numpy()
             self.d2h_bytes += w.nbytes
             out.update({i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(agents)})
+        if any(self.mixing[i] is not None for i in out):
+            mix = self.mixing_matrices()
+            for i in out:
+                if i in mix:
+                    out[i] = np.einsum("tk,tkl->tl", out[i].astype(np.float64), mix[i]).astype(np.float32)
+        return out
+
+    def mixing_matrices(self):
+        """{cooperative agent i that mixes: float32 [2, n_in, n_in]}: the mixing matrix M of the last epoch of the last
+        update round, M[k, l] = 1/|N_k| if in-neighbour l (in_nodes[i] order) is among the nearest of k and 0 otherwise
+        (rcmarl_nnm_mix); [0] for the critic, [1] for the team-reward net."""
+        if not self.mix_agents:
+            return {}
+        m = self.mix_weights.cpu().numpy()
+        self.d2h_bytes += m.nbytes
+        out = {}
+        for q, i in enumerate(self.mix_agents):
+            n = len(self.in_nodes[i])
+            out[i] = m[2 * q:2 * q + 2, :n * n].reshape(2, n, n).copy()
         return out
 
     def attack_gammas(self):
@@ -439,7 +492,7 @@ class Trainer:
             if i in self.vec_row or i in self.dnc_row:   # the aggregate as the single in-node: clip returns it exactly
                 nodes, H, rule = [self.vec_row.get(i, self.dnc_row.get(i))], 0, L.AGG_CLIP
             else:
-                nodes, H, rule = self._receiver_nodes(i), self.H[i], self.aggregation[i]
+                nodes, H, rule = self._rule_nodes(i), self.H[i], self.aggregation[i]
             cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
             cons_jobs.append(ops.consensus_job(self.tr[i], self.msg_t, self.PT, nets.n_hidden_params(3 * NA), nodes, H, rule))
             team_jobs.append(ops.team_job(self.critic[i], L.IN_S, self.msg_c, self.PC, nodes, H, sums=self.sums_team[2 * n], rule=rule))
@@ -477,11 +530,19 @@ class Trainer:
         tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
                        for g in range(0, len(tail_jobs), L.MAX_JOBS)]
 
-        # distance-based aggregates over the messages each receiver hears (crafted Byzantine ones included): at most 16
+        # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
+        # 16 cooperative agents x 2 nets, so one launch per epoch
+        mix_jobs = []
+        for q, i in enumerate(self.mix_agents):
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i), self.H[i],
+                                               L.MIX_NNM, weights_out=self.mix_weights[2 * q + t]))
+        mix_jobs = ops.job_array(L.VectorJob, mix_jobs) if mix_jobs else None
+        # distance-based aggregates over the messages each receiver hears (or their mixed rows): at most 16
         # cooperative agents x 2 nets, so one launch per epoch
         vec_jobs = []
         for q, i in enumerate(self.vec_agents):
-            nodes, row = self._receiver_nodes(i), self.vec_row[i]
+            nodes, row = self._rule_nodes(i), self.vec_row[i]
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
                 vec_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], self.vector_rule[i],
                                                weights_out=self.vec_weights[2 * q + t]))
@@ -489,7 +550,7 @@ class Trainer:
         # the dnc aggregates likewise, in one launch of their own
         dnc_jobs = []
         for q, i in enumerate(self.dnc_agents):
-            nodes, row = self._receiver_nodes(i), self.dnc_row[i]
+            nodes, row = self._rule_nodes(i), self.dnc_row[i]
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
                 dnc_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], L.SPECTRAL_DNC,
                                                weights_out=self.dnc_weights[2 * q + t]))
@@ -522,6 +583,9 @@ class Trainer:
                 self.launches += 1
             for g in tail_groups:                                          # no epoch dependence either
                 ops.tailored_attack(g)
+                self.launches += 1
+            if mix_jobs is not None:
+                ops.nnm_mix(mix_jobs)
                 self.launches += 1
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)

@@ -11,7 +11,9 @@ attack) and the rule-aware attacks tuned against each receiver's own rule and H 
 tailored_std, tailored_sgn, range multiplier 2 by default); an entry is a name or name:param.  For those the table also
 reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in the last epoch of the last round
 (Trainer.attack_gammas, both nets and every receiver), over the seeds.  The tailored attacks do not model dnc: those
-cells are marked refused.
+cells are marked refused.  A rule may be written nnm+<rule> (e.g. nnm+mkrum): every cooperative agent then mixes the
+messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, and the weight reported for a
+whole-message rule is the effective weight w M of agent 4's message.  The tailored attacks do not model mixing either.
 
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
@@ -45,6 +47,14 @@ n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
 out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_out")
 RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
+
+
+def split_rule(rule):
+    """(mixing, aggregation rule) of a rule name: "nnm+mkrum" -> ("nnm", "mkrum"), "mkrum" -> (None, "mkrum")."""
+    return ("nnm", rule[4:]) if rule.startswith("nnm+") else (None, rule)
+
+
+BASES = tuple(split_rule(r)[1] for r in RULES)
 VECTOR = ("krum", "mkrum", "scclip", "gmed")
 WHOLE = VECTOR + ("dnc",)                       # the rules that report neighbour weights
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
@@ -91,8 +101,8 @@ def timing():
 
 def timed_rules():
     """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc if listed."""
-    return (("clip",) + (("gmed", "mkrum") if any(r in VECTOR for r in RULES) else ())
-            + (("dnc",) if "dnc" in RULES else ()))
+    return (("clip",) + (("gmed", "mkrum") if any(r in VECTOR for r in BASES) else ())
+            + (("dnc",) if "dnc" in BASES else ()))
 
 
 def rule_timing():
@@ -165,7 +175,7 @@ name, power = card()
 result = dict(card=name, power_limit_w=power, n_blocks=n_blocks, n_envs=n_envs, timing=timing(), cells=[])
 print(f"{name}, power limit {power} W: update round {result['timing']['Faulty']['median_ms']:.2f} ms (Faulty) vs "
       f"{result['timing']['Byzantine']['median_ms']:.2f} ms (Byzantine)", flush=True)
-vector = any(r in WHOLE for r in RULES)
+vector = any(r in WHOLE for r in BASES)
 
 
 def timing_line(rt):
@@ -201,11 +211,12 @@ for rule in RULES:
                     nets_i.append([z[f"{tag}/agent{i}/n{n}_k{k}"] for k in range(6)])
                     n += 1
                 w.append(nets_i[:3])
+            mixing, base = split_rule(rule)
             try:
                 tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
-                             desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=rule,
-                             attack=attack, **bench.HYPER)
-            except RcmarlError as ex:                   # e.g. a tailored attack against dnc
+                             desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=base,
+                             attack=attack, mixing=mixing, **bench.HYPER)
+            except RcmarlError as ex:                   # e.g. a tailored attack against dnc or mixing
                 refused = str(ex)
                 break
             t, e = [], []
@@ -219,16 +230,16 @@ for rule in RULES:
         if refused is not None:
             cell = dict(rule=rule, attack=attack[0], param=attack[1], refused=refused)
             result["cells"].append(cell)
-            print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: refused ({refused})", flush=True)
+            print(f"{rule:9s} {attack[0]:5s} {attack[1]:4.1f}: refused ({refused})", flush=True)
             continue
         cell = dict(rule=rule, attack=attack[0], param=attack[1], seeds=len(runs), team=float(np.mean(team)),
                     est=float(np.mean(est)), team_per_seed=team, est_per_seed=est)
         if vector:
-            cell["byz_weight"] = float(np.mean(byz)) if rule in WHOLE else None
+            cell["byz_weight"] = float(np.mean(byz)) if split_rule(rule)[1] in WHOLE else None
         if adaptive:
             cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED else None
         result["cells"].append(cell)
-        print(f"{rule:5s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}"
+        print(f"{rule:9s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}"
               + (f"  weight of agent 4 {cell['byz_weight']:.3f}" if cell.get("byz_weight") is not None else "")
               + (f"  gamma {cell['gamma']:.3f}" if cell.get("gamma") is not None else ""), flush=True)
 
