@@ -269,6 +269,78 @@ typedef struct {
 } rcmarl_tailored_attack_job;
 int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* The dissensus attack (rcmarl_dissensus_attack) of He, Karimireddy & Jaggi, "Byzantine-robust decentralized learning
+ * via ClippedGossip" (2022), under the threat model of rcmarl_attack: each Byzantine neighbour sends receiver j the
+ * message that cancels (eps = 1) or reverses (eps > 1) the pull of j's honest neighbours.  One job is one (attacker,
+ * receiver j, net).  All arithmetic is fp32.  With x = msgs + own * msg_stride (the receiver's own message) and the
+ * honest rows v_k = msgs + honest[k] * msg_stride (S_j in list order, repeats included, S_j holding j itself), per
+ * packed parameter p < n:
+ *   delta_p = sum_k (v_k,p - x_p)   (summed in list order from 0),   c = eps / (float)n_byz,
+ *   dst[p] = c == 0 ? x_p : fmaf(-c, delta_p, x_p),
+ * so eps = 0 sends x bitwise.  n_byz is the number of entries of in_nodes[j] held by dissensus attackers (repeats
+ * included): colluders split the cancellation, and under a plain mean eps = 1 leaves the receiver where it was.  This is
+ * the paper's x_i - eps sum_good W_ik (x_k - x_i) / sum_byz W_ij under uniform weights.
+ * One thread per coordinate, fixed summation order, no atomics: bitwise reproducible, independent of the job order and
+ * of how jobs are split over launches.  Refused (RCMARL_ERR_ARG, nothing launched, dst untouched): n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_honest outside 1..RCMARL_MAX_NEIGHBOURS, a negative honest or own
+ * row, n_byz outside 1..RCMARL_MAX_NEIGHBOURS, an eps that is not finite or is < 0, a dst that overlaps an honest or own
+ * row of any job of the launch, and two dsts of the launch that overlap.  NaN inputs are not supported. */
+typedef struct {
+    float* dst;                 /* the crafted message (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    int32_t n;                  /* parameters crafted: dst[0:n] */
+    int32_t own;                /* the receiver's message row x */
+    int32_t n_honest;
+    int32_t honest[RCMARL_MAX_NEIGHBOURS];
+    int32_t n_byz;              /* dissensus entries of the receiver's in_nodes, repeats included */
+    float eps;                  /* eps >= 0; 1 cancels the honest pull under a plain mean */
+    int32_t reserved;
+} rcmarl_dissensus_job;
+int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs_host, int n_jobs, void* stream);
+
+/* The mimic attack (rcmarl_mimic_attack) of Karimireddy, He & Jaggi, "Byzantine-robust learning on heterogeneous
+ * datasets via bucketing" (ICLR 2022): the attacker sends an exact copy of one honest neighbour's message, the one that
+ * lies furthest along the honest messages' principal direction z, which it tracks by power iteration.  The copy is an
+ * honest message, so no rule can flag it as an outlier; it over-weights one agent's view in the receiver's consensus.
+ * One job is one (attacker, receiver j, net); z [n] is the job's direction state, read and written.  All arithmetic is
+ * fp32; every sum over p is taken by one warp (lane-strided fmaf partials, then the fixed xor butterfly), and a sum
+ * that is not finite counts as +inf.  Over the honest rows v_k = msgs + honest[k] * msg_stride (k < n_honest, in list
+ * order, repeats included):
+ *   Centre  mu exactly as rcmarl_attack computes it (same summation order); c_k,p = v_k,p - mu_p.
+ *   Init    only when every z_p == 0: e_k = sum_p c_k,p^2, k0 = argmax_k e_k over all k (ties to the smaller k); if
+ *           e_k0 is positive and finite, z_p = c_k0,p / sqrtf(e_k0), otherwise z stays 0.
+ *   Step    only when update == 1 and z != 0 (after Init): one power-iteration step on the honest covariance,
+ *           s_k = sum_p c_k,p z_p,  u_p = sum_k s_k c_k,p (k order, fmaf from 0),  q = sum_p u_p^2;
+ *           if q is positive and finite, z_p = u_p / sqrtf(q), otherwise z is unchanged.
+ *   Choose  over the candidates (bit k of candidate_mask), with the final z: t_k = sum_p c_k,p z_p, a t_k that is not
+ *           finite counting as -inf; k* = argmax t_k, ties to the smaller k; k* = the lowest candidate if z = 0 or every
+ *           t_k is -inf.
+ *   Output  dst[0:n] = v_k* copied bitwise, z written back, target_out (optional, one int32) = k*.
+ * One CTA per job: the centred honest rows, mu, z and u staged in shared memory, fixed summation orders, no atomics:
+ * bitwise reproducible, independent of the job order and of how jobs are split over launches.  Jobs with equal inputs
+ * (colluding attackers of one receiver) keep bitwise equal states and copy the same row.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, z and target_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a
+ * null dst, msgs or z, n < 1, n_honest outside 1..RCMARL_MAX_NEIGHBOURS, a negative honest row, an empty candidate_mask
+ * or one with a bit at or past n_honest, update other than 0 or 1, (n_honest + 3) * n > RCMARL_MIMIC_MAX_FLOATS (the
+ * staging bound: 16 honest rows, mu, z and u of up to 1536 parameters), a dst, z or target_out that overlaps an honest
+ * row of any job of the launch, and two written ranges (dsts, zs, target_outs) of the launch that overlap.  NaN inputs
+ * are not supported. */
+#define RCMARL_MIMIC_MAX_FLOATS (19 * 1536)
+typedef struct {
+    float* dst;                 /* the copied message (packed network) */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    float* z;                   /* [n] direction state, read and written; all zero: not yet initialised */
+    int32_t* target_out;        /* optional [1]: k* */
+    int32_t n;                  /* parameters per message */
+    int32_t n_honest;
+    int32_t honest[RCMARL_MAX_NEIGHBOURS];
+    uint32_t candidate_mask;    /* bit k: honest entry k may be copied */
+    int32_t update;             /* 1: take one power step; 0: keep z (after Init) */
+} rcmarl_mimic_job;
+int rcmarl_mimic_attack(const rcmarl_mimic_job* jobs_host, int n_jobs, void* stream);
+
 /* Distance-based resilient aggregation of whole messages (rcmarl_vector_aggregate).  The rules above are coordinate-wise;
  * these compare the in-neighbours' messages as vectors.  One job: its n = n_in messages x_k = msgs + in_nodes[k] *
  * msg_stride, k = 0 .. n-1 (k = 0 is the receiver's own; repeats in in_nodes count), each of P = job.n packed

@@ -17,6 +17,9 @@
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
+//   dissensus_attack_kernel  Byzantine messages that cancel the receiver's honest pull (rcmarl_dissensus_attack)
+//   mimic_attack_kernel  copies of the honest message furthest along the tracked principal direction
+//                   (rcmarl_mimic_attack)
 //   consensus, sgd/adam apply, reward mix: the small glue kernels.
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
@@ -1008,6 +1011,144 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) tailored_attack_kernel(const _
     for (int p = tid; p < n; p += ADA_THREADS) job.dst[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
 }
 
+// Dissensus messages (rcmarl_dissensus_attack, include/rcmarl.h): one thread per coordinate, as attack_kernel; the
+// honest pull delta is summed in list order from 0.
+struct DissensusParams { rcmarl_dissensus_job jobs[RCMARL_MAX_JOBS]; };
+__global__ void __launch_bounds__(256) dissensus_attack_kernel(const __grid_constant__ DissensusParams P) {
+    const rcmarl_dissensus_job& job = P.jobs[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= job.n) return;
+    const float x = __ldg(job.msgs + (int64_t)job.own * job.msg_stride + i);
+    float delta = 0.f;
+    for (int k = 0; k < job.n_honest; ++k) delta += __ldg(job.msgs + (int64_t)job.honest[k] * job.msg_stride + i) - x;
+    const float c = job.eps / (float)job.n_byz;
+    job.dst[i] = c == 0.f ? x : fmaf(-c, delta, x);
+}
+
+// Mimic messages (rcmarl_mimic_attack, include/rcmarl.h): one CTA of 256 threads per job.  The honest rows are staged
+// in shared memory and centred in place (mu as attack_kernel), next to mu, z and u.  Every sum over p is taken by ONE
+// warp (warp_dot), so its value does not depend on which warp takes it; the per-row sums are spread over the warps, the
+// choices run on thread 0 and the elementwise steps take one thread per coordinate.
+struct MimicParams { rcmarl_mimic_job jobs[RCMARL_MAX_JOBS]; };
+
+__global__ void __launch_bounds__(ADA_THREADS) mimic_attack_kernel(const __grid_constant__ MimicParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = ADA_THREADS / 32;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float sk[MAXN];                     // e_k (Init), s_k (Step), t_k (Choose)
+    __shared__ float scal;                         // the divisor sqrtf(e_k0) or sqrtf(q)
+    __shared__ int pick, live;                     // k0 / k*; whether z is to be rescaled
+    const rcmarl_mimic_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nh = job.n_honest;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float* cs = smem;                              // [n_honest][n]: c_k = v_k - mu
+    float* mu = smem + (int64_t)nh * n;            // [n]
+    float* z = mu + n;                             // [n]
+    float* u = z + n;                              // [n]
+    for (int k = 0; k < nh; ++k) {
+        const float* src = job.msgs + (int64_t)job.honest[k] * job.msg_stride;
+        for (int p = tid; p < n; p += ADA_THREADS) cs[k * n + p] = __ldg(src + p);
+    }
+    int nonzero = 0;
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        const float v = job.z[p];
+        z[p] = v;
+        nonzero |= v != 0.f;
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        float s = 0.f;
+        for (int k = 0; k < nh; ++k) s += cs[k * n + p];
+        const float m = s / (float)nh;
+        mu[p] = m;
+        for (int k = 0; k < nh; ++k) cs[k * n + p] = cs[k * n + p] - m;
+    }
+    bool zero = !__syncthreads_or(nonzero);
+    if (zero) {                                                       // Init: the largest centred row, normalised
+        for (int k = warp; k < nh; k += NW) {
+            const float e = warp_dot(cs + k * n, cs + k * n, n, lane);
+            if (lane == 0) sk[k] = isfinite(e) ? e : INFINITY;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int k0 = 0;
+            for (int k = 1; k < nh; ++k)
+                if (sk[k] > sk[k0]) k0 = k;
+            const float e = sk[k0];
+            live = e > 0.f && isfinite(e);
+            pick = k0;
+            scal = sqrtf(e);
+        }
+        __syncthreads();
+        int set = 0;
+        if (live) {
+            const float* c = cs + pick * n;
+            const float r = scal;
+            for (int p = tid; p < n; p += ADA_THREADS) {
+                const float v = c[p] / r;
+                z[p] = v;
+                set |= v != 0.f;
+            }
+        }
+        zero = !__syncthreads_or(set);
+    }
+    if (job.update == 1 && !zero) {                                  // Step: z <- C^T C z / ||C^T C z||
+        for (int k = warp; k < nh; k += NW) {
+            const float s = warp_dot(cs + k * n, z, n, lane);
+            if (lane == 0) sk[k] = isfinite(s) ? s : INFINITY;
+        }
+        __syncthreads();
+        for (int p = tid; p < n; p += ADA_THREADS) {
+            float a = 0.f;
+            for (int k = 0; k < nh; ++k) a = fmaf(sk[k], cs[k * n + p], a);
+            u[p] = a;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const float q = warp_dot(u, u, n, lane);
+            if (lane == 0) {
+                const float qq = isfinite(q) ? q : INFINITY;
+                live = qq > 0.f && isfinite(qq);
+                scal = sqrtf(qq);
+            }
+        }
+        __syncthreads();
+        if (live) {
+            const float r = scal;
+            for (int p = tid; p < n; p += ADA_THREADS) z[p] = u[p] / r;
+        }
+        __syncthreads();
+    }
+    // Choose: the candidate furthest along z (ties to the smaller k; not finite: -inf)
+    if (!zero) {
+        for (int k = warp; k < nh; k += NW) {
+            if (!((job.candidate_mask >> k) & 1u)) continue;
+            const float t = warp_dot(cs + k * n, z, n, lane);
+            if (lane == 0) sk[k] = isfinite(t) ? t : -INFINITY;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int best = __ffs((int)job.candidate_mask) - 1;                // the lowest candidate
+        if (!zero) {
+            float bt = -INFINITY;
+            for (int k = 0; k < nh; ++k)
+                if (((job.candidate_mask >> k) & 1u) && sk[k] > bt) {
+                    bt = sk[k];
+                    best = k;
+                }
+        }
+        pick = best;
+        if (job.target_out) *job.target_out = best;
+    }
+    __syncthreads();
+    const float* src = job.msgs + (int64_t)job.honest[pick] * job.msg_stride;
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        job.dst[p] = __ldg(src + p);
+        job.z[p] = z[p];
+    }
+}
+
 struct SgdParams { rcmarl_sgd_job jobs[RCMARL_MAX_JOBS]; };
 __global__ void __launch_bounds__(256) sgd_kernel(const __grid_constant__ SgdParams P) {
     const rcmarl_sgd_job& job = P.jobs[blockIdx.y];
@@ -1760,6 +1901,84 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
         return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     tailored_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    DissensusParams P;
+    int maxn = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_dissensus_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS || q.own < 0)
+            return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_honest; ++k)
+            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (q.n_byz < 1 || q.n_byz > RCMARL_MAX_NEIGHBOURS || !std::isfinite(q.eps) || q.eps < 0.f) return RCMARL_ERR_ARG;
+        P.jobs[j] = q;
+        if (q.n > maxn) maxn = q.n;
+    }
+    // one thread per coordinate reads every row it needs before it writes, but other CTAs run concurrently: no dst may
+    // overlap an honest or own row of any job of the launch or another dst
+    constexpr int MAX_R = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1);
+    uintptr_t w0[RCMARL_MAX_JOBS], w1[RCMARL_MAX_JOBS], r0[MAX_R], r1[MAX_R];
+    int n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_dissensus_job& q = jobs[j];
+        float_range(q.dst, 0, 0, q.n, w0[j], w1[j]);
+        float_range(q.msgs, q.own, q.msg_stride, q.n, r0[n_r], r1[n_r]);
+        ++n_r;
+        for (int k = 0; k < q.n_honest; ++k, ++n_r) float_range(q.msgs, q.honest[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_jobs, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    dissensus_attack_kernel<<<dim3((maxn + 255) / 256, n_jobs), 256, 0, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_mimic_attack(const rcmarl_mimic_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    MimicParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_mimic_job& q = jobs[j];
+        if (!q.dst || !q.msgs || !q.z || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS)
+            return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_honest; ++k)
+            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (q.candidate_mask == 0u || (q.candidate_mask >> q.n_honest) != 0u) return RCMARL_ERR_ARG;
+        if (q.update != 0 && q.update != 1) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_honest + 3) * q.n;
+        if (floats > RCMARL_MIMIC_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate: no written range (a dst, a z, a target_out) may overlap an honest row of any job of the
+    // launch or another written range
+    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_mimic_job& q = jobs[j];
+        float_range(q.dst, 0, 0, q.n, w0[n_w], w1[n_w]);
+        ++n_w;
+        float_range(q.z, 0, 0, q.n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (q.target_out) {
+            w0[n_w] = (uintptr_t)q.target_out;
+            w1[n_w] = w0[n_w] + sizeof(int32_t);
+            ++n_w;
+        }
+        for (int k = 0; k < q.n_honest; ++k, ++n_r) float_range(q.msgs, q.honest[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    // the staging bound is above the default 48 KB of dynamic shared memory
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)mimic_attack_kernel, (int)(sizeof(float) * RCMARL_MIMIC_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    mimic_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

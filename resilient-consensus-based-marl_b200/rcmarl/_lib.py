@@ -48,6 +48,8 @@ DNC_MAX_FLOATS = 48 * 1024
 MIX_NNM = 0                                       # rcmarl_mixing_rule
 MIXING_RULES = {"nnm": MIX_NNM}
 NNM_MAX_FLOATS = 48 * 1024
+MIMIC_MAX_FLOATS = 19 * 1536                      # rcmarl_mimic_attack's staging bound
+MIMIC_MAX_T0 = 2 ** 31 - 1                        # the mimic attack's power steps T0: an integer in 0 .. 2^31 - 1
 
 c_fp = C.c_void_p  # device pointers travel as integers
 
@@ -83,6 +85,18 @@ class TailoredAttackJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("gamma_out", c_fp), ("n", C.c_int32),
                 ("n_in", C.c_int32), ("slots", C.c_int32 * MAX_NEIGHBOURS), ("honest_mask", C.c_uint32),
                 ("family", C.c_int32), ("rule", C.c_int32), ("H", C.c_int32), ("dev", C.c_int32), ("scale", C.c_float)]
+
+
+class DissensusJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("n", C.c_int32), ("own", C.c_int32),
+                ("n_honest", C.c_int32), ("honest", C.c_int32 * MAX_NEIGHBOURS), ("n_byz", C.c_int32),
+                ("eps", C.c_float), ("reserved", C.c_int32)]
+
+
+class MimicJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("z", c_fp), ("target_out", c_fp),
+                ("n", C.c_int32), ("n_honest", C.c_int32), ("honest", C.c_int32 * MAX_NEIGHBOURS),
+                ("candidate_mask", C.c_uint32), ("update", C.c_int32)]
 
 
 class ValueJob(C.Structure):
@@ -143,6 +157,8 @@ SYMBOLS = [
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
+    ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
+    ("rcmarl_mimic_attack", C.c_int, [C.POINTER(MimicJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
     ("rcmarl_grad", C.c_int, [C.POINTER(Rows), C.POINTER(GradJob), C.c_int, C.c_int, c_fp, C.c_int64, c_fp]),
     ("rcmarl_sgd_apply", C.c_int, [C.POINTER(SgdJob), C.c_int, c_fp]),
@@ -281,23 +297,48 @@ def is_tailored_attack(name):
     return isinstance(name, str) and name in TAILORED_ATTACKS
 
 
+class DissensusKind(int):
+    """The kind check_attack gives the dissensus attack (rcmarl_dissensus_attack), a type of its own so that it is told
+    apart from the other attacks' kinds; its parameter is eps >= 0."""
+
+    def __repr__(self):
+        return "DissensusKind()"
+
+
+class MimicKind(int):
+    """The kind check_attack gives the mimic attack (rcmarl_mimic_attack), a type of its own so that it is told apart
+    from the other attacks' kinds; its parameter is T0, the number of power steps each (attacker, receiver) pair takes."""
+
+    def __repr__(self):
+        return "MimicKind()"
+
+
+STATE_ATTACKS = {"dissensus": DissensusKind(0), "mimic": MimicKind(0)}
+
+
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss", the adaptive and the tailored attacks also >= 0), as rcmarl_attack / rcmarl_adaptive_attack /
-    rcmarl_tailored_attack require (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and
-    "gauss", the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s
-    (1 is the paper's attack), and the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, whose parameter is
-    the range multiplier s."""
+    "gauss", the adaptive and the tailored attacks and "dissensus" also >= 0; for "mimic" an integer in
+    0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack / rcmarl_dissensus_attack /
+    rcmarl_mimic_attack require (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
+    the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the
+    paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, whose parameter is the range
+    multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
+    and MimicKind for "mimic", whose parameter is T0 (the power steps each pair takes before its direction freezes)."""
     try:
         name, param = attack
         param = float(param)
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
-    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS}
+    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **STATE_ATTACKS}
     if not isinstance(name, str) or name not in known:
         raise RcmarlError(f"unknown attack {name!r}: expected one of "
-                          f"{sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS)}")
-    nonneg = name == "gauss" or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS
+                          f"{sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(STATE_ATTACKS)}")
+    if name == "mimic":
+        if not (math.isfinite(param) and param == int(param) and 0 <= param <= MIMIC_MAX_T0):
+            raise RcmarlError(f"attack 'mimic' needs an integer T0 in 0 .. {MIMIC_MAX_T0}, got {param}")
+        return known[name], param
+    nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
     return known[name], param

@@ -355,6 +355,48 @@ def tailored_attack(jobs):
     L.check(L.lib().rcmarl_tailored_attack(a, len(a), _stream()), "rcmarl_tailored_attack")
 
 
+def dissensus_attack_job(dst, msgs, msg_stride, n, own, honest, n_byz, eps):
+    """own: the receiver's message row; honest: the message rows of its honest set in list order; n_byz: the dissensus
+    entries of its in_nodes (repeats included); eps >= 0 (include/rcmarl.h).  Limits are checked by the library."""
+    j = L.DissensusJob()
+    j.dst, j.msgs, j.msg_stride, j.n, j.own = dst.data_ptr(), msgs.data_ptr(), msg_stride, n, own
+    j.n_honest = len(honest)
+    for k, v in enumerate(honest[:L.MAX_NEIGHBOURS]):
+        j.honest[k] = v
+    j.n_byz, j.eps = n_byz, eps
+    j._keep = (dst, msgs)
+    return j
+
+
+def dissensus_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.DissensusJob, jobs)
+    L.check(L.lib().rcmarl_dissensus_attack(a, len(a), _stream()), "rcmarl_dissensus_attack")
+
+
+def mimic_attack_job(dst, msgs, msg_stride, n, honest, candidates, z, update, target_out=None):
+    """honest: the message rows of the receiver's honest set in list order; candidates: the indices into `honest` that
+    may be copied; z: the job's direction state [>= n] float32 (zero: not yet initialised); update: 1 to take a power
+    step (include/rcmarl.h).  The indices are checked here, limits by the library."""
+    j = L.MimicJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.z, j.target_out = z.data_ptr(), ptr(target_out)
+    j.n_honest = len(honest)
+    for k, v in enumerate(honest[:L.MAX_NEIGHBOURS]):
+        j.honest[k] = v
+    bad = [k for k in candidates if not (isinstance(k, (int, np.integer)) and 0 <= k < min(len(honest), 32))]
+    if bad:
+        raise L.RcmarlError(f"candidate indices {bad} are outside the honest set of {len(honest)}")
+    j.candidate_mask = sum(1 << int(k) for k in set(candidates))
+    j.update = int(update)
+    j._keep = (dst, msgs, z, target_out)
+    return j
+
+
+def mimic_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.MimicJob, jobs)
+    L.check(L.lib().rcmarl_mimic_attack(a, len(a), _stream()), "rcmarl_mimic_attack")
+
+
 def vector_job(dst, msgs, msg_stride, n, in_nodes, H, rule, weights_out=None):
     """rule: distance-based rule name ("krum", "mkrum", "scclip", "gmed") or rcmarl_vector_rule id (include/rcmarl.h).
     Names are checked here, ids and limits by the library."""

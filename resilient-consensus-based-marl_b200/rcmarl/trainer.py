@@ -152,6 +152,12 @@ class Trainer:
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
         # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
+        # the mimic attack's direction state z of each mimic pair (row q = mimic_pairs[q]; [q, 0, :PC] critic, [q, 1] TR),
+        # the index into S_j each copied in the last epoch, and the power steps each has taken (host)
+        self.mimic_z = torch.zeros(len(self.mimic_pairs), 2, self.PT, **f32) if self.mimic_pairs else None
+        self.mimic_target = (torch.zeros(len(self.mimic_pairs), 2, dtype=torch.int32, device=self.dev)
+                             if self.mimic_pairs else None)
+        self.mimic_steps = [0] * len(self.mimic_pairs)
         self.adam_m = torch.zeros(NA, self.PA, **f32)
         self.adam_v = torch.zeros(NA, self.PA, **f32)
         self.adam_t = [0] * NA
@@ -237,6 +243,12 @@ class Trainer:
         self.tailor_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                              if isinstance(self.attack[b][0], L.TailoredKind)]
         self.gamma_pairs = self.adapt_pairs + self.tailor_pairs
+        # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
+        # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
+        # tailored one
+        self.diss_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                           if isinstance(self.attack[b][0], L.DissensusKind)]
+        self.mimic_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs) if isinstance(self.attack[b][0], L.MimicKind)]
 
     def _receiver_nodes(self, j):
         """in_nodes[j] with each Byzantine neighbour replaced by the message row crafted for receiver j."""
@@ -291,6 +303,20 @@ class Trainer:
         g = self.att_gamma.cpu().numpy()
         self.d2h_bytes += g.nbytes
         return {self.byz_pairs[e][:2]: g[q].copy() for q, e in enumerate(self.gamma_pairs)}
+
+    def mimic_targets(self):
+        """{(attacker b, cooperative receiver j) of a mimic attack: int32 [2]}: the agent whose message b copied for j in
+        the last epoch of the last update round (include/rcmarl.h, rcmarl_mimic_attack); entry 0 for the critic, 1 for
+        the team-reward net."""
+        if not self.mimic_pairs:
+            return {}
+        k = self.mimic_target.cpu().numpy()
+        self.d2h_bytes += k.nbytes
+        out = {}
+        for q, e in enumerate(self.mimic_pairs):
+            b, j, honest = self.byz_pairs[e]
+            out[(b, j)] = np.array([honest[k[q, t]] for t in range(2)], np.int32)
+        return out
 
     def _tailored_slots(self, j):
         """(slots, honest) of receiver j for rcmarl_tailored_attack: _receiver_nodes(j) with every Byzantine pair row
@@ -505,11 +531,30 @@ class Trainer:
         # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
         # (the min-max / min-sum pairs in a job list of their own, with the gamma of each message)
         # (and the tailored pairs in a third, against their receiver's own rule and H)
-        att_jobs, ada_jobs, tail_jobs = [], [], []
+        # (then the dissensus pairs, and the mimic pairs with their direction states)
+        att_jobs, ada_jobs, tail_jobs, diss_jobs, mimic_jobs = [], [], [], [], []
         ada_row = {e: q for q, e in enumerate(self.adapt_pairs)}
         tail_row = {e: len(self.adapt_pairs) + q for q, e in enumerate(self.tailor_pairs)}
+        diss_set = set(self.diss_pairs)
+        mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
         for e, (b, j, honest) in enumerate(self.byz_pairs):
             kind, param = self.attack[b]
+            if e in diss_set:
+                # colluding dissensus attackers of j split the cancellation: n_byz counts their entries of in_nodes[j]
+                n_byz = sum(isinstance(self.attack[k][0], L.DissensusKind) for k in self.in_nodes[j]
+                            if lab[k] == BYZANTINE)
+                for msgs, P in ((self.msg_c, self.PC), (self.msg_t, self.PT)):
+                    diss_jobs.append(ops.dissensus_attack_job(msgs[NA + e], msgs, P, P, j, honest, n_byz, param))
+                continue
+            if e in mimic_row:
+                # copying the receiver to itself only slows its consensus: the candidates are S_j without j's own
+                # entries, unless that leaves none
+                q = mimic_row[e]
+                cand = [k for k, i in enumerate(honest) if i != j] or list(range(len(honest)))
+                for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                    mimic_jobs.append(ops.mimic_attack_job(msgs[NA + e], msgs, P, P, honest, cand, self.mimic_z[q, t],
+                                                           0, target_out=self.mimic_target[q, t:t + 1]))
+                continue
             if e in tail_row:
                 slots, hon = self._tailored_slots(j)
                 rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
@@ -529,6 +574,12 @@ class Trainer:
                       for g in range(0, len(ada_jobs), L.MAX_JOBS)]
         tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
                        for g in range(0, len(tail_jobs), L.MAX_JOBS)]
+        diss_groups = [ops.job_array(L.DissensusJob, diss_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(diss_jobs), L.MAX_JOBS)]
+        # mimic job 2q + t belongs to pair mimic_pairs[q]; its T0 is the attacker's parameter
+        mimic_t0 = [int(self.attack[self.byz_pairs[e][0]][1]) for e in self.mimic_pairs]
+        mimic_groups = [(g, ops.job_array(L.MimicJob, mimic_jobs[g:g + L.MAX_JOBS]))
+                        for g in range(0, len(mimic_jobs), L.MAX_JOBS)]
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
         # 16 cooperative agents x 2 nets, so one launch per epoch
@@ -584,6 +635,17 @@ class Trainer:
             for g in tail_groups:                                          # no epoch dependence either
                 ops.tailored_attack(g)
                 self.launches += 1
+            for g in diss_groups:                                          # no epoch dependence either
+                ops.dissensus_attack(g)
+                self.launches += 1
+            if mimic_groups:                                               # a power step in each pair's first T0 epochs
+                update = [int(s < t0) for s, t0 in zip(self.mimic_steps, mimic_t0)]
+                for g0, g in mimic_groups:
+                    for k, job in enumerate(g):
+                        job.update = update[(g0 + k) // 2]
+                    ops.mimic_attack(g)
+                    self.launches += 1
+                self.mimic_steps = [s + u for s, u in zip(self.mimic_steps, update)]
             if mix_jobs is not None:
                 ops.nnm_mix(mix_jobs)
                 self.launches += 1
@@ -700,16 +762,27 @@ class Trainer:
                   adam_m=self.adam_m.cpu(), adam_v=self.adam_v.cpu())
         if include_buffer:
             sd.update(sa=self.sa[:T].cpu(), ns=self.ns[:T].cpu(), r=self.r[:T].cpu())
+        if self.mimic_pairs:                       # the mimic attack's state carries over between rounds
+            sd.update(mimic_z=self.mimic_z.cpu(), mimic_steps=list(self.mimic_steps))
         return sd
 
     def load_state_dict(self, sd):
         if list(sd["labels"]) != list(self.labels) or int(sd["n_envs"]) != self.N:
             raise L.RcmarlError("checkpoint was written for a different agent set / environment count")
+        if self.mimic_pairs:
+            if "mimic_z" not in sd or "mimic_steps" not in sd:
+                raise L.RcmarlError("checkpoint holds no mimic attack state, and this trainer has mimic attackers")
+            if tuple(sd["mimic_z"].shape) != tuple(self.mimic_z.shape) or len(sd["mimic_steps"]) != len(self.mimic_steps):
+                raise L.RcmarlError(f"checkpointed mimic state of shape {tuple(sd['mimic_z'].shape)} does not match "
+                                    f"this trainer's {tuple(self.mimic_z.shape)}")
         for name in ("actor", "critic", "tr", "critic_local", "adam_m", "adam_v"):
             getattr(self, name).copy_(sd[name])
         self.adam_t = [int(t) for t in sd["adam_t"]]
         self.episodes_done = int(sd["episodes_done"])
         self._perm_gen.set_state(sd["perm_rng"])
+        if self.mimic_pairs:
+            self.mimic_z.copy_(sd["mimic_z"])
+            self.mimic_steps = [int(s) for s in sd["mimic_steps"]]
         self.t_filled = 0
         if "sa" in sd:
             T = int(sd["t_filled"]) * self.N

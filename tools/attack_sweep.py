@@ -14,13 +14,17 @@ reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in
 cells are marked refused.  A rule may be written nnm+<rule> (e.g. nnm+mkrum): every cooperative agent then mixes the
 messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, and the weight reported for a
 whole-message rule is the effective weight w M of agent 4's message.  The tailored attacks do not model mixing either.
+The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
+the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
+by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
+agent 4 copied in the last epoch of the last round (Trainer.mimic_targets, critic / team-reward net), over the seeds.
 
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
 and when it names dnc, on clip and dnc (all of them when it names both), alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
-tailored_std (every cooperative agent on clip) against gauss.
+tailored_std (every cooperative agent on clip) against gauss, and when it names mimic, the round on mimic against gauss.
 
     python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
                                  [rules=clip,trim,wmsr] [attacks=alie,ipm,gauss]
@@ -41,7 +45,8 @@ import torch                                   # noqa: E402
 from rcmarl._lib import RcmarlError            # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
-PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0}
+PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0,
+          "dissensus": 1.0, "mimic": 50.0}
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -185,6 +190,7 @@ def timing_line(rt):
 
 adaptive = any(a in ADAPTIVE + TAILORED for a, _ in ATTACKS)
 tailored = any(a in TAILORED for a, _ in ATTACKS)
+mimic = any(a == "mimic" for a, _ in ATTACKS)
 if vector:
     result["rule_timing"] = rt = rule_timing()
     print(f"update round with agent 4 Byzantine: {timing_line(rt)}", flush=True)
@@ -196,9 +202,21 @@ if tailored:
     result["tailored_timing"] = tt = adaptive_timing("tailored_std")
     print(f"update round with agent 4 Byzantine: gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std "
           f"{tt['tailored_std']['median_ms']:.2f} ms ({tt['tailored_std_added_ms']:+.3f})", flush=True)
+if mimic:
+    result["mimic_timing"] = mt = adaptive_timing("mimic")
+    print(f"update round with agent 4 Byzantine: gauss {mt['gauss']['median_ms']:.2f} ms, mimic "
+          f"{mt['mimic']['median_ms']:.2f} ms ({mt['mimic_added_ms']:+.3f})", flush=True)
+
+
+def copied_line(targets):
+    """'j: critic copies / TR copies' per receiver j over the seeds, e.g. '1: 3,3,2 / 2,3,3'."""
+    return "; ".join(f"{j}: " + ",".join(str(c) for c, _ in ks) + " / " + ",".join(str(t) for _, t in ks)
+                     for j, ks in sorted(targets.items()))
+
+
 for rule in RULES:
     for attack in ATTACKS:
-        team, est, byz, gam = [], [], [], []
+        team, est, byz, gam, copied = [], [], [], [], {}
         refused = None
         for tag in runs:
             _, _, ss = tag.split("/")
@@ -227,6 +245,8 @@ for rule in RULES:
             team.append(float(np.mean(t[-tail:]))); est.append(float(np.mean(e[-tail:])))
             byz.append(byzantine_weight(tr))
             gam.append(mean_gamma(tr))
+            for (_, j), k in tr.mimic_targets().items():
+                copied.setdefault(int(j), []).append([int(x) for x in k])
         if refused is not None:
             cell = dict(rule=rule, attack=attack[0], param=attack[1], refused=refused)
             result["cells"].append(cell)
@@ -238,10 +258,13 @@ for rule in RULES:
             cell["byz_weight"] = float(np.mean(byz)) if split_rule(rule)[1] in WHOLE else None
         if adaptive:
             cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED else None
+        if mimic:
+            cell["copied"] = {str(j): ks for j, ks in copied.items()} if copied else None
         result["cells"].append(cell)
         print(f"{rule:9s} {attack[0]:5s} {attack[1]:4.1f}: team {cell['team']:7.2f}  estimate {cell['est']:7.2f}"
               + (f"  weight of agent 4 {cell['byz_weight']:.3f}" if cell.get("byz_weight") is not None else "")
-              + (f"  gamma {cell['gamma']:.3f}" if cell.get("gamma") is not None else ""), flush=True)
+              + (f"  gamma {cell['gamma']:.3f}" if cell.get("gamma") is not None else "")
+              + (f"  copied {copied_line(copied)}" if copied else ""), flush=True)
 
 os.makedirs(out_dir, exist_ok=True)
 json.dump(result, open(os.path.join(out_dir, "attack_sweep.json"), "w"))
@@ -249,15 +272,19 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
     f.write(f"{name}, power limit {power} W; {len(runs)} seeds, {n_blocks} blocks x 50 episodes, {n_envs} environments; "
             "means of the last 500 episodes\n\n| rule | attack | team return | critic estimate |"
             + (" weight of agent 4 |" if vector else "") + (" gamma |" if adaptive else "")
-            + "\n|---|---|---|---|" + ("---|" if vector else "") + ("---|" if adaptive else "") + "\n")
+            + (" copied (receiver: critic / TR, per seed) |" if mimic else "")
+            + "\n|---|---|---|---|" + ("---|" if vector else "") + ("---|" if adaptive else "") + ("---|" if mimic else "")
+            + "\n")
     for c in result["cells"]:
         if "refused" in c:
             f.write(f"| {c['rule']} | {c['attack']} {c['param']} | refused | refused |" + (" - |" if vector else "")
-                    + (" - |" if adaptive else "") + "\n")
+                    + (" - |" if adaptive else "") + (" - |" if mimic else "") + "\n")
             continue
         f.write(f"| {c['rule']} | {c['attack']} {c['param']} | {c['team']:.2f} | {c['est']:.2f} |"
                 + ((f" {c['byz_weight']:.3f} |" if c["byz_weight"] is not None else " - |") if vector else "")
-                + ((f" {c['gamma']:.3f} |" if c["gamma"] is not None else " - |") if adaptive else "") + "\n")
+                + ((f" {c['gamma']:.3f} |" if c["gamma"] is not None else " - |") if adaptive else "")
+                + ((f" {copied_line({int(j): k for j, k in c['copied'].items()})} |" if c["copied"] else " - |")
+                   if mimic else "") + "\n")
     t = result["timing"]
     f.write(f"\nC2 update round at {t['n_envs']} environments (median of {timed_rounds}, alternated): "
             f"{t['Faulty']['median_ms']:.2f} ms with agent 4 Faulty, {t['Byzantine']['median_ms']:.2f} ms Byzantine (gauss), "
@@ -276,4 +303,9 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
         f.write(f"\nC2 update round at {tt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
                 f"gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std {tt['tailored_std']['median_ms']:.2f} ms "
                 f"({tt['tailored_std_added_ms']:+.3f} ms)\n")
+    if mimic:
+        mt = result["mimic_timing"]
+        f.write(f"\nC2 update round at {mt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
+                f"gauss {mt['gauss']['median_ms']:.2f} ms, mimic {mt['mimic']['median_ms']:.2f} ms "
+                f"({mt['mimic_added_ms']:+.3f} ms)\n")
 print(open(os.path.join(out_dir, "attack_sweep.md")).read())
