@@ -445,8 +445,50 @@ int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* s
  * memory), a written range (the n_in dst rows, the n_in^2 weights) that overlaps an in-node row of any job of the
  * launch, and two written ranges of the launch that overlap. */
 #define RCMARL_NNM_MAX_FLOATS (48 * 1024)
-typedef enum { RCMARL_MIX_NNM = 0 } rcmarl_mixing_rule;
+typedef enum { RCMARL_MIX_NNM = 0, RCMARL_MIX_BUCKET = 1 } rcmarl_mixing_rule;
 int rcmarl_nnm_mix(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
+/* Randomized bucketing (rcmarl_bucket_mix): the pre-aggregation step of Karimireddy, He & Jaggi, "Byzantine-robust
+ * learning on heterogeneous datasets via bucketing" (ICLR 2022).  The messages a receiver hears are shuffled into
+ * buckets of s and each bucket is replaced by its mean; the receiver's own rule then runs on the bucket means.  Unlike
+ * the paper, the receiver's own message x_0 -- the one row it knows to be honest -- passes through and is not bucketed,
+ * so n_in = 4 at s = 2 gives the rule 3 rows.  One job is one (receiver, net): n = n_in message slots x_0 .. x_{n-1},
+ * x_k = msgs + in_nodes[k] * msg_stride (x_0 the receiver's own; repeats in in_nodes count), each of P = job.n packed
+ * parameters.  All arithmetic is fp32.  With m = n - 1:
+ *   Permutation  pi = [1, .., m] shuffled by Fisher-Yates for i = m-1 down to 1 (0-based positions): draw t (t = 0 for
+ *            the first swap) is the 32-bit word u = word (t & 3) of Philox4x32-10 with key (seed low word, seed high
+ *            word) and counter (t >> 2, receiver | net << 8 | 0x20000000, round, epoch); j = (u * (i + 1)) >> 32 in 64
+ *            bits, and pi[i], pi[j] are swapped.  Bit 29 of word 1 keeps the stream apart from the rollout's and from
+ *            rcmarl_attack's (bit 30).  The draw depends on (seed, round, epoch, receiver, net) only, never on the
+ *            launch or the job order.
+ *   Buckets  B = ceil(m / s); bucket b holds the slots pi[b*s .. min((b+1)*s, m) - 1].
+ *   Output   n_out = 1 + B rows at dst + r * msg_stride: row 0 = x_0 bitwise; row 1 + b = (sum of bucket b's members,
+ *            in increasing slot order (not pi order), an fp32 sum from 0) / (float)|bucket b| (multi-Krum's and
+ *            rcmarl_nnm_mix's arithmetic; the paper's 1/s when s divides m).  If any coordinate of that mean is not
+ *            finite, every coordinate of row 1 + b is +inf, so at most H poisoned inputs give at most H poisoned rows.
+ *            weights_out, when not NULL, receives M row-major [n_out][n_in]: M_00 = 1, M_(1+b)l = 1/|bucket b| for
+ *            every slot l in bucket b, 0 elsewhere.
+ * n_in = 1 gives the own row only; s >= m a single bucket (the mean of every received message); s = 1 the received
+ * messages in permuted order, each copied bitwise.  NaN inputs are not supported.  One CTA per job, the permutation in
+ * shared memory, fixed summation orders, no atomics: bitwise reproducible, independent of the job order and of how jobs
+ * are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, every dst row and weights_out untouched): n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, s < 1, net
+ * other than 0 or 1, receiver > 255, a written range (the n_out dst rows, the n_out * n_in weights) that overlaps an
+ * in-node row of any job of the launch, and two written ranges of the launch that overlap. */
+typedef struct {
+    float* dst;                 /* n_out rows at dst + r * msg_stride */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    float* weights_out;         /* optional [n_out * n_in]: M */
+    int32_t n;                  /* parameters per message */
+    int32_t n_in;
+    int32_t s;                  /* bucket size, >= 1 */
+    int32_t in_nodes[RCMARL_MAX_NEIGHBOURS];
+    uint64_t seed;              /* Philox key */
+    uint32_t receiver, net, round, epoch;   /* Philox counter words */
+} rcmarl_bucket_job;
+int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs_host, int n_jobs, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]

@@ -9,13 +9,16 @@ Same constructor and method names, argument meaning and mutation conventions as 
                                  ("dnc") aggregate of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
                                  With mixing="nnm", every consensus step first replaces each received message by the
-                                 mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix)
+                                 mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix); with
+                                 mixing="bucket" or ("bucket", s) it keeps its own message and replaces the others by
+                                 the means of random buckets of s (randomized bucketing, rcmarl_bucket_mix)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
 Tensors may be NumPy arrays, torch tensors or facade Tensors; they are moved to the GPU.  Calling these methods one
 by one is the compatibility path; training.train_agents.train_RPBCAC drives the same kernels fused over all agents."""
 import torch
 
+import tensorflow
 from tensorflow import keras
 from tensorflow.keras import Tensor
 from rcmarl import _lib as L
@@ -36,10 +39,14 @@ class RPBCAC_agent():
         if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation)):
             L.agg_rule(aggregation)
         self.aggregation = aggregation
-        # pre-aggregation mixing of the received messages: None or "nnm" (rcmarl_mixing_rule)
+        # pre-aggregation mixing of the received messages: None, "nnm", "bucket" or ("bucket", s) (rcmarl_mixing_rule)
         if mixing is not None:
             L.check_mixing(mixing, 0, 1)
-        self.mixing = mixing
+        self.mixing = L.mixing_entry(mixing)
+        # bucketing draws its permutations from Philox keyed by the facade seed of tf.random.set_seed at construction,
+        # with receiver 0 and epoch 0; the round is a per-net count of hidden consensus calls (0 critic, 1 team reward)
+        self._bucket_seed = tensorflow.random.seed
+        self._consensus_calls = [0, 0]
         self.n_actions = self.actor.output_shape[1]
         self.fast_lr = fast_lr
         self.slow_lr = slow_lr
@@ -52,7 +59,7 @@ class RPBCAC_agent():
     def _resilient_aggregation(self, values_innodes):
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
-        v = self._mixed(v.reshape(v.shape[0], -1).contiguous())
+        v = self._mixed(v.reshape(v.shape[0], -1).contiguous(), net=0, round=0)
         if self._whole_messages():                # the rows as whole vectors: out = sum_k w_k v_k
             out = self._with_aggregate(v)[-1]
         elif L.agg_rule(self.aggregation) == L.AGG_CLIP:
@@ -64,12 +71,18 @@ class RPBCAC_agent():
                                                     self.aggregation)])
         return Tensor(out.reshape(shape))
 
-    def _mixed(self, stack):
-        """[n, P] device stack (own = row 0) -> its n nearest-neighbour mixed rows if the agent mixes, else the stack."""
+    def _mixed(self, stack, net, round):
+        """[n, P] device stack (own = row 0) -> its n nearest-neighbour mixed rows, or its 1 + ceil((n - 1) / s) rows
+        bucketed with the draws of (net, round), if the agent mixes; else the stack."""
         if self.mixing is None:
             return stack
         n, P = stack.shape
         L.check_mixing(self.mixing, self.H, n)
+        if L.is_bucket_mixing(self.mixing):
+            out = torch.empty(L.mixed_rows(self.mixing, n), P, dtype=stack.dtype, device=stack.device)
+            ops.bucket_mix([ops.bucket_job(out, stack, P, P, list(range(n)), self.mixing[1], seed=self._bucket_seed,
+                                           receiver=0, net=net, round=round & 0xFFFFFFFF, epoch=0)])
+            return out
         out = torch.empty_like(stack)
         ops.nnm_mix([ops.vector_job(out, stack, P, P, list(range(n)), self.H, L.MIX_NNM)])
         return out
@@ -91,11 +104,11 @@ class RPBCAC_agent():
             ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
         return out
 
-    def _consensus_inputs(self, stack):
+    def _consensus_inputs(self, stack, net, round):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
         distance-based or dnc rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
-        Trainer.  An agent that mixes does so first."""
-        stack = self._mixed(stack)
+        Trainer.  An agent that mixes does so first (a bucketing agent with the draws of (net, round))."""
+        stack = self._mixed(stack, net, round)
         if self._whole_messages():
             return self._with_aggregate(stack), [stack.shape[0]], 0, "clip"
         return stack, list(range(stack.shape[0])), self.H, self.aggregation
@@ -134,32 +147,37 @@ class RPBCAC_agent():
         return A.DeviceWeights(msg, self.TR.d_in, 1), loss
 
     # ------------------------------------------------------------------ hidden-layer consensus (:142-166)
-    def _hidden(self, model, msgs_innodes):
+    def _hidden(self, model, msgs_innodes, net):
         dev = model.flat.device
-        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]))
+        round = self._consensus_calls[net]
+        self._consensus_calls[net] += 1
+        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]),
+                                                       net, round)
         ops.consensus_hidden([ops.consensus_job(model.flat, stack, stack.shape[1], nets.n_hidden_params(model.d_in_k),
                                                 nodes, H, rule)])
 
     def resilient_consensus_critic_hidden(self, critic_weights_innodes):
-        self._hidden(self.critic, critic_weights_innodes)
+        self._hidden(self.critic, critic_weights_innodes, 0)
 
     def resilient_consensus_TR_hidden(self, TR_weights_innodes):
-        self._hidden(self.TR, TR_weights_innodes)
+        self._hidden(self.TR, TR_weights_innodes, 1)
 
     # ------------------------------------------------------------------ estimate consensus (:168-206)
-    def _estimates(self, model, x, msgs_innodes):
+    def _estimates(self, model, x, msgs_innodes, net):
+        # the round of the last hidden consensus of this net: both see the same buckets, as in one Trainer epoch
         rows, kind, xf = A.rows_for(x, self.n_agents)
         dev = xf.device
-        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]))
+        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]),
+                                                       net, max(self._consensus_calls[net] - 1, 0))
         agg = torch.empty(xf.shape[0], dtype=torch.float32, device=dev)
         ops.team(rows, [ops.team_job(model.flat, kind, stack, stack.shape[1], nodes, H, agg_out=agg, rule=rule)])
         return Tensor(agg.reshape(-1, 1))
 
     def resilient_consensus_critic(self, s, critic_weights_innodes):
-        return self._estimates(self.critic, s, critic_weights_innodes)
+        return self._estimates(self.critic, s, critic_weights_innodes, 0)
 
     def resilient_consensus_TR(self, sa, TR_weights_innodes):
-        return self._estimates(self.TR, sa, TR_weights_innodes)
+        return self._estimates(self.TR, sa, TR_weights_innodes, 1)
 
     # ------------------------------------------------------------------ acting (:208-219)
     def get_action(self, state, mu=0.1):

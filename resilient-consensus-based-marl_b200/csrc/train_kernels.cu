@@ -14,6 +14,8 @@
 //   dnc_agg_kernel  divide-and-conquer: removes the messages furthest along the top principal direction
 //                   (rcmarl_dnc_aggregate)
 //   nnm_mix_kernel  nearest-neighbour mixing: each message becomes the mean of its n - H nearest (rcmarl_nnm_mix)
+//   bucket_mix_kernel  randomized bucketing: the received messages are shuffled into buckets of s and replaced by the
+//                   bucket means (rcmarl_bucket_mix)
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
@@ -778,6 +780,77 @@ __global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_const
     if (job.weights_out && tid < nin * nin) {
         const unsigned mask = sel[tid / nin];
         job.weights_out[tid] = ((mask >> (tid % nin)) & 1u) ? 1.f / (float)__popc(mask) : 0.f;
+    }
+}
+
+// Randomized bucketing (rcmarl_bucket_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  Thread 0 draws
+// the permutation into shared memory and keeps each bucket as a bit mask over the slots; the rows take one thread per
+// coordinate and add each bucket's members in slot order straight from global memory (every received row is read
+// once).  A bucket with a non-finite mean coordinate raises its flag, and after the barrier its row is rewritten as +inf.
+struct BucketParams { rcmarl_bucket_job jobs[RCMARL_MAX_JOBS]; };
+
+__global__ void __launch_bounds__(VEC_THREADS) bucket_mix_kernel(const __grid_constant__ BucketParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    static_assert(MAXN * MAXN <= VEC_THREADS, "one thread per entry of M");
+    __shared__ int pi[MAXN];
+    __shared__ unsigned members[MAXN];             // bucket b: bit l set for slot l in the bucket
+    __shared__ int poisoned[MAXN];                 // bucket b's mean has a coordinate that is not finite
+    const rcmarl_bucket_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in, m = nin - 1;
+    const int nb = m == 0 ? 0 : (m - 1) / job.s + 1;   // ceil(m / s) without overflow at a huge s
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        for (int q = 0; q < m; ++q) pi[q] = q + 1;
+        const uint2 key = make_uint2((uint32_t)job.seed, (uint32_t)(job.seed >> 32));
+        uint4 r = make_uint4(0u, 0u, 0u, 0u);
+        for (int i = m - 1, t = 0; i >= 1; --i, ++t) {
+            if ((t & 3) == 0)
+                r = philox4x32_10(make_uint4((uint32_t)(t >> 2), job.receiver | job.net << 8 | 0x20000000u, job.round,
+                                             job.epoch), key);
+            const uint32_t u = (t & 3) == 0 ? r.x : (t & 3) == 1 ? r.y : (t & 3) == 2 ? r.z : r.w;
+            const int j = (int)(((uint64_t)u * (uint64_t)(i + 1)) >> 32);
+            const int a = pi[i];
+            pi[i] = pi[j];
+            pi[j] = a;
+        }
+        for (int b = 0; b < nb; ++b) {
+            members[b] = 0u;
+            poisoned[b] = 0;
+        }
+        for (int q = 0; q < m; ++q) members[q / job.s] |= 1u << pi[q];
+    }
+    __syncthreads();
+    const float* own = job.msgs + (int64_t)job.in_nodes[0] * job.msg_stride;
+    for (int p = tid; p < n; p += VEC_THREADS) job.dst[p] = __ldg(own + p);
+    for (int b = 0; b < nb; ++b) {
+        const unsigned mask = members[b];
+        const float cnt = (float)__popc(mask);
+        float* dst = job.dst + (int64_t)(1 + b) * job.msg_stride;
+        bool bad = false;
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            float s = 0.f;
+            for (int l = 1; l < nin; ++l)
+                if ((mask >> l) & 1u) s += __ldg(job.msgs + (int64_t)job.in_nodes[l] * job.msg_stride + p);
+            const float v = s / cnt;
+            bad |= !isfinite(v);
+            dst[p] = v;
+        }
+        if (bad) poisoned[b] = 1;                  // every writer stores the same value
+    }
+    __syncthreads();
+    for (int b = 0; b < nb; ++b) {
+        if (!poisoned[b]) continue;
+        float* dst = job.dst + (int64_t)(1 + b) * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) dst[p] = INFINITY;
+    }
+    if (job.weights_out && tid < (1 + nb) * nin) {
+        const int r = tid / nin, l = tid % nin;
+        float w = r == 0 && l == 0 ? 1.f : 0.f;
+        if (r > 0) {
+            const unsigned mask = members[r - 1];
+            w = ((mask >> l) & 1u) ? 1.f / (float)__popc(mask) : 0.f;
+        }
+        job.weights_out[tid] = w;
     }
 }
 
@@ -1796,6 +1869,39 @@ int rcmarl_nnm_mix(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (int e = opt_in_smem((const void*)nnm_mix_kernel, (int)(sizeof(float) * RCMARL_NNM_MAX_FLOATS), opted)) return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     nnm_mix_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    BucketParams P;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_bucket_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (q.s < 1 || q.net > 1u || q.receiver > 255u) return RCMARL_ERR_ARG;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_nnm_mix, with n_out = 1 + ceil((n_in - 1) / s) dst rows per job: no written range (a dst row, a
+    // weights_out) may overlap an in-node row of any job of the launch or another written range
+    constexpr int MAX_W = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1), MAX_R = RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS;
+    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_bucket_job& q = jobs[j];
+        const int n_out = q.n_in == 1 ? 1 : 1 + (q.n_in - 2) / q.s + 1;
+        for (int k = 0; k < n_out; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
+        if (q.weights_out) {
+            float_range(q.weights_out, 0, 0, (int64_t)n_out * q.n_in, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < q.n_in; ++k, ++n_r)
+            float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    bucket_mix_kernel<<<n_jobs, VEC_THREADS, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

@@ -6,6 +6,7 @@ fails, an exception is raised.  The library is built in-tree by
 """
 import ctypes as C
 import math
+import numbers
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -48,6 +49,9 @@ DNC_MAX_FLOATS = 48 * 1024
 MIX_NNM = 0                                       # rcmarl_mixing_rule
 MIXING_RULES = {"nnm": MIX_NNM}
 NNM_MAX_FLOATS = 48 * 1024
+MIX_BUCKET = 1                                    # rcmarl_mixing_rule: randomized bucketing, ("bucket", s)
+BUCKET_DEFAULT_S = 2                              # the bucket size of a plain "bucket" entry
+BUCKET_MAX_S = 2 ** 31 - 1
 MIMIC_MAX_FLOATS = 19 * 1536                      # rcmarl_mimic_attack's staging bound
 MIMIC_MAX_T0 = 2 ** 31 - 1                        # the mimic attack's power steps T0: an integer in 0 .. 2^31 - 1
 
@@ -97,6 +101,12 @@ class MimicJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("z", c_fp), ("target_out", c_fp),
                 ("n", C.c_int32), ("n_honest", C.c_int32), ("honest", C.c_int32 * MAX_NEIGHBOURS),
                 ("candidate_mask", C.c_uint32), ("update", C.c_int32)]
+
+
+class BucketJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("weights_out", c_fp), ("n", C.c_int32),
+                ("n_in", C.c_int32), ("s", C.c_int32), ("in_nodes", C.c_int32 * MAX_NEIGHBOURS), ("seed", C.c_uint64),
+                ("receiver", C.c_uint32), ("net", C.c_uint32), ("round", C.c_uint32), ("epoch", C.c_uint32)]
 
 
 class ValueJob(C.Structure):
@@ -155,6 +165,7 @@ SYMBOLS = [
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
@@ -265,15 +276,48 @@ def check_spectral_rule(H, n_in):
     return SPECTRAL_DNC
 
 
+def mixing_entry(mixing):
+    """A pre-aggregation mixing entry in its stored form: None, "nnm" (rcmarl_nnm_mix) or ("bucket", s)
+    (rcmarl_bucket_mix, bucket size s); "bucket" stands for ("bucket", BUCKET_DEFAULT_S).  Raise RcmarlError for
+    anything else, an s that is not an integer in 1 .. BUCKET_MAX_S included."""
+    if mixing is None or (isinstance(mixing, str) and mixing in MIXING_RULES):
+        return mixing
+    if isinstance(mixing, str) and mixing == "bucket":
+        return ("bucket", BUCKET_DEFAULT_S)
+    if isinstance(mixing, tuple) and len(mixing) == 2 and isinstance(mixing[0], str) and mixing[0] == "bucket":
+        s = mixing[1]
+        if not (isinstance(s, numbers.Integral) and not isinstance(s, bool) and 1 <= s <= BUCKET_MAX_S):
+            raise RcmarlError(f"mixing 'bucket' needs an integer bucket size s in 1 .. {BUCKET_MAX_S}, got {s!r}")
+        return ("bucket", int(s))
+    raise RcmarlError(f"unknown mixing rule {mixing!r}: expected None or one of "
+                      f"{sorted(MIXING_RULES) + ['bucket', ('bucket', 's')]}")
+
+
+def is_bucket_mixing(mixing):
+    """True for a bucketing entry ("bucket" or ("bucket", s)); the entry is not otherwise checked."""
+    return mixing == "bucket" or (isinstance(mixing, tuple) and len(mixing) == 2 and mixing[0] == "bucket")
+
+
 def check_mixing(name, H, n_in):
-    """Raise RcmarlError unless `name` names a pre-aggregation mixing rule (rcmarl_mixing_rule: "nnm") that allows H
-    out of n_in messages (rcmarl_nnm_mix, include/rcmarl.h): 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  Returns
-    the rcmarl_mixing_rule id."""
-    if not isinstance(name, str) or name not in MIXING_RULES:
-        raise RcmarlError(f"unknown mixing rule {name!r}: expected None or one of {sorted(MIXING_RULES)}")
+    """Raise RcmarlError unless `name` is a pre-aggregation mixing entry ("nnm", "bucket" or ("bucket", s), see
+    mixing_entry) that allows H out of n_in messages (rcmarl_nnm_mix / rcmarl_bucket_mix, include/rcmarl.h):
+    1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  Returns the rcmarl_mixing_rule id."""
+    entry = mixing_entry(name)
+    if entry is None:
+        raise RcmarlError(f"unknown mixing rule {name!r}: expected None or one of "
+                          f"{sorted(MIXING_RULES) + ['bucket', ('bucket', 's')]}")
     if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
         raise RcmarlError(f"mixing {name!r} with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
-    return MIXING_RULES[name]
+    return MIX_BUCKET if is_bucket_mixing(entry) else MIXING_RULES[entry]
+
+
+def mixed_rows(mixing, n_in):
+    """The number of rows an agent's rule reads after its mixing entry over n_in received messages: n_in without
+    mixing and for "nnm"; 1 + ceil((n_in - 1) / s) for bucketing (the own row, then one mean per bucket)."""
+    entry = mixing_entry(mixing)
+    if entry is None or entry == "nnm":
+        return n_in
+    return 1 + -(-(n_in - 1) // entry[1])
 
 
 def is_adaptive_attack(name):

@@ -498,3 +498,25 @@ def env_step(state, action, desired, nrow, reward=None):
     L.check(L.lib().rcmarl_env_step(state.data_ptr(), action.data_ptr(), desired.data_ptr(), n_envs, n_agents, nrow,
                                     reward.data_ptr(), _stream()), "rcmarl_env_step")
     return reward
+
+
+def bucket_job(dst, msgs, msg_stride, n, in_nodes, s, seed=0, receiver=0, net=0, round=0, epoch=0, weights_out=None):
+    """rcmarl_bucket_job: in_nodes the receiver's message rows (own first); s the bucket size; (seed, receiver, net,
+    round, epoch) the Philox key and counter words of the permutation; weights_out [n_out * n_in] for M
+    (include/rcmarl.h).  Limits are checked by the library."""
+    j = L.BucketJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.weights_out = ptr(weights_out)
+    j.n_in, j.s = len(in_nodes), s
+    for k, v in enumerate(in_nodes[:L.MAX_NEIGHBOURS]):
+        j.in_nodes[k] = v
+    j.seed, j.receiver, j.net, j.round, j.epoch = int(seed), receiver, net, round, epoch
+    j._keep = (dst, msgs, weights_out)
+    return j
+
+
+def bucket_mix(jobs):
+    """rcmarl_bucket_mix over bucket_job jobs: row r of the n_out = 1 + ceil((n_in - 1) / s) output rows goes to
+    dst + r * msg_stride."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.BucketJob, jobs)
+    L.check(L.lib().rcmarl_bucket_mix(a, len(a), _stream()), "rcmarl_bucket_mix")

@@ -66,16 +66,22 @@ class Trainer:
         self.dnc = [L.is_spectral_rule(a) for a in agg] + [False] * (NA - n_real)
         self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) or L.is_spectral_rule(a) else L.agg_rule(a) for a in agg] \
             + [L.AGG_CLIP] * (NA - n_real)
-        for i in self.coop:
+
+        def check_rule(i, n):
             if self.vector_rule[i] is not None:
-                L.check_vector_rule(agg[i], self.H[i], len(self.in_nodes[i]))
+                L.check_vector_rule(agg[i], self.H[i], n)
             elif self.dnc[i]:
-                L.check_spectral_rule(self.H[i], len(self.in_nodes[i]))
+                L.check_spectral_rule(self.H[i], n)
             else:
-                L.check_aggregation(agg[i], self.H[i], len(self.in_nodes[i]))
-        # Nearest-neighbour mixing ("nnm") before a cooperative agent's rule: its n_in received messages become n_in
-        # mixed message rows (rcmarl_nnm_mix), which its rule then reads in their place with the same H
-        mix = [mixing] * n_real if mixing is None or isinstance(mixing, str) else list(mixing)
+                L.check_aggregation(agg[i], self.H[i], n)
+        for i in self.coop:
+            check_rule(i, len(self.in_nodes[i]))
+        # Pre-aggregation mixing before a cooperative agent's rule, which then reads the mixed rows in place of its
+        # received messages with the same H: nearest-neighbour mixing ("nnm", rcmarl_nnm_mix) gives n_in mixed rows;
+        # bucketing (("bucket", s), rcmarl_bucket_mix) gives the own row and ceil((n_in - 1) / s) bucket means, so the
+        # rule is checked again at that smaller count
+        one = mixing is None or isinstance(mixing, str) or L.is_bucket_mixing(mixing)
+        mix = [mixing] * n_real if one else list(mixing)
         if len(mix) != n_real:
             raise L.RcmarlError("mixing must be None, one mixing rule or one entry per agent")
         self.mixing = [None] * NA
@@ -83,8 +89,16 @@ class Trainer:
             if mix[i] is None:
                 continue
             if i in self.coop:
-                L.check_mixing(mix[i], self.H[i], len(self.in_nodes[i]))
-                self.mixing[i] = mix[i]
+                n_in = len(self.in_nodes[i])
+                L.check_mixing(mix[i], self.H[i], n_in)
+                self.mixing[i] = L.mixing_entry(mix[i])
+                if L.is_bucket_mixing(self.mixing[i]):
+                    n_out = L.mixed_rows(self.mixing[i], n_in)
+                    try:
+                        check_rule(i, n_out)
+                    except L.RcmarlError as ex:
+                        raise L.RcmarlError(f"agent {i} buckets its {n_in} messages into {n_out} rows (mixing "
+                                            f"{self.mixing[i]!r}): {ex}") from None
             else:                                  # only cooperative agents aggregate: the name alone is checked
                 L.check_mixing(mix[i], 0, 1)
         self._init_attacks(attack)
@@ -102,12 +116,13 @@ class Trainer:
         self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
         self.dnc_agents = [i for i in self.coop if self.dnc[i]]
         self.dnc_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + q for q, i in enumerate(self.dnc_agents)}
-        # then the n_in mixed rows of each cooperative agent that mixes: mixed row k at mix_row[i] + k
+        # then the mixed rows of each cooperative agent that mixes (n_in for nnm, n_out for bucketing): mixed row k at
+        # mix_row[i] + k
         self.mix_agents = [i for i in self.coop if self.mixing[i] is not None]
         self.mix_row, row = {}, NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
         for i in self.mix_agents:
             self.mix_row[i] = row
-            row += len(self.in_nodes[i])
+            row += L.mixed_rows(self.mixing[i], len(self.in_nodes[i]))
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -141,14 +156,15 @@ class Trainer:
         # vec_row[i] / dnc_row[i] the aggregate of cooperative agent i's distance-based / dnc rule; mix_row[i] + k its
         # mixed message k
         n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) \
-            + sum(len(self.in_nodes[i]) for i in self.mix_agents)
+            + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
         self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
         # ... and of each dnc aggregate: row 2q critic, 2q + 1 TR of dnc_agents[q]
         self.dnc_weights = torch.zeros(2 * len(self.dnc_agents), L.MAX_NEIGHBOURS, **f32) if self.dnc_agents else None
-        # mixing matrix M (row-major [n_in][n_in]) of each agent that mixes: row 2q critic, 2q + 1 TR of mix_agents[q]
+        # mixing matrix M (row-major [n_rows][n_in], n_rows = len(_rule_nodes(i))) of each agent that mixes: row 2q
+        # critic, 2q + 1 TR of mix_agents[q]
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
         # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
@@ -259,20 +275,21 @@ class Trainer:
         """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, else _receiver_nodes(j)."""
         if self.mixing[j] is None:
             return self._receiver_nodes(j)
-        return list(range(self.mix_row[j], self.mix_row[j] + len(self.in_nodes[j])))
+        return list(range(self.mix_row[j], self.mix_row[j] + L.mixed_rows(self.mixing[j], len(self.in_nodes[j]))))
 
     def neighbour_weights(self):
         """{cooperative agent i with a distance-based or the dnc rule: float32 [2, n_in]}: the weight w_k its rule gave
         each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in
         the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.  For an agent that
-        mixes, the rule weighs the mixed messages, and the entry is the effective weight w M of each in-neighbour."""
+        mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry is the effective
+        weight w M of each in-neighbour."""
         out = {}
         for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights)):
             if not agents:
                 continue
             w = weights.cpu().numpy()
             self.d2h_bytes += w.nbytes
-            out.update({i: w[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(agents)})
+            out.update({i: w[2 * q:2 * q + 2, :len(self._rule_nodes(i))].copy() for q, i in enumerate(agents)})
         if any(self.mixing[i] is not None for i in out):
             mix = self.mixing_matrices()
             for i in out:
@@ -281,17 +298,19 @@ class Trainer:
         return out
 
     def mixing_matrices(self):
-        """{cooperative agent i that mixes: float32 [2, n_in, n_in]}: the mixing matrix M of the last epoch of the last
-        update round, M[k, l] = 1/|N_k| if in-neighbour l (in_nodes[i] order) is among the nearest of k and 0 otherwise
-        (rcmarl_nnm_mix); [0] for the critic, [1] for the team-reward net."""
+        """{cooperative agent i that mixes: float32 [2, n_out, n_in]}: the mixing matrix M of the last epoch of the last
+        update round; [0] for the critic, [1] for the team-reward net.  For nnm n_out = n_in and M[k, l] = 1/|N_k| if
+        in-neighbour l (in_nodes[i] order) is among the nearest of k and 0 otherwise (rcmarl_nnm_mix); for bucketing
+        n_out = 1 + ceil((n_in - 1) / s), M[0, 0] = 1 and M[1 + b, l] = 1/|bucket b| if l is in bucket b
+        (rcmarl_bucket_mix)."""
         if not self.mix_agents:
             return {}
         m = self.mix_weights.cpu().numpy()
         self.d2h_bytes += m.nbytes
         out = {}
         for q, i in enumerate(self.mix_agents):
-            n = len(self.in_nodes[i])
-            out[i] = m[2 * q:2 * q + 2, :n * n].reshape(2, n, n).copy()
+            n, n_out = len(self.in_nodes[i]), len(self._rule_nodes(i))
+            out[i] = m[2 * q:2 * q + 2, :n_out * n].reshape(2, n_out, n).copy()
         return out
 
     def attack_gammas(self):
@@ -582,13 +601,23 @@ class Trainer:
                         for g in range(0, len(mimic_jobs), L.MAX_JOBS)]
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
-        # 16 cooperative agents x 2 nets, so one launch per epoch
-        mix_jobs = []
+        # 16 cooperative agents x 2 nets, so one nnm launch and one bucketing launch per epoch.  A bucketing job draws
+        # its permutation from (seed, round, epoch, receiver, net), so every epoch buckets anew and every rank of a
+        # data-parallel run draws the same buckets.
+        mix_jobs, bucket_jobs = [], []
         for q, i in enumerate(self.mix_agents):
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
-                mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i), self.H[i],
-                                               L.MIX_NNM, weights_out=self.mix_weights[2 * q + t]))
+                if L.is_bucket_mixing(self.mixing[i]):
+                    bucket_jobs.append(ops.bucket_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i),
+                                                      self.mixing[i][1], seed=self.seed, receiver=i, net=t,
+                                                      round=self.episodes_done & 0xFFFFFFFF,
+                                                      weights_out=self.mix_weights[2 * q + t]))
+                else:
+                    mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i),
+                                                   self.H[i], L.MIX_NNM, weights_out=self.mix_weights[2 * q + t]))
         mix_jobs = ops.job_array(L.VectorJob, mix_jobs) if mix_jobs else None
+        bucket_groups = [ops.job_array(L.BucketJob, bucket_jobs[g:g + L.MAX_JOBS])
+                         for g in range(0, len(bucket_jobs), L.MAX_JOBS)]
         # distance-based aggregates over the messages each receiver hears (or their mixed rows): at most 16
         # cooperative agents x 2 nets, so one launch per epoch
         vec_jobs = []
@@ -648,6 +677,11 @@ class Trainer:
                 self.mimic_steps = [s + u for s, u in zip(self.mimic_steps, update)]
             if mix_jobs is not None:
                 ops.nnm_mix(mix_jobs)
+                self.launches += 1
+            for g in bucket_groups:
+                for job in g:
+                    job.epoch = epoch
+                ops.bucket_mix(g)
                 self.launches += 1
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)

@@ -13,7 +13,10 @@ reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in
 (Trainer.attack_gammas, both nets and every receiver), over the seeds.  The tailored attacks do not model dnc: those
 cells are marked refused.  A rule may be written nnm+<rule> (e.g. nnm+mkrum): every cooperative agent then mixes the
 messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, and the weight reported for a
-whole-message rule is the effective weight w M of agent 4's message.  The tailored attacks do not model mixing either.
+whole-message rule is the effective weight w M of agent 4's message.  Likewise bucket+<rule> (s = 2) or
+bucket<s>+<rule> (e.g. bucket3+gmed) buckets the messages (rcmarl_bucket_mix) before the rule, which then reads the own
+row and ceil(3 / s) bucket means at C2; a rule that refuses that many rows at H = 1 (krum, mkrum at s = 2) is marked
+refused.  The tailored attacks do not model mixing either.
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -55,8 +58,14 @@ RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","
 
 
 def split_rule(rule):
-    """(mixing, aggregation rule) of a rule name: "nnm+mkrum" -> ("nnm", "mkrum"), "mkrum" -> (None, "mkrum")."""
-    return ("nnm", rule[4:]) if rule.startswith("nnm+") else (None, rule)
+    """(mixing, aggregation rule) of a rule name: "nnm+mkrum" -> ("nnm", "mkrum"), "bucket+gmed" -> (("bucket", 2),
+    "gmed"), "bucket3+gmed" -> (("bucket", 3), "gmed"), "mkrum" -> (None, "mkrum")."""
+    if rule.startswith("nnm+"):
+        return "nnm", rule[4:]
+    if rule.startswith("bucket") and "+" in rule:
+        s, base = rule[6:].split("+", 1)
+        return ("bucket", int(s) if s else 2), base
+    return None, rule
 
 
 BASES = tuple(split_rule(r)[1] for r in RULES)
