@@ -244,14 +244,15 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs_host, int n_jo
  * orders, no atomics -- bitwise reproducible, independent of the job order and of how jobs are split over launches.
  * Refused (RCMARL_ERR_ARG, nothing launched, dst and gamma_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null dst
  * or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, no crafted slot, no honest slot, a crafted slot marked honest,
- * a honest_mask bit at or past n_in, a slot below -1, an unknown family, rule or dev, an H the rule refuses for n_in
- * (the checks of rcmarl_consensus_hidden and rcmarl_vector_aggregate), a scale that is not finite or is < 0,
+ * a honest_mask bit at or past n_in, a slot below -1, an unknown family (RCMARL_TAILOR_SPECTRAL too: only
+ * rcmarl_pipeline_attack models DnC), rule or dev, an H the rule refuses for n_in (the checks of
+ * rcmarl_consensus_hidden and rcmarl_vector_aggregate), a scale that is not finite or is < 0,
  * (n_in + 3) * n > RCMARL_TAILORED_MAX_FLOATS (the staging bound: 15 real slots, mu, d, the candidate and the work row
  * of up to 1536 parameters), a dst or gamma_out that overlaps a real slot's row of any job of the launch, and two
  * written ranges (dsts, gamma_outs) of the launch that overlap.  NaN inputs are not supported. */
 #define RCMARL_TAILORED_STEPS 32
 #define RCMARL_TAILORED_MAX_FLOATS (19 * 1536)
-typedef enum { RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1 } rcmarl_tailored_family;
+typedef enum { RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1, RCMARL_TAILOR_SPECTRAL = 2 } rcmarl_tailored_family;
 typedef struct {
     float* dst;                 /* the crafted message (packed network) */
     const float* msgs;          /* base of the message stack */
@@ -490,6 +491,59 @@ typedef struct {
 } rcmarl_bucket_job;
 int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs_host, int n_jobs, void* stream);
 
+/* Pipeline-aware Byzantine messages (rcmarl_pipeline_attack): the AGR-tailored attack of rcmarl_tailored_attack against
+ * the receiver's whole aggregation pipeline -- its mixing step (none, rcmarl_nnm_mix or rcmarl_bucket_mix), then its rule,
+ * DnC included.  Threat model: that of rcmarl_tailored_attack, plus the receiver's mixing step; a bucketing receiver's
+ * shuffle stays secret (it is that defence's premise), so the attacker draws shuffles of its own.  One job is one
+ * (attacker, receiver j, net); `attack` holds the fields of rcmarl_tailored_attack_job with their meaning there.  All
+ * arithmetic is fp32 (DnC's centring and eigen-solve fp64, as in rcmarl_dnc_aggregate).
+ *   Search.  mu, d, gamma_mm, Gamma, the K + 1 candidates gamma_i, m(gamma_i) and the slot list x(gamma_i) exactly as in
+ *           rcmarl_tailored_attack (the same device code and summation orders).
+ *   Mixing.  x(gamma_i) is mixed first, and the rule then reads the mixed rows with H:
+ *             RCMARL_PIPE_NONE    the n_in slots (n_rows = n_in);
+ *             RCMARL_PIPE_NNM     the n_in mixed rows of rcmarl_nnm_mix at H, bitwise (n_rows = n_in);
+ *             RCMARL_PIPE_BUCKET  the own slot, then the bucket means exactly as rcmarl_bucket_mix computes them (the
+ *                                 +inf poisoned rows included) under the attacker's sample q of the shuffle
+ *                                 (n_rows = 1 + ceil((n_in - 1) / s)).
+ *           Sample q < n_perms is the Fisher-Yates of rcmarl_bucket_mix whose draw t is word t & 3 of Philox4x32-10 with
+ *           key (seed low word, seed high word) and counter ((q << 2) | (t >> 2), attacker | receiver << 8 | net << 16 |
+ *           0x10000000, round, epoch).  Bit 28 of word 1 keeps this stream apart from rcmarl_bucket_mix's (bit 29),
+ *           rcmarl_attack's (bit 30) and the rollout's resets (bit 31).  Without bucketing there is one sample.
+ *   Rule.    family COORD: resilient_mean per coordinate over the n_rows rows (rcmarl_consensus_hidden's arithmetic);
+ *           VECTOR: exactly rcmarl_vector_aggregate's output; SPECTRAL (rule RCMARL_SPECTRAL_DNC): exactly
+ *           rcmarl_dnc_aggregate's output.  R_q(gamma_i) is the rule's output on sample q.
+ *   Objective.  O_i,q = sum_p (R_q(gamma_i)_p - mu_p)^2 as in rcmarl_tailored_attack (-inf if not finite);
+ *           Obar_i = (sum_q O_i,q, q order, an fp32 sum from 0) / (float)n_perms, -inf if some O_i,q is -inf or Obar_i
+ *           is not finite.  i* = argmax_i Obar_i, ties to the smaller i, i* = 0 if every Obar_i is -inf.
+ *   Output.  dst[0:n] = m(gamma_i*), gamma_out (optional, one float) = gamma_i*, model_out (optional, n floats) =
+ *           R_0(gamma_i*): the receiver's aggregate as the attacker models it (under bucketing, with sample 0).
+ * With mixing none and family COORD or VECTOR, dst and gamma_out are bitwise those of rcmarl_tailored_attack.  A
+ * zero-initialised mixing field is RCMARL_PIPE_NONE; s, n_perms and the Philox words are read only under bucketing.
+ * One CTA per job: the real slots, mu, d, the candidate, the output row, the mixed rows and (DnC) the fp64 mean staged
+ * in shared memory, fixed summation orders, no atomics -- bitwise reproducible, independent of the job order and of how
+ * jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, gamma_out and model_out untouched): everything rcmarl_tailored_attack
+ * refuses (family SPECTRAL with rule RCMARL_SPECTRAL_DNC excepted; its H must lie in [0, n_rows)), an unknown mixing,
+ * an H the rule refuses at n_rows, under bucketing s < 1, n_perms outside 1..RCMARL_PIPELINE_MAX_PERMS, attacker or
+ * receiver > 255 or net other than 0 or 1, a staging size (n_real + n_mixed + 4 + (DnC ? 2 : 0)) * n above
+ * RCMARL_PIPELINE_MAX_FLOATS (n_real the real slots; n_mixed = 0 without mixing, n_in under nnm and n_rows - 1 under
+ * bucketing, whose own row is read in place; the bound admits the 16-agent team-reward net, 1421 parameters, at n_in =
+ * 16 under nnm with any family), a written range (dst, gamma_out, model_out) that overlaps a real slot's row of any job
+ * of the launch, and two written ranges of the launch that overlap.  NaN inputs are not supported. */
+#define RCMARL_PIPELINE_MAX_FLOATS (37 * 1421)
+#define RCMARL_PIPELINE_MAX_PERMS 16
+typedef enum { RCMARL_PIPE_NONE = 0, RCMARL_PIPE_NNM = 1, RCMARL_PIPE_BUCKET = 2 } rcmarl_pipeline_mixing;
+typedef struct {
+    rcmarl_tailored_attack_job attack;   /* family COORD, VECTOR or SPECTRAL; slots, H and dev as for the tailored attack */
+    float* model_out;           /* optional [n]: R_0(gamma_i*) */
+    uint64_t seed;              /* Philox key (bucketing) */
+    int32_t mixing;             /* rcmarl_pipeline_mixing; 0 (a zero-initialised job) is none */
+    int32_t s;                  /* bucket size, >= 1 (bucketing) */
+    int32_t n_perms;            /* the attacker's shuffle samples, 1..RCMARL_PIPELINE_MAX_PERMS (bucketing) */
+    uint32_t attacker, receiver, net, round, epoch;   /* Philox counter words (bucketing) */
+} rcmarl_pipeline_attack_job;
+int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))
@@ -658,7 +712,9 @@ int rcmarl_comm_destroy(void* comm);
  * and get_action takes random_action = min(floor(u0 * 5), 4), the policy action = #{o : cdf_o / cdf_4 <= u1} (capped
  * at 4, cdf in fp32), and the policy action if u2 < 1 - mu, else the random one.  Word 1 keeps the streams apart: bit
  * 31 is set in every reset counter and clear in every action counter, and rcmarl_attack's word 1 (attacker | receiver
- * << 8 | 0x40000000) has bit 31 clear and bit 30 set, so while g < 2^62 no two of the three streams share a counter.
+ * << 8 | 0x40000000) has bit 31 clear and bit 30 set, rcmarl_bucket_mix's (receiver | net << 8 | 0x20000000) bits 31
+ * and 30 clear and bit 29 set, and rcmarl_pipeline_attack's (attacker | receiver << 8 | net << 16 | 0x10000000) bits
+ * 31 to 29 clear and bit 28 set, so while g < 2^60 no two of the five streams share a counter.
  * Within a stream the counters are distinct while j * NA + i < 2^32; the episode word repeats after 2^32 episodes.
  * An injected `uniforms` / `init_state` replaces the draws one for one, laid out [episode][step][env][n_active][3] and
  * [episode][env][n_active][2]. */

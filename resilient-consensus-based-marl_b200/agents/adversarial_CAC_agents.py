@@ -79,7 +79,9 @@ class Byzantine_CAC_agent(Faulty_CAC_agent):
     ("minmax_uv" | "minmax_std" | "minmax_sgn" | "minsum_uv" | "minsum_std" | "minsum_sgn", s) with s >= 0 and s = 1 the
     paper's attack, at rcmarl_adaptive_attack; or a rule-aware attack tuned against the receiver's own rule and H,
     ("tailored_uv" | "tailored_std" | "tailored_sgn", s) with the range multiplier s >= 0, at rcmarl_tailored_attack; or
-    the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
+    the same search against the receiver's whole pipeline -- its mixing step (nnm or bucketing, the latter over shuffles
+    of the attacker's own) and then its rule, DnC included -- ("pipeline_uv" | "pipeline_std" | "pipeline_sgn", s), at
+    rcmarl_pipeline_attack; or the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
     with eps >= 0, at rcmarl_dissensus_attack; or the mimic attack that copies the honest neighbour furthest along the
     honest messages' principal direction, ("mimic", T0) with T0 the number of power steps, an integer in 0 .. 2^31 - 1,
     after which the direction is frozen, at rcmarl_mimic_attack).

@@ -19,6 +19,8 @@
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
 //                   (rcmarl_adaptive_attack)
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
+//   pipeline_attack_kernel  the same search against the receiver's mixing step and rule, DnC included
+//                   (rcmarl_pipeline_attack)
 //   dissensus_attack_kernel  Byzantine messages that cancel the receiver's honest pull (rcmarl_dissensus_attack)
 //   mimic_attack_kernel  copies of the honest message furthest along the tracked principal direction
 //                   (rcmarl_mimic_attack)
@@ -589,46 +591,45 @@ __device__ __forceinline__ double warp_sum_f64(double v) {
 // (lane-strided fp64 fma partials, then the fixed xor butterfly), so its value does not depend on which warp takes it.
 // The Jacobi eigen-solve runs on warp 0, one lane per row of the m x m matrix, with every lane computing each rotation
 // identically; scores, selection and weights also run on warp 0, and the output takes one thread per coordinate.
-__global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_constant__ VectorParams P) {
+struct DncShared {
+    double A[RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];   // G, reduced in place by the Jacobi rotations
+    double V[RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];   // the accumulated rotations: column c is the eigenvector of A[c][c]
+    int ulist[RCMARL_MAX_NEIGHBOURS];                          // U in index order
+    int flagged[RCMARL_MAX_NEIGHBOURS];
+    float wt[RCMARL_MAX_NEIGHBOURS];
+    int m;
+};
+
+// The body of rcmarl_dnc_aggregate over nin messages row(0) .. row(nin - 1) of n floats in shared memory: writes the
+// aggregate to out[0:n] and leaves w_k in S.wt (the caller synchronises before reading either).  mu is a shared work
+// row of n doubles.  Called by the whole CTA of VEC_THREADS threads; Row maps a message index to its staged row.
+template <class Row>
+__device__ __forceinline__ void dnc_rule(const Row& row, int n, int nin, int H, double* mu, float* out, DncShared& S) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     constexpr int NW = VEC_THREADS / 32;
-    extern __shared__ __align__(16) float smem[];
-    __shared__ double A[MAXN * MAXN];              // G, reduced in place by the Jacobi rotations
-    __shared__ double V[MAXN * MAXN];              // the accumulated rotations: column c is the eigenvector of A[c][c]
-    __shared__ int ulist[MAXN];                    // U in index order
-    __shared__ int flagged[MAXN];
-    __shared__ float wt[MAXN];
-    __shared__ int m_s;
-    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
-    const int n = job.n, nin = job.n_in;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    double* mu = reinterpret_cast<double*>(smem);  // [n]
-    float* xs = smem + 2 * (int64_t)n;             // [n_in][n]
-    for (int k = 0; k < nin; ++k) {
-        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
-        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
-    }
-    __syncthreads();
+    double* A = S.A;
+    double* V = S.V;
     for (int k = warp; k < nin; k += NW) {
         bool inf = false;
-        for (int p = lane; p < n; p += 32) inf |= isinf(xs[k * n + p]);
+        for (int p = lane; p < n; p += 32) inf |= isinf(row.at(k, p));
         inf = __any_sync(0xffffffffu, inf);
-        if (lane == 0) flagged[k] = inf ? 1 : 0;
+        if (lane == 0) S.flagged[k] = inf ? 1 : 0;
     }
     __syncthreads();
     if (tid == 0) {
         int m = 0;
         for (int k = 0; k < nin; ++k)
-            if (!flagged[k]) ulist[m++] = k;
-        m_s = m;
+            if (!S.flagged[k]) S.ulist[m++] = k;
+        S.m = m;
     }
     __syncthreads();
-    const int m = m_s;
+    const int m = S.m;
     if (m > 0) {
         const double inv_m = 1.0 / (double)m;
         for (int p = tid; p < n; p += VEC_THREADS) {
             double s = 0.0;
-            for (int a = 0; a < m; ++a) s += (double)xs[ulist[a] * n + p];
+            for (int a = 0; a < m; ++a) s += (double)row.at(S.ulist[a], p);
             mu[p] = s * inv_m;
         }
         __syncthreads();
@@ -636,8 +637,8 @@ __global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_const
             int a = 0, r = t;
             while (r >= m - a) { r -= m - a; ++a; }
             const int b = a + r;
-            const float* xa = xs + ulist[a] * n;
-            const float* xb = xs + ulist[b] * n;
+            const float* xa = row(S.ulist[a]);
+            const float* xb = row(S.ulist[b]);
             double s = 0.0;
             for (int p = lane; p < n; p += 32) s = fma((double)xa[p] - mu[p], (double)xb[p] - mu[p], s);
             s = warp_sum_f64(s);
@@ -693,64 +694,74 @@ __global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_const
             // U position of lane k's row (k < nin), or -1 if flagged; its score
             int pos = -1;
             for (int a = 0; a < m; ++a)
-                if (ulist[a] == k) pos = a;
+                if (S.ulist[a] == k) pos = a;
             double sc = INFINITY;
             if (pos >= 0) {
                 const double u = V[pos * MAXN + top];
                 sc = lambda * (u * u);
             }
             // rows above k in the removal order: a higher score, or an equal one at a higher index (F is all +inf)
-            const int n_flag = nin - m, n_rm = max(n_flag, job.H);
+            const int n_flag = nin - m, n_rm = max(n_flag, H);
             int above = 0;
             for (int l = 0; l < nin; ++l) {
                 const double sl = __shfl_sync(0xffffffffu, sc, l);
                 if (l != k && l < nin) above += (sl > sc || (sl == sc && l > k)) ? 1 : 0;
             }
-            if (k < nin) wt[k] = above < n_rm ? 0.f : 1.f / (float)(nin - n_rm);
+            if (k < nin) S.wt[k] = above < n_rm ? 0.f : 1.f / (float)(nin - n_rm);
         }
     } else if (tid < nin) {
-        wt[tid] = tid == 0 ? 1.f : 0.f;                              // every row flagged: out = x_0
+        S.wt[tid] = tid == 0 ? 1.f : 0.f;                            // every row flagged: out = x_0
     }
     __syncthreads();
     for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = |I| (1 when every row is flagged)
         float s = 0.f, cnt = 0.f;
         for (int k = 0; k < nin; ++k)
-            if (wt[k] != 0.f) { s += xs[k * n + p]; cnt += 1.f; }
-        job.dst[p] = s / cnt;
+            if (S.wt[k] != 0.f) { s += row.at(k, p); cnt += 1.f; }
+        out[p] = s / cnt;
     }
-    if (job.weights_out && tid < nin) job.weights_out[tid] = wt[tid];
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_constant__ VectorParams P) {
+    extern __shared__ __align__(16) float smem[];
+    __shared__ DncShared S;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    double* mu = reinterpret_cast<double*>(smem);  // [n]
+    float* xs = smem + 2 * (int64_t)n;             // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    dnc_rule(StagedRows{xs, n}, n, nin, job.H, mu, job.dst, S);
+    if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
 }
 
 // Nearest-neighbour mixing (rcmarl_nnm_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The n_in
 // messages are staged in shared memory and every distance of a pair k < l is summed by ONE warp with warp_sqdist, as in
 // vector_rule, so D_kl is bitwise Krum's.  The selections N_k run on warp 0, one lane per k, with rank counts over
 // registers, and are kept as bit masks; the output takes one thread per coordinate and adds each N_k in index order.
-__global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_constant__ VectorParams P) {
+//
+// The body over nin messages row(0) .. row(nin - 1) of n floats in shared memory: writes mixed row k to dst(k)[0:n] and
+// leaves N_k in sel[k] (bit l set for l in N_k).  Shared scratch: dist [MAXN * MAXN].  Called by the whole CTA of
+// VEC_THREADS threads; the caller synchronises before reading a mixed row.
+template <class Row, class Dst>
+__device__ __forceinline__ void nnm_rows(const Row& row, int n, int nin, int H, float* dist, unsigned* sel,
+                                         const Dst& dst) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     constexpr int NW = VEC_THREADS / 32;
-    static_assert(MAXN * MAXN <= VEC_THREADS, "one thread per entry of M");
-    extern __shared__ __align__(16) float smem[];
-    __shared__ float dist[MAXN * MAXN];
-    __shared__ unsigned sel[MAXN];                 // N_k: bit l set for l in N_k
-    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
-    const int n = job.n, nin = job.n_in;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    float* xs = smem;                              // [n_in][n]
-    for (int k = 0; k < nin; ++k) {
-        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
-        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
-    }
-    __syncthreads();
     for (int t = warp; t < nin * (nin - 1) / 2; t += NW) {           // unordered pairs k < l
         int k = 0, r = t;
         while (r >= nin - 1 - k) { r -= nin - 1 - k; ++k; }
         const int l = k + 1 + r;
-        const float d = warp_sqdist(xs + k * n, xs + l * n, n, lane);
+        const float d = warp_sqdist(row(k), row(l), n, lane);
         if (lane == 0) { dist[k * MAXN + l] = d; dist[l * MAXN + k] = d; }
     }
     __syncthreads();
     if (warp == 0 && lane < nin) {
-        const int k = lane, m = nin - job.H;
+        const int k = lane, m = nin - H;
         float v[MAXN];
 #pragma unroll
         for (int l = 0; l < MAXN; ++l) v[l] = (l < nin && l != k) ? dist[k * MAXN + l] : 0.f;
@@ -769,14 +780,33 @@ __global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_const
     for (int k = 0; k < nin; ++k) {
         const unsigned mask = sel[k];
         const float cnt = (float)__popc(mask);
-        float* dst = job.dst + (int64_t)k * job.msg_stride;
+        float* out = dst(k);
         for (int p = tid; p < n; p += VEC_THREADS) {
             float s = 0.f;
             for (int l = 0; l < nin; ++l)
-                if ((mask >> l) & 1u) s += xs[l * n + p];
-            dst[p] = s / cnt;
+                if ((mask >> l) & 1u) s += row.at(l, p);
+            out[p] = s / cnt;
         }
     }
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    static_assert(MAXN * MAXN <= VEC_THREADS, "one thread per entry of M");
+    extern __shared__ __align__(16) float smem[];
+    __shared__ float dist[MAXN * MAXN];
+    __shared__ unsigned sel[MAXN];                 // N_k: bit l set for l in N_k
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    float* xs = smem;                              // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    nnm_rows(StagedRows{xs, n}, n, nin, job.H, dist, sel,
+             [&](int k) { return job.dst + (int64_t)k * job.msg_stride; });
     if (job.weights_out && tid < nin * nin) {
         const unsigned mask = sel[tid / nin];
         job.weights_out[tid] = ((mask >> (tid % nin)) & 1u) ? 1.f / (float)__popc(mask) : 0.f;
@@ -786,63 +816,78 @@ __global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_const
 // Randomized bucketing (rcmarl_bucket_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  Thread 0 draws
 // the permutation into shared memory and keeps each bucket as a bit mask over the slots; the rows take one thread per
 // coordinate and add each bucket's members in slot order straight from global memory (every received row is read
-// once).  A bucket with a non-finite mean coordinate raises its flag, and after the barrier its row is rewritten as +inf.
+// once).  A bucket with a non-finite mean coordinate is found by a block-wide vote, and its row is rewritten as +inf.
 struct BucketParams { rcmarl_bucket_job jobs[RCMARL_MAX_JOBS]; };
+
+// The received messages of a bucketing job, read from global memory: message k at msgs + in_nodes[k] * stride.
+struct GlobalRows {
+    const float* msgs;
+    const int32_t* in_nodes;
+    int64_t stride;
+    __device__ __forceinline__ float at(int k, int p) const { return __ldg(msgs + (int64_t)in_nodes[k] * stride + p); }
+};
+
+// The buckets of one shuffle (one thread): pi[0:m] = the received slots 1 .. m by Fisher-Yates, i = m-1 down to 1, draw
+// t = word t & 3 of Philox4x32-10 at counter (ctr.x | t >> 2, ctr.y, ctr.z, ctr.w); members[b] = bit l for each slot l
+// of bucket b (pi[b*s .. (b+1)*s - 1]).  pi is shared scratch of m ints.
+__device__ __forceinline__ void bucket_draw(uint4 ctr, uint2 key, int m, int s, int* pi, unsigned* members) {
+    const int nb = m == 0 ? 0 : (m - 1) / s + 1;   // ceil(m / s) without overflow at a huge s
+    for (int q = 0; q < m; ++q) pi[q] = q + 1;
+    uint4 r = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = m - 1, t = 0; i >= 1; --i, ++t) {
+        if ((t & 3) == 0) r = philox4x32_10(make_uint4(ctr.x | (uint32_t)(t >> 2), ctr.y, ctr.z, ctr.w), key);
+        const uint32_t u = (t & 3) == 0 ? r.x : (t & 3) == 1 ? r.y : (t & 3) == 2 ? r.z : r.w;
+        const int j = (int)(((uint64_t)u * (uint64_t)(i + 1)) >> 32);
+        const int a = pi[i];
+        pi[i] = pi[j];
+        pi[j] = a;
+    }
+    for (int b = 0; b < nb; ++b) members[b] = 0u;
+    for (int q = 0; q < m; ++q) members[q / s] |= 1u << pi[q];
+}
+
+// The bucket means of rcmarl_bucket_mix over the slots row.at(l, p), l = 1 .. nin - 1: bucket b's mean to dst(b)[0:n],
+// or +inf throughout if a coordinate of it is not finite.  Called by the whole CTA of VEC_THREADS threads; each thread
+// writes its own coordinates only, and the caller synchronises before reading another's.
+template <class Row, class Dst>
+__device__ __forceinline__ void bucket_means(const Row& row, int n, int nin, int nb, const unsigned* members,
+                                             const Dst& dst) {
+    const int tid = threadIdx.x;
+    for (int b = 0; b < nb; ++b) {
+        const unsigned mask = members[b];
+        const float cnt = (float)__popc(mask);
+        float* out = dst(b);
+        bool bad = false;
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            float s = 0.f;
+            for (int l = 1; l < nin; ++l)
+                if ((mask >> l) & 1u) s += row.at(l, p);
+            const float v = s / cnt;
+            bad |= !isfinite(v);
+            out[p] = v;
+        }
+        if (__syncthreads_or(bad))
+            for (int p = tid; p < n; p += VEC_THREADS) out[p] = INFINITY;
+    }
+}
 
 __global__ void __launch_bounds__(VEC_THREADS) bucket_mix_kernel(const __grid_constant__ BucketParams P) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     static_assert(MAXN * MAXN <= VEC_THREADS, "one thread per entry of M");
     __shared__ int pi[MAXN];
     __shared__ unsigned members[MAXN];             // bucket b: bit l set for slot l in the bucket
-    __shared__ int poisoned[MAXN];                 // bucket b's mean has a coordinate that is not finite
     const rcmarl_bucket_job& job = P.jobs[blockIdx.x];
     const int n = job.n, nin = job.n_in, m = nin - 1;
-    const int nb = m == 0 ? 0 : (m - 1) / job.s + 1;   // ceil(m / s) without overflow at a huge s
+    const int nb = m == 0 ? 0 : (m - 1) / job.s + 1;
     const int tid = threadIdx.x;
-    if (tid == 0) {
-        for (int q = 0; q < m; ++q) pi[q] = q + 1;
-        const uint2 key = make_uint2((uint32_t)job.seed, (uint32_t)(job.seed >> 32));
-        uint4 r = make_uint4(0u, 0u, 0u, 0u);
-        for (int i = m - 1, t = 0; i >= 1; --i, ++t) {
-            if ((t & 3) == 0)
-                r = philox4x32_10(make_uint4((uint32_t)(t >> 2), job.receiver | job.net << 8 | 0x20000000u, job.round,
-                                             job.epoch), key);
-            const uint32_t u = (t & 3) == 0 ? r.x : (t & 3) == 1 ? r.y : (t & 3) == 2 ? r.z : r.w;
-            const int j = (int)(((uint64_t)u * (uint64_t)(i + 1)) >> 32);
-            const int a = pi[i];
-            pi[i] = pi[j];
-            pi[j] = a;
-        }
-        for (int b = 0; b < nb; ++b) {
-            members[b] = 0u;
-            poisoned[b] = 0;
-        }
-        for (int q = 0; q < m; ++q) members[q / job.s] |= 1u << pi[q];
-    }
+    if (tid == 0)
+        bucket_draw(make_uint4(0u, job.receiver | job.net << 8 | 0x20000000u, job.round, job.epoch),
+                    make_uint2((uint32_t)job.seed, (uint32_t)(job.seed >> 32)), m, job.s, pi, members);
     __syncthreads();
     const float* own = job.msgs + (int64_t)job.in_nodes[0] * job.msg_stride;
     for (int p = tid; p < n; p += VEC_THREADS) job.dst[p] = __ldg(own + p);
-    for (int b = 0; b < nb; ++b) {
-        const unsigned mask = members[b];
-        const float cnt = (float)__popc(mask);
-        float* dst = job.dst + (int64_t)(1 + b) * job.msg_stride;
-        bool bad = false;
-        for (int p = tid; p < n; p += VEC_THREADS) {
-            float s = 0.f;
-            for (int l = 1; l < nin; ++l)
-                if ((mask >> l) & 1u) s += __ldg(job.msgs + (int64_t)job.in_nodes[l] * job.msg_stride + p);
-            const float v = s / cnt;
-            bad |= !isfinite(v);
-            dst[p] = v;
-        }
-        if (bad) poisoned[b] = 1;                  // every writer stores the same value
-    }
-    __syncthreads();
-    for (int b = 0; b < nb; ++b) {
-        if (!poisoned[b]) continue;
-        float* dst = job.dst + (int64_t)(1 + b) * job.msg_stride;
-        for (int p = tid; p < n; p += VEC_THREADS) dst[p] = INFINITY;
-    }
+    bucket_means(GlobalRows{job.msgs, job.in_nodes, job.msg_stride}, n, nin, nb, members,
+                 [&](int b) { return job.dst + (int64_t)(1 + b) * job.msg_stride; });
     if (job.weights_out && tid < (1 + nb) * nin) {
         const int r = tid / nin, l = tid % nin;
         float w = r == 0 && l == 0 ? 1.f : 0.f;
@@ -1008,17 +1053,97 @@ struct SlotRows {
     __device__ __forceinline__ float at(int k, int p) const { return xs[off[k] + p]; }
 };
 
+// Shared scratch of the tailored and pipeline searches (see adaptive_gamma and vector_rule for dist .. total).
+struct TailoredShared {
+    float dist[RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];
+    float ek[RCMARL_MAX_NEIGHBOURS], bk[RCMARL_MAX_NEIGHBOURS], wt[RCMARL_MAX_NEIGHBOURS], score[RCMARL_MAX_NEIGHBOURS];
+    float scal[2], total, best_o;
+    int off[RCMARL_MAX_NEIGHBOURS], best_i;         // slot k at xs + off[k]; the search's best objective and index
+};
+
+// The coordinate-wise rule over nrows rows: z[p] = resilient_mean_small of row(0 .. nrows - 1) at p, own = row 0.
+template <class Row>
+__device__ __forceinline__ void coord_rule(const Row& row, int n, int nrows, int H, int rule, float* z) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    for (int p = threadIdx.x; p < n; p += ADA_THREADS) {
+        float v[MAXN];
+#pragma unroll
+        for (int k = 0; k < MAXN; ++k) v[k] = k < nrows ? row.at(k, p) : 0.f;
+        z[p] = resilient_mean_small<MAXN>(v, nrows, H, rule);
+    }
+}
+
+// Stage a tailored job's real slots at xs (the honest ones first), point every crafted slot at cand (S.off), and
+// compute mu, d and Gamma = scale * gamma_mm, 0 if that fp32 product is not finite (a huge scale: dst = mu).  Called
+// by the whole CTA; returns Gamma in every thread.
+__device__ __forceinline__ float tailored_setup(const rcmarl_tailored_attack_job& job, int nh, float* xs, float* mu,
+                                                float* d, const float* cand, TailoredShared& S) {
+    const int n = job.n, nin = job.n_in, tid = threadIdx.x;
+    if (tid == 0) {
+        int h = 0, o = nh;
+        for (int k = 0; k < nin; ++k)
+            S.off[k] = job.slots[k] < 0 ? (int)(cand - xs) : ((job.honest_mask >> k) & 1u ? h++ : o++) * n;
+        S.best_o = -INFINITY;
+        S.best_i = 0;
+    }
+    __syncthreads();
+    for (int k = 0; k < nin; ++k) {
+        if (job.slots[k] < 0) continue;
+        const float* src = job.msgs + (int64_t)job.slots[k] * job.msg_stride;
+        float* row = xs + S.off[k];
+        for (int p = tid; p < n; p += ADA_THREADS) row[p] = __ldg(src + p);
+    }
+    __syncthreads();
+    constexpr int kind = RCMARL_ADAPT_MINMAX;
+    adaptive_gamma(xs, nh, n, kind, job.dev, mu, d, S.dist, S.ek, S.bk, S.scal, [&](float g) { S.scal[1] = g; });
+    __syncthreads();
+    const float prod = job.scale * S.scal[1];
+    return isfinite(prod) ? prod : 0.f;
+}
+
+// The candidate search: for i = 0 .. K, cand = m(gamma_i), then for each sample q < nq eval(q) writes the modelled
+// aggregate R_q(gamma_i) to z[0:n] and warp 0 sums O_i,q; Obar_i = (sum_q O_i,q in q order, from 0) / nq, -inf once an
+// O_i,q or Obar_i is not finite (at nq = 1, Obar_i = O_i bitwise).  Called by the whole CTA after tailored_setup;
+// returns i* (ties to the smaller i) in every thread.
+template <class Eval>
+__device__ __forceinline__ int tailored_search(const float* mu, const float* d, float* cand, const float* z, int n,
+                                               float range, int nq, TailoredShared& S, const Eval& eval) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (int i = 0; i <= RCMARL_TAILORED_STEPS; ++i) {
+        const float g = range * (float)i / (float)RCMARL_TAILORED_STEPS;
+        for (int p = tid; p < n; p += ADA_THREADS) cand[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
+        float acc = 0.f;                                              // warp 0: sum_q O_i,q
+        for (int q = 0; q < nq; ++q) {
+            __syncthreads();                                          // x(gamma_i) complete; the last objective read
+            eval(q);
+            __syncthreads();                                          // R_q(x(gamma_i)) complete
+            if (warp == 0) {                                          // O_i,q = sum_p (R_p - mu_p)^2, one warp
+                float s = 0.f;
+                for (int p = lane; p < n; p += 32) {
+                    const float e = z[p] - mu[p];
+                    s = fmaf(e, e, s);
+                }
+                s = warp_sum(s);
+                acc = isfinite(s) ? acc + s : -INFINITY;              // not finite: -inf, and -inf stays
+            }
+        }
+        const float o = acc / (float)nq;
+        if (tid == 0 && isfinite(o) && o > S.best_o) {                // ties to the smaller i
+            S.best_o = o;
+            S.best_i = i;
+        }
+    }
+    __syncthreads();
+    return S.best_i;
+}
+
 // (at most one CTA per job and 117 KB of staging per CTA: the register budget of one CTA per SM keeps it free of spills)
 __global__ void __launch_bounds__(ADA_THREADS, 1) tailored_attack_kernel(const __grid_constant__ TailoredParams P) {
-    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     extern __shared__ __align__(16) float smem[];
-    __shared__ float dist[MAXN * MAXN];
-    __shared__ float ek[MAXN], bk[MAXN], wt[MAXN], score[MAXN];
-    __shared__ float scal[2], total, best_o;
-    __shared__ int off[MAXN], best_i;
+    __shared__ TailoredShared S;
     const rcmarl_tailored_attack_job& job = P.jobs[blockIdx.x];
     const int n = job.n, nin = job.n_in;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     int nh = 0, nr = 0;                            // honest slots, real slots
     for (int k = 0; k < nin; ++k) {
         nh += (job.honest_mask >> k) & 1u;
@@ -1029,59 +1154,98 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) tailored_attack_kernel(const _
     float* d = mu + n;                             // [n]
     float* cand = d + n;                           // [n]: m(gamma_i), every crafted slot
     float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
-    if (tid == 0) {
-        int h = 0, o = nh;
-        for (int k = 0; k < nin; ++k)
-            off[k] = job.slots[k] < 0 ? (int)(cand - xs) : ((job.honest_mask >> k) & 1u ? h++ : o++) * n;
-        best_o = -INFINITY;
-        best_i = 0;
-    }
-    __syncthreads();
-    for (int k = 0; k < nin; ++k) {
-        if (job.slots[k] < 0) continue;
-        const float* src = job.msgs + (int64_t)job.slots[k] * job.msg_stride;
-        float* row = xs + off[k];
-        for (int p = tid; p < n; p += ADA_THREADS) row[p] = __ldg(src + p);
-    }
-    __syncthreads();
-    constexpr int kind = RCMARL_ADAPT_MINMAX;
-    adaptive_gamma(xs, nh, n, kind, job.dev, mu, d, dist, ek, bk, scal, [&](float g) { scal[1] = g; });
-    __syncthreads();
-    const float prod = job.scale * scal[1];
-    const float range = isfinite(prod) ? prod : 0.f;   // Gamma = s * gamma_mm; 0 if that overflows (dst = mu)
-    const SlotRows rows{xs, off};
-    for (int i = 0; i <= RCMARL_TAILORED_STEPS; ++i) {
-        const float g = range * (float)i / (float)RCMARL_TAILORED_STEPS;
-        for (int p = tid; p < n; p += ADA_THREADS) cand[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
-        __syncthreads();                                              // x(gamma_i) complete; the last objective read
-        if (job.family == RCMARL_TAILOR_COORD) {
-            for (int p = tid; p < n; p += ADA_THREADS) {
-                float v[MAXN];
-#pragma unroll
-                for (int k = 0; k < MAXN; ++k) v[k] = k < nin ? rows.at(k, p) : 0.f;
-                z[p] = resilient_mean_small<MAXN>(v, nin, job.H, job.rule);
-            }
-        } else {
-            vector_rule(rows, n, nin, job.H, job.rule, z, z, dist, wt, score, total);
-        }
-        __syncthreads();                                              // R_j(x(gamma_i)) complete
-        if (warp == 0) {                                              // O_i = sum_p (R_p - mu_p)^2, one warp
-            float s = 0.f;
-            for (int p = lane; p < n; p += 32) {
-                const float e = z[p] - mu[p];
-                s = fmaf(e, e, s);
-            }
-            s = warp_sum(s);
-            if (lane == 0 && isfinite(s) && s > best_o) {             // ties to the smaller i; not finite: -inf
-                best_o = s;
-                best_i = i;
-            }
-        }
-    }
-    __syncthreads();
-    const float g = range * (float)best_i / (float)RCMARL_TAILORED_STEPS;
+    const float range = tailored_setup(job, nh, xs, mu, d, cand, S);
+    const SlotRows rows{xs, S.off};
+    const int best = tailored_search(mu, d, cand, z, n, range, 1, S, [&](int) {
+        if (job.family == RCMARL_TAILOR_COORD)
+            coord_rule(rows, n, nin, job.H, job.rule, z);
+        else
+            vector_rule(rows, n, nin, job.H, job.rule, z, z, S.dist, S.wt, S.score, S.total);
+    });
+    const float g = range * (float)best / (float)RCMARL_TAILORED_STEPS;
     if (tid == 0 && job.gamma_out) *job.gamma_out = g;
     for (int p = tid; p < n; p += ADA_THREADS) job.dst[p] = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
+}
+
+// Pipeline-aware Byzantine messages (rcmarl_pipeline_attack, include/rcmarl.h): tailored_attack_kernel's staging and
+// search, with the receiver's mixing step before its rule.  Behind the real slots, mu, d, the candidate and the output
+// row come the mixed rows (nnm: n_in; bucketing: the bucket means, the own row being read in place), and for DnC the
+// fp64 mean sits in front, 8-byte aligned.  The mixing and the rule read their rows through slot offsets, so one
+// instantiation of each body serves every mixing.  The attacker's bucketing shuffles are drawn once per job by thread 0.
+struct PipelineParams { rcmarl_pipeline_attack_job jobs[RCMARL_MAX_JOBS]; };
+static_assert(ADA_THREADS == VEC_THREADS, "dnc_rule, nnm_rows, bucket_means and vector_rule stride by VEC_THREADS");
+
+__global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const __grid_constant__ PipelineParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ TailoredShared S;
+    __shared__ DncShared D;
+    __shared__ unsigned sel[MAXN];                                   // nnm: N_k
+    __shared__ unsigned members[RCMARL_PIPELINE_MAX_PERMS * MAXN];   // bucketing: bucket b of sample q at [q * MAXN + b]
+    __shared__ int pi[MAXN];
+    __shared__ int roff[MAXN];                                       // the rule's row k at xs + roff[k]
+    const rcmarl_pipeline_attack_job& pj = P.jobs[blockIdx.x];
+    const rcmarl_tailored_attack_job& job = pj.attack;
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    const bool bucket = pj.mixing == RCMARL_PIPE_BUCKET;
+    const int nb = bucket ? (nin - 2) / pj.s + 1 : 0;                // ceil((n_in - 1) / s); n_in >= 2
+    const int nrows = bucket ? 1 + nb : nin, nq = bucket ? pj.n_perms : 1;
+    int nh = 0, nr = 0;                            // honest slots, real slots
+    for (int k = 0; k < nin; ++k) {
+        nh += (job.honest_mask >> k) & 1u;
+        nr += job.slots[k] >= 0 ? 1 : 0;
+    }
+    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC: [n]
+    float* xs = smem + (job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
+    float* mu = xs + (int64_t)nr * n;              // [n]
+    float* d = mu + n;                             // [n]
+    float* cand = d + n;                           // [n]: m(gamma_i), every crafted slot
+    float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
+    float* mixed = z + n;                          // nnm: [n_in][n]; bucketing: [nb][n]
+    if (tid == 0 && bucket)
+        for (int q = 0; q < nq; ++q)
+            bucket_draw(make_uint4((uint32_t)q << 2, pj.attacker | pj.receiver << 8 | pj.net << 16 | 0x10000000u,
+                                   pj.round, pj.epoch),
+                        make_uint2((uint32_t)pj.seed, (uint32_t)(pj.seed >> 32)), nin - 1, pj.s, pi, members + q * MAXN);
+    const float range = tailored_setup(job, nh, xs, mu, d, cand, S);
+    if (tid == 0) {
+        const int base = (int)(mixed - xs);
+        for (int k = 0; k < nrows; ++k)
+            roff[k] = pj.mixing == RCMARL_PIPE_NONE ? S.off[k] : pj.mixing == RCMARL_PIPE_NNM ? base + k * n
+                    : k == 0 ? S.off[0] : base + (k - 1) * n;
+    }
+    __syncthreads();
+    const SlotRows slots{xs, S.off}, rows{xs, roff};
+    const auto eval = [&](int q) {
+        if (pj.mixing == RCMARL_PIPE_NNM) {
+            nnm_rows(slots, n, nin, job.H, S.dist, sel, [&](int k) { return mixed + k * n; });
+            __syncthreads();                                          // the mixed rows complete
+        } else if (bucket) {
+            bucket_means(slots, n, nin, nb, members + q * MAXN, [&](int b) { return mixed + b * n; });
+            __syncthreads();
+        }
+        if (job.family == RCMARL_TAILOR_COORD)
+            coord_rule(rows, n, nrows, job.H, job.rule, z);
+        else if (job.family == RCMARL_TAILOR_VECTOR)
+            vector_rule(rows, n, nrows, job.H, job.rule, z, z, S.dist, S.wt, S.score, S.total);
+        else
+            dnc_rule(rows, n, nrows, job.H, mu64, z, D);
+    };
+    const int best = tailored_search(mu, d, cand, z, n, range, nq, S, eval);
+    const float g = range * (float)best / (float)RCMARL_TAILORED_STEPS;
+    if (tid == 0 && job.gamma_out) *job.gamma_out = g;
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        const float v = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
+        job.dst[p] = v;
+        cand[p] = v;
+    }
+    if (pj.model_out) {                            // R_0(gamma_i*), the same for every thread of the CTA
+        __syncthreads();
+        eval(0);
+        __syncthreads();
+        for (int p = tid; p < n; p += ADA_THREADS) pj.model_out[p] = z[p];
+    }
 }
 
 // Dissensus messages (rcmarl_dissensus_attack, include/rcmarl.h): one thread per coordinate, as attack_kernel; the
@@ -1949,13 +2113,45 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs, int n_jobs, v
     return RCMARL_OK;
 }
 
-// the receiver model of a tailored job: a known family and rule, and an H that rule allows for n_in messages (the
-// checks of rcmarl_consensus_hidden and rcmarl_vector_aggregate)
-static bool bad_tailored_rule(const rcmarl_tailored_attack_job& q) {
-    if (q.H < 0 || q.H >= q.n_in) return true;
-    if (q.family == RCMARL_TAILOR_COORD) return bad_rule(q.rule, q.H, q.n_in);
-    if (q.family != RCMARL_TAILOR_VECTOR || q.rule < RCMARL_VEC_KRUM || q.rule > RCMARL_VEC_GMED) return true;
-    return (q.rule == RCMARL_VEC_KRUM || q.rule == RCMARL_VEC_MKRUM) && q.n_in < q.H + 3;
+// the receiver's rule of a tailored or pipeline job: a known family and rule, and an H that rule allows for n_rows
+// messages (the checks of rcmarl_consensus_hidden, rcmarl_vector_aggregate and rcmarl_dnc_aggregate)
+static bool bad_receiver_rule(int family, int rule, int H, int n_rows) {
+    if (H < 0 || H >= n_rows) return true;
+    if (family == RCMARL_TAILOR_COORD) return bad_rule(rule, H, n_rows);
+    if (family == RCMARL_TAILOR_SPECTRAL) return rule != RCMARL_SPECTRAL_DNC;
+    if (family != RCMARL_TAILOR_VECTOR || rule < RCMARL_VEC_KRUM || rule > RCMARL_VEC_GMED) return true;
+    return (rule == RCMARL_VEC_KRUM || rule == RCMARL_VEC_MKRUM) && n_rows < H + 3;
+}
+
+// the slot list, direction and scale of a tailored job (everything but its rule); n_real receives its real slots
+static bool bad_tailored_slots(const rcmarl_tailored_attack_job& q, int& n_real) {
+    if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return true;
+    if (q.honest_mask >> q.n_in) return true;                        // a bit past the slot list
+    n_real = 0;
+    for (int k = 0; k < q.n_in; ++k) {
+        if (q.slots[k] < -1) return true;
+        if (q.slots[k] == -1 && ((q.honest_mask >> k) & 1u)) return true;   // a crafted slot marked honest
+        n_real += q.slots[k] >= 0 ? 1 : 0;
+    }
+    if (n_real == q.n_in || q.honest_mask == 0u) return true;        // no crafted slot, no honest slot
+    if (q.dev < RCMARL_DEV_UV || q.dev > RCMARL_DEV_SGN) return true;
+    return !std::isfinite(q.scale) || q.scale < 0.f;
+}
+
+// the written ranges (dst, gamma_out) and the read ranges (the real slots' rows) of a tailored job
+static void tailored_ranges(const rcmarl_tailored_attack_job& q, uintptr_t* w0, uintptr_t* w1, int& n_w, uintptr_t* r0,
+                            uintptr_t* r1, int& n_r) {
+    float_range(q.dst, 0, 0, q.n, w0[n_w], w1[n_w]);
+    ++n_w;
+    if (q.gamma_out) {
+        float_range(q.gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
+        ++n_w;
+    }
+    for (int k = 0; k < q.n_in; ++k)
+        if (q.slots[k] >= 0) {
+            float_range(q.msgs, q.slots[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+            ++n_r;
+        }
 }
 
 int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, void* stream) {
@@ -1964,19 +2160,9 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_tailored_attack_job& q = jobs[j];
-        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        if (q.honest_mask >> q.n_in) return RCMARL_ERR_ARG;            // a bit past the slot list
-        int n_crafted = 0;
-        for (int k = 0; k < q.n_in; ++k) {
-            if (q.slots[k] < -1) return RCMARL_ERR_ARG;
-            if (q.slots[k] == -1) {
-                if ((q.honest_mask >> k) & 1u) return RCMARL_ERR_ARG;  // a crafted slot marked honest
-                ++n_crafted;
-            }
-        }
-        if (n_crafted == 0 || q.honest_mask == 0u) return RCMARL_ERR_ARG;
-        if (bad_tailored_rule(q) || q.dev < RCMARL_DEV_UV || q.dev > RCMARL_DEV_SGN) return RCMARL_ERR_ARG;
-        if (!std::isfinite(q.scale) || q.scale < 0.f) return RCMARL_ERR_ARG;
+        int n_real = 0;
+        if (bad_tailored_slots(q, n_real)) return RCMARL_ERR_ARG;
+        if (q.family == RCMARL_TAILOR_SPECTRAL || bad_receiver_rule(q.family, q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)(q.n_in + 3) * q.n;
         if (floats > RCMARL_TAILORED_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
@@ -1987,19 +2173,7 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
     uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
         r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
     int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (jobs[j].gamma_out) {
-            float_range(jobs[j].gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < jobs[j].n_in; ++k)
-            if (jobs[j].slots[k] >= 0) {
-                float_range(jobs[j].msgs, jobs[j].slots[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
-                ++n_r;
-            }
-    }
+    for (int j = 0; j < n_jobs; ++j) tailored_ranges(jobs[j], w0, w1, n_w, r0, r1, n_r);
     if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
     // the staging bound is above the default 48 KB of dynamic shared memory
     static bool opted[64] = {};
@@ -2007,6 +2181,53 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
         return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     tailored_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    PipelineParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_pipeline_attack_job& pj = jobs[j];
+        const rcmarl_tailored_attack_job& q = pj.attack;
+        int n_real = 0;
+        if (bad_tailored_slots(q, n_real)) return RCMARL_ERR_ARG;
+        int n_rows = q.n_in, n_mixed = 0;
+        if (pj.mixing == RCMARL_PIPE_NNM) {
+            n_mixed = q.n_in;
+        } else if (pj.mixing == RCMARL_PIPE_BUCKET) {
+            if (pj.s < 1 || pj.n_perms < 1 || pj.n_perms > RCMARL_PIPELINE_MAX_PERMS) return RCMARL_ERR_ARG;
+            if (pj.attacker > 255u || pj.receiver > 255u || pj.net > 1u) return RCMARL_ERR_ARG;
+            n_rows = 1 + (q.n_in - 2) / pj.s + 1;                    // n_in >= 2: a crafted and an honest slot
+            n_mixed = n_rows - 1;
+        } else if (pj.mixing != RCMARL_PIPE_NONE) {
+            return RCMARL_ERR_ARG;
+        }
+        if (bad_receiver_rule(q.family, q.rule, q.H, n_rows)) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(n_real + n_mixed + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        if (floats > RCMARL_PIPELINE_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = pj;
+    }
+    // as rcmarl_tailored_attack, with model_out among the written ranges
+    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        tailored_ranges(jobs[j].attack, w0, w1, n_w, r0, r1, n_r);
+        if (jobs[j].model_out) {
+            float_range(jobs[j].model_out, 0, 0, jobs[j].attack.n, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)pipeline_attack_kernel, (int)(sizeof(float) * RCMARL_PIPELINE_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    pipeline_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

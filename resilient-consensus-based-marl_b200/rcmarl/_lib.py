@@ -38,7 +38,7 @@ DEV_UV, DEV_STD, DEV_SGN = 0, 1, 2                # rcmarl_adaptive_dev
 ADAPTIVE_ATTACKS = {f"{k}_{d}": (kind, dev) for k, kind in (("minmax", ADAPT_MINMAX), ("minsum", ADAPT_MINSUM))
                     for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
 ADAPTIVE_MAX_FLOATS = 18 * 1536
-TAILOR_COORD, TAILOR_VECTOR = 0, 1                # rcmarl_tailored_family
+TAILOR_COORD, TAILOR_VECTOR, TAILOR_SPECTRAL = 0, 1, 2   # rcmarl_tailored_family
 # rule-aware attacks (rcmarl_tailored_attack): candidate steps K and the staging bound; the names are TAILORED_ATTACKS
 TAILORED_STEPS = 32
 TAILORED_MAX_FLOATS = 19 * 1536
@@ -52,6 +52,12 @@ NNM_MAX_FLOATS = 48 * 1024
 MIX_BUCKET = 1                                    # rcmarl_mixing_rule: randomized bucketing, ("bucket", s)
 BUCKET_DEFAULT_S = 2                              # the bucket size of a plain "bucket" entry
 BUCKET_MAX_S = 2 ** 31 - 1
+# pipeline-aware attacks (rcmarl_pipeline_attack): rcmarl_pipeline_mixing, the staging bound, the most shuffle samples
+# and the samples the trainer draws; the names are PIPELINE_ATTACKS
+PIPE_NONE, PIPE_NNM, PIPE_BUCKET = 0, 1, 2
+PIPELINE_MAX_FLOATS = 37 * 1421
+PIPELINE_MAX_PERMS = 16
+PIPELINE_PERMS = 4
 MIMIC_MAX_FLOATS = 19 * 1536                      # rcmarl_mimic_attack's staging bound
 MIMIC_MAX_T0 = 2 ** 31 - 1                        # the mimic attack's power steps T0: an integer in 0 .. 2^31 - 1
 
@@ -89,6 +95,12 @@ class TailoredAttackJob(C.Structure):
     _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("gamma_out", c_fp), ("n", C.c_int32),
                 ("n_in", C.c_int32), ("slots", C.c_int32 * MAX_NEIGHBOURS), ("honest_mask", C.c_uint32),
                 ("family", C.c_int32), ("rule", C.c_int32), ("H", C.c_int32), ("dev", C.c_int32), ("scale", C.c_float)]
+
+
+class PipelineAttackJob(C.Structure):
+    _fields_ = [("attack", TailoredAttackJob), ("model_out", c_fp), ("seed", C.c_uint64), ("mixing", C.c_int32),
+                ("s", C.c_int32), ("n_perms", C.c_int32), ("attacker", C.c_uint32), ("receiver", C.c_uint32),
+                ("net", C.c_uint32), ("round", C.c_uint32), ("epoch", C.c_uint32)]
 
 
 class DissensusJob(C.Structure):
@@ -168,6 +180,7 @@ SYMBOLS = [
     ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
+    ("rcmarl_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, c_fp]),
     ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
     ("rcmarl_mimic_attack", C.c_int, [C.POINTER(MimicJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -341,6 +354,23 @@ def is_tailored_attack(name):
     return isinstance(name, str) and name in TAILORED_ATTACKS
 
 
+class PipelineKind(int):
+    """The kind check_attack gives a pipeline-aware attack (rcmarl_pipeline_attack): its rcmarl_adaptive_dev, as a type
+    of its own so that it is told apart from the tailored attacks, which model the receiver's rule only."""
+
+    def __repr__(self):
+        return f"PipelineKind({int(self)})"
+
+
+PIPELINE_ATTACKS = {f"pipeline_{d}": PipelineKind(dev) for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+
+
+def is_pipeline_attack(name):
+    """True for the name of a pipeline-aware attack (rcmarl_pipeline_attack): "pipeline_uv", "pipeline_std",
+    "pipeline_sgn"."""
+    return isinstance(name, str) and name in PIPELINE_ATTACKS
+
+
 class DissensusKind(int):
     """The kind check_attack gives the dissensus attack (rcmarl_dissensus_attack), a type of its own so that it is told
     apart from the other attacks' kinds; its parameter is eps >= 0."""
@@ -362,27 +392,29 @@ STATE_ATTACKS = {"dissensus": DissensusKind(0), "mimic": MimicKind(0)}
 
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss", the adaptive and the tailored attacks and "dissensus" also >= 0; for "mimic" an integer in
-    0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack / rcmarl_dissensus_attack /
-    rcmarl_mimic_attack require (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
+    "gauss", the adaptive, the tailored and the pipeline attacks and "dissensus" also >= 0; for "mimic" an integer in
+    0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack / rcmarl_pipeline_attack /
+    rcmarl_dissensus_attack / rcmarl_mimic_attack require (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
     the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the
-    paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, whose parameter is the range
-    multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
+    paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack and the PipelineKind of a pipeline
+    attack, whose parameter is the range multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
     and MimicKind for "mimic", whose parameter is T0 (the power steps each pair takes before its direction freezes)."""
     try:
         name, param = attack
         param = float(param)
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
-    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **STATE_ATTACKS}
+    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **PIPELINE_ATTACKS, **STATE_ATTACKS}
     if not isinstance(name, str) or name not in known:
-        raise RcmarlError(f"unknown attack {name!r}: expected one of "
-                          f"{sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(STATE_ATTACKS)}")
+        names = sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(PIPELINE_ATTACKS) \
+            + sorted(STATE_ATTACKS)
+        raise RcmarlError(f"unknown attack {name!r}: expected one of {names}")
     if name == "mimic":
         if not (math.isfinite(param) and param == int(param) and 0 <= param <= MIMIC_MAX_T0):
             raise RcmarlError(f"attack 'mimic' needs an integer T0 in 0 .. {MIMIC_MAX_T0}, got {param}")
         return known[name], param
-    nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS
+    nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS \
+        or name in PIPELINE_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
     return known[name], param

@@ -355,6 +355,37 @@ def tailored_attack(jobs):
     L.check(L.lib().rcmarl_tailored_attack(a, len(a), _stream()), "rcmarl_tailored_attack")
 
 
+def pipeline_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack, scale, mixing=None, n_perms=1, seed=0,
+                        attacker=0, receiver=0, net=0, round=0, epoch=0, gamma_out=None, model_out=None):
+    """rcmarl_pipeline_attack_job: slots, honest, H and scale as tailored_attack_job; rule: the receiver's rule name
+    (those of tailored_attack_job, or "dnc") or a (rcmarl_tailored_family, rule id) pair; attack: "pipeline_uv",
+    "pipeline_std", "pipeline_sgn" or an rcmarl_adaptive_dev id; mixing: the receiver's mixing entry (None, "nnm",
+    "bucket" or ("bucket", s), see _lib.mixing_entry); n_perms: the attacker's shuffle samples under bucketing; (seed,
+    attacker, receiver, net, round, epoch): the Philox key and counter words of those samples; model_out [n]: R_0 of the
+    pick.  Names are checked here, ids and limits by the library."""
+    if isinstance(attack, str):
+        if not L.is_pipeline_attack(attack):
+            raise L.RcmarlError(f"unknown pipeline attack {attack!r}: expected one of {sorted(L.PIPELINE_ATTACKS)}")
+        attack = L.PIPELINE_ATTACKS[attack]
+    if L.is_spectral_rule(rule):
+        rule = (L.TAILOR_SPECTRAL, L.SPECTRAL_RULES[rule])
+    mixing = L.mixing_entry(mixing)
+    j = L.PipelineAttackJob()
+    j.attack = tailored_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, int(attack), scale, gamma_out)
+    j.model_out = ptr(model_out)
+    j.mixing = L.PIPE_NONE if mixing is None else L.PIPE_NNM if mixing == "nnm" else L.PIPE_BUCKET
+    j.s = mixing[1] if L.is_bucket_mixing(mixing) else 0
+    j.n_perms = n_perms
+    j.seed, j.attacker, j.receiver, j.net, j.round, j.epoch = int(seed), attacker, receiver, net, round, epoch
+    j._keep = (dst, msgs, gamma_out, model_out)
+    return j
+
+
+def pipeline_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.PipelineAttackJob, jobs)
+    L.check(L.lib().rcmarl_pipeline_attack(a, len(a), _stream()), "rcmarl_pipeline_attack")
+
+
 def dissensus_attack_job(dst, msgs, msg_stride, n, own, honest, n_byz, eps):
     """own: the receiver's message row; honest: the message rows of its honest set in list order; n_byz: the dissensus
     entries of its in_nodes (repeats included); eps >= 0 (include/rcmarl.h).  Limits are checked by the library."""

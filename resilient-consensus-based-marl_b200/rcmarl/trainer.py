@@ -166,7 +166,7 @@ class Trainer:
         # mixing matrix M (row-major [n_rows][n_in], n_rows = len(_rule_nodes(i))) of each agent that mixes: row 2q
         # critic, 2q + 1 TR of mix_agents[q]
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
-        # gamma of each adaptive or tailored attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
+        # gamma of each adaptive, tailored or pipeline attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         # the mimic attack's direction state z of each mimic pair (row q = mimic_pairs[q]; [q, 0, :PC] critic, [q, 1] TR),
         # the index into S_j each copied in the last epoch, and the power steps each has taken (host)
@@ -258,7 +258,11 @@ class Trainer:
         # their own too, after the adaptive one
         self.tailor_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                              if isinstance(self.attack[b][0], L.TailoredKind)]
-        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs
+        # the pairs whose attacker runs a pipeline-aware attack (rcmarl_pipeline_attack, kind L.PipelineKind), which
+        # models the receiver's mixing step and every rule, DnC included: a launch of their own, after the tailored one
+        self.pipe_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                           if isinstance(self.attack[b][0], L.PipelineKind)]
+        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs
         # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
         # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
         # tailored one
@@ -314,9 +318,10 @@ class Trainer:
         return out
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum or a tailored attack: float32 [2]}: the gamma of
-        the message b crafted for j in the last epoch of the last update round (include/rcmarl.h, rcmarl_adaptive_attack;
-        for a tailored attack gamma_i*, rcmarl_tailored_attack); entry 0 for the critic, 1 for the team-reward net."""
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored or a pipeline attack: float32 [2]}:
+        the gamma of the message b crafted for j in the last epoch of the last update round (include/rcmarl.h,
+        rcmarl_adaptive_attack; for a tailored or pipeline attack gamma_i*, rcmarl_tailored_attack /
+        rcmarl_pipeline_attack); entry 0 for the critic, 1 for the team-reward net."""
         if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
@@ -550,10 +555,12 @@ class Trainer:
         # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
         # (the min-max / min-sum pairs in a job list of their own, with the gamma of each message)
         # (and the tailored pairs in a third, against their receiver's own rule and H)
+        # (and the pipeline pairs in a fourth, against their receiver's mixing step, rule and H)
         # (then the dissensus pairs, and the mimic pairs with their direction states)
-        att_jobs, ada_jobs, tail_jobs, diss_jobs, mimic_jobs = [], [], [], [], []
+        att_jobs, ada_jobs, tail_jobs, pipe_jobs, diss_jobs, mimic_jobs = [], [], [], [], [], []
         ada_row = {e: q for q, e in enumerate(self.adapt_pairs)}
         tail_row = {e: len(self.adapt_pairs) + q for q, e in enumerate(self.tailor_pairs)}
+        pipe_row = {e: len(self.adapt_pairs) + len(self.tailor_pairs) + q for q, e in enumerate(self.pipe_pairs)}
         diss_set = set(self.diss_pairs)
         mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
         for e, (b, j, honest) in enumerate(self.byz_pairs):
@@ -574,12 +581,18 @@ class Trainer:
                     mimic_jobs.append(ops.mimic_attack_job(msgs[NA + e], msgs, P, P, honest, cand, self.mimic_z[q, t],
                                                            0, target_out=self.mimic_target[q, t:t + 1]))
                 continue
-            if e in tail_row:
+            if e in tail_row or e in pipe_row:
                 slots, hon = self._tailored_slots(j)
                 rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
+                        else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
                         else (L.TAILOR_COORD, self.aggregation[j]))
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
-                if e in tail_row:
+                if e in pipe_row:
+                    pipe_jobs.append(ops.pipeline_attack_job(
+                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, mixing=self.mixing[j],
+                        n_perms=L.PIPELINE_PERMS, seed=self.seed, attacker=b, receiver=j, net=t,
+                        round=self.episodes_done & 0xFFFFFFFF, gamma_out=self.att_gamma[pipe_row[e], t:t + 1]))
+                elif e in tail_row:
                     tail_jobs.append(ops.tailored_attack_job(msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind,
                                                              param, gamma_out=self.att_gamma[tail_row[e], t:t + 1]))
                 elif e in ada_row:
@@ -593,6 +606,8 @@ class Trainer:
                       for g in range(0, len(ada_jobs), L.MAX_JOBS)]
         tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
                        for g in range(0, len(tail_jobs), L.MAX_JOBS)]
+        pipe_groups = [ops.job_array(L.PipelineAttackJob, pipe_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(pipe_jobs), L.MAX_JOBS)]
         diss_groups = [ops.job_array(L.DissensusJob, diss_jobs[g:g + L.MAX_JOBS])
                        for g in range(0, len(diss_jobs), L.MAX_JOBS)]
         # mimic job 2q + t belongs to pair mimic_pairs[q]; its T0 is the attacker's parameter
@@ -663,6 +678,11 @@ class Trainer:
                 self.launches += 1
             for g in tail_groups:                                          # no epoch dependence either
                 ops.tailored_attack(g)
+                self.launches += 1
+            for g in pipe_groups:                                          # a bucketing receiver's samples per epoch
+                for job in g:
+                    job.epoch = epoch
+                ops.pipeline_attack(g)
                 self.launches += 1
             for g in diss_groups:                                          # no epoch dependence either
                 ops.dissensus_attack(g)

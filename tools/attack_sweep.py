@@ -16,7 +16,9 @@ messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, 
 whole-message rule is the effective weight w M of agent 4's message.  Likewise bucket+<rule> (s = 2) or
 bucket<s>+<rule> (e.g. bucket3+gmed) buckets the messages (rcmarl_bucket_mix) before the rule, which then reads the own
 row and ceil(3 / s) bucket means at C2; a rule that refuses that many rows at H = 1 (krum, mkrum at s = 2) is marked
-refused.  The tailored attacks do not model mixing either.
+refused.  The tailored attacks do not model mixing either; the pipeline-aware attacks (rcmarl_pipeline_attack:
+pipeline_uv, pipeline_std, pipeline_sgn, range multiplier 2 by default) model the receiver's mixing step and every rule,
+dnc included, and are never refused (their gamma is reported as the tailored attacks').
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -27,7 +29,8 @@ agent 4 Faulty, alternating the two trainers round by round (CUDA events around 
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
 and when it names dnc, on clip and dnc (all of them when it names both), alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
-tailored_std (every cooperative agent on clip) against gauss, and when it names mimic, the round on mimic against gauss.
+tailored_std (every cooperative agent on clip) against gauss, when it names a pipeline attack, the round on
+pipeline_std against gauss, and when it names mimic, the round on mimic against gauss.
 
     python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
                                  [rules=clip,trim,wmsr] [attacks=alie,ipm,gauss]
@@ -49,7 +52,7 @@ from rcmarl._lib import RcmarlError            # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
 PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0,
-          "dissensus": 1.0, "mimic": 50.0}
+          "pipeline_uv": 2.0, "pipeline_std": 2.0, "pipeline_sgn": 2.0, "dissensus": 1.0, "mimic": 50.0}
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -73,6 +76,7 @@ VECTOR = ("krum", "mkrum", "scclip", "gmed")
 WHOLE = VECTOR + ("dnc",)                       # the rules that report neighbour weights
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
 TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
+PIPELINE = ("pipeline_uv", "pipeline_std", "pipeline_sgn")
 ATTACKS = tuple((a.split(":")[0], float(a.split(":")[1]) if ":" in a else PARAMS.get(a, 1.0))
                 for a in (sys.argv[6] if len(sys.argv) > 6 else "alie,ipm,gauss").split(","))
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
@@ -197,8 +201,9 @@ def timing_line(rt):
                                                                for k in timed_rules()[1:]])
 
 
-adaptive = any(a in ADAPTIVE + TAILORED for a, _ in ATTACKS)
+adaptive = any(a in ADAPTIVE + TAILORED + PIPELINE for a, _ in ATTACKS)
 tailored = any(a in TAILORED for a, _ in ATTACKS)
+pipeline = any(a in PIPELINE for a, _ in ATTACKS)
 mimic = any(a == "mimic" for a, _ in ATTACKS)
 if vector:
     result["rule_timing"] = rt = rule_timing()
@@ -211,6 +216,10 @@ if tailored:
     result["tailored_timing"] = tt = adaptive_timing("tailored_std")
     print(f"update round with agent 4 Byzantine: gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std "
           f"{tt['tailored_std']['median_ms']:.2f} ms ({tt['tailored_std_added_ms']:+.3f})", flush=True)
+if pipeline:
+    result["pipeline_timing"] = pt = adaptive_timing("pipeline_std")
+    print(f"update round with agent 4 Byzantine: gauss {pt['gauss']['median_ms']:.2f} ms, pipeline_std "
+          f"{pt['pipeline_std']['median_ms']:.2f} ms ({pt['pipeline_std_added_ms']:+.3f})", flush=True)
 if mimic:
     result["mimic_timing"] = mt = adaptive_timing("mimic")
     print(f"update round with agent 4 Byzantine: gauss {mt['gauss']['median_ms']:.2f} ms, mimic "
@@ -266,7 +275,7 @@ for rule in RULES:
         if vector:
             cell["byz_weight"] = float(np.mean(byz)) if split_rule(rule)[1] in WHOLE else None
         if adaptive:
-            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED else None
+            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED + PIPELINE else None
         if mimic:
             cell["copied"] = {str(j): ks for j, ks in copied.items()} if copied else None
         result["cells"].append(cell)
@@ -312,6 +321,11 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
         f.write(f"\nC2 update round at {tt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
                 f"gauss {tt['gauss']['median_ms']:.2f} ms, tailored_std {tt['tailored_std']['median_ms']:.2f} ms "
                 f"({tt['tailored_std_added_ms']:+.3f} ms)\n")
+    if pipeline:
+        pt = result["pipeline_timing"]
+        f.write(f"\nC2 update round at {pt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
+                f"gauss {pt['gauss']['median_ms']:.2f} ms, pipeline_std {pt['pipeline_std']['median_ms']:.2f} ms "
+                f"({pt['pipeline_std_added_ms']:+.3f} ms)\n")
     if mimic:
         mt = result["mimic_timing"]
         f.write(f"\nC2 update round at {mt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "

@@ -1,12 +1,15 @@
-"""Compare the outputs of the distance-based rules (rcmarl_vector_aggregate) and the min-max / min-sum attacks
-(rcmarl_adaptive_attack) between two builds of librcmarl.so, bit for bit.  Their kernels share their rule bodies with
-tailored_attack_kernel (vector_rule, adaptive_gamma in csrc/train_kernels.cu), so a change there may change their
-register allocation and SASS; this shows whether it changed anything they compute.
+"""Compare the outputs of the distance-based rules (rcmarl_vector_aggregate), the min-max / min-sum attacks
+(rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
+(rcmarl_bucket_mix) and the tailored attacks (rcmarl_tailored_attack) between two builds of librcmarl.so, bit for bit.
+Their kernels share their bodies with tailored_attack_kernel and pipeline_attack_kernel (vector_rule, adaptive_gamma,
+dnc_rule, nnm_rows, bucket_draw / bucket_means and the candidate search in csrc/train_kernels.cu), so a change there
+may change their register allocation and SASS; this shows whether it changed anything they compute.
 
 Each build runs in its own process (RCMARL_LIB selects the library) on the same inputs: 24 messages of 1421 parameters
 around a common centre, four of them 1e3 times larger and one holding 1e30; every vector rule at n_in 1 .. 16 (H drawn
-per job, repeated in-nodes) with the weights, and every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
-gamma), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a build
+per job, repeated in-nodes) with the weights, every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
+gamma), DnC, nnm and bucketing (s = 1, 2, 3) at n_in 1 .. 16 with their weights or mixing matrices, and every tailored
+attack x rule at n_in 2 .. 16 (scale 2, with gamma), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a build
 from before rcmarl_tailored_attack existed loads too.
 
     python tools/compare_builds.py LIB_A LIB_B [out_dir]     -> prints whether every output is bitwise equal
@@ -60,6 +63,43 @@ for a in ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "m
         dsts.append(d)
     ops.adaptive_attack(jobs)
     outs += [d.cpu().numpy() for d in dsts]
+if hasattr(lib, "rcmarl_bucket_mix"):
+    # nnm and bucketing read their messages and write their rows at one stride: the messages padded to P + 256
+    wide = torch.full((24, P + 256), float("nan"), device="cuda")
+    wide[:, :P] = msgs
+    for kind in ("dnc", "nnm", 1, 2, 3):
+        jobs, dsts = [], []
+        for n_in in range(1, 17):
+            d = torch.full((17, P + 256), float("nan"), device="cuda")
+            nodes = [int(x) for x in rs.choice(24, size=n_in)]
+            H, n = int(rs.randint(0, n_in)), PC[n_in % 4]
+            if kind == "dnc":
+                jobs.append(ops.vector_job(d[0], msgs, P, n, nodes, H, L.SPECTRAL_DNC, weights_out=d[16, :16]))
+            elif kind == "nnm":
+                jobs.append(ops.vector_job(d, wide, P + 256, n, nodes, H, L.MIX_NNM, weights_out=d[16]))
+            else:
+                jobs.append(ops.bucket_job(d, wide, P + 256, n, nodes, kind, seed=n_in * 977, receiver=n_in, net=n_in & 1,
+                                           round=3 * n_in, epoch=n_in % 5, weights_out=d[16]))
+            dsts.append(d)
+        (ops.dnc_aggregate if kind == "dnc" else ops.nnm_mix if kind == "nnm" else ops.bucket_mix)(jobs)
+        outs += [d.cpu().numpy() for d in dsts]
+    for rule in ("clip", "trim", "wmsr", "krum", "mkrum", "scclip", "gmed"):
+        for a in ("tailored_uv", "tailored_std", "tailored_sgn"):
+            jobs, dsts = [], []
+            for n_in in range(2, 17):
+                if rule in ("krum", "mkrum") and n_in < 3:
+                    continue
+                n_cr = 1 + n_in % 3 if n_in > 3 else 1
+                real = [int(x) for x in rs.choice(24, size=n_in - n_cr)]
+                slots = real[:1] + [-1] * n_cr + real[1:]
+                honest = [k for k, s in enumerate(slots) if 0 <= s < 20] or [0]
+                top = n_in - 3 if rule in ("krum", "mkrum") else (n_in - 1) // 2 if rule == "trim" else n_in - 1
+                d = torch.full((P + 1,), float("nan"), device="cuda")
+                jobs.append(ops.tailored_attack_job(d[:P], msgs, P, PC[n_in % 4], slots, honest, rule,
+                                                    int(rs.randint(0, top + 1)), a, 2.0, gamma_out=d[P:]))
+                dsts.append(d)
+            ops.tailored_attack(jobs)
+            outs += [d.cpu().numpy() for d in dsts]
 np.savez(sys.argv[1], *outs)
 '''
 
@@ -78,7 +118,8 @@ def main():
     a = dump(sys.argv[1], os.path.join(out_dir, "outputs_a.npz"))
     b = dump(sys.argv[2], os.path.join(out_dir, "outputs_b.npz"))
     diff = [k for k in a.files if a[k].tobytes() != b[k].tobytes()]
-    print(f"{len(a.files)} output arrays (vector_aggregate outputs and weights, adaptive_attack messages and gamma): "
+    print(f"{len(a.files)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix and "
+          "tailored_attack outputs): "
           + ("bitwise equal" if not diff and a.files == b.files else f"{len(diff)} differ: {diff[:8]}"))
     sys.exit(1 if diff or a.files != b.files else 0)
 
