@@ -347,7 +347,9 @@ int rcmarl_mimic_attack(const rcmarl_mimic_job* jobs_host, int n_jobs, void* str
  * msg_stride, k = 0 .. n-1 (k = 0 is the receiver's own; repeats in in_nodes count), each of P = job.n packed
  * parameters (the whole network, hidden layers and head).  In fp32:
  *   D_kl = sum_p (x_k,p - x_l,p)^2,   d_k(z) = sqrt(sum_p (x_k,p - z_p)^2);
- * a distance that is not finite (overflow, e.g. a message of 1e30, or +-inf) counts as +inf.  Every rule outputs
+ * a distance that is not finite (overflow, e.g. a message of 1e30, or +-inf) counts as +inf, and a term (x_k,p -
+ * x_l,p)^2 below the fp32 range rounds to 0 (messages that differ by less than about 1e-23 per coordinate are at
+ * distance 0, and the index tie rules decide).  Every rule outputs
  *   out = sum_k w_k x_k,   w_k >= 0,   sum_k w_k = 1,
  * and writes w to weights_out when it is not NULL.
  *   KRUM    (Blanchard et al., NeurIPS 2017)  n >= H + 3.  score_k = the sum of the n - H - 2 smallest D_kl over l != k,

@@ -4,7 +4,7 @@ agent whose hidden-layer and estimate consensus use the aggregate of the packed 
 (oracle/rpbcac_oracle.py), which stays unchanged.
 
 The kernel's distances are fp32, so here a squared distance that is not finite or exceeds the fp32 range counts as +inf
-in either dtype: a message of 1e30 is at an infinite distance in both."""
+in either dtype: a message of 1e30 is at an infinite distance in both; and a term that underflows in fp32 is 0 in both."""
 import numpy as np
 
 import agg_oracle as AO
@@ -14,13 +14,17 @@ from oracle import rpbcac_oracle as O
 RULES = ("krum", "mkrum", "scclip", "gmed")
 GMED_ITERS, GMED_NU = 8, 1e-6
 F32_MAX = float(np.finfo(np.float32).max)
+F32_HALF_TINY = 2.0 ** -150                          # half the smallest fp32 subnormal: rounds to 0
 
 
 def sqdist(a, b):
-    """sum_p (a_p - b_p)^2 in a's dtype; +inf where not finite or beyond the fp32 range."""
+    """sum_p (a_p - b_p)^2 in a's dtype; +inf where not finite or beyond the fp32 range.  A term below half the
+    smallest fp32 subnormal is 0, as the kernel's fp32 product rounds it: in fp64 too, rows that differ by less than
+    about 1e-23 per coordinate are at distance 0."""
     with np.errstate(over="ignore", invalid="ignore"):
         d = np.asarray(a) - np.asarray(b)
-        s = (d * d).sum(-1)
+        t = d * d
+        s = np.where(t <= F32_HALF_TINY, t.dtype.type(0), t).sum(-1)
     return s if np.isfinite(s) and s <= F32_MAX else s.dtype.type(np.inf)
 
 
