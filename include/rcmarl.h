@@ -424,6 +424,43 @@ int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void
 typedef enum { RCMARL_SPECTRAL_DNC = 0 } rcmarl_spectral_rule;
 int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
+/* Exact subset-selection aggregation of whole messages (rcmarl_subset_aggregate): average the n - H messages that agree
+ * most as a set, found by searching every subset.  MDA, minimum-diameter averaging (El-Mhamdi, Guerraoui & Rouault,
+ * ICLR 2021), picks the subset of smallest diameter; SMEA, smallest-maximum-eigenvalue averaging (Allouah, Guerraoui,
+ * Gupta, Pinot & Stephan, ICML 2023), the subset whose covariance has the smallest top eigenvalue.  It takes
+ * rcmarl_vector_job with rule = RCMARL_SUBSET_MDA or RCMARL_SUBSET_SMEA; its n = n_in messages x_0 .. x_{n-1}, x_k =
+ * msgs + in_nodes[k] * msg_stride (x_0 the receiver's own; repeats in in_nodes count) each hold P = job.n floats.
+ *   Flagged    F = the rows holding +-inf (DnC's convention); U = every other row, in index order.  If U is empty:
+ *              out = x_0, w = e_0.  A row of 1e30 is finite and not flagged: fp64 holds its squared distances.
+ *   Distances  D_kl = sum_p ((double)x_k,p - (double)x_l,p)^2 for k, l in U, in fp64 (each pair summed by one warp:
+ *              lane-strided fma partials, then the fixed xor butterfly).  D_kk = 0, not computed.
+ *   Candidates s = n - max(|F|, H) (>= 1, as 0 <= H < n); the candidates are every s-subset of U, ranked in the
+ *              lexicographic order of their sorted index lists.
+ *   Criterion  c(S) = 0 when s = 1.  Otherwise MDA: c(S) = max over a < b in S of D_ab.  SMEA: c(S) = lambda_max(B_S),
+ *              B_S = -1/2 J D_S J the double-centred squared-distance matrix, in fp64 in this order: r_a = (sum_{b in
+ *              S, in order} D_ab) / s, t = (sum_{a in S, in order} r_a) / s, B_ab = -0.5 * (((D_ab - r_a) - r_b) + t)
+ *              for positions a <= b in S, B_ba = B_ab; lambda_max by cyclic Jacobi with exactly DnC's rotation and skip
+ *              rules and at most RCMARL_DNC_SWEEPS sweeps, the largest diagonal entry.  The covariance's top
+ *              eigenvalue is lambda_max / s; every candidate has the same s, so the 1/s is dropped.
+ *   Selection  S* = argmin c(S), ties to the lower rank.
+ *   Output     out = (sum_{k in S*, index order} x_k) / (float)s, an fp32 sum from 0 (multi-Krum's and DnC's
+ *              arithmetic); w_k = 1/(float)s on S*, 0 elsewhere, written to weights_out when it is not NULL.
+ * H = 0 with no flagged row gives the plain mean, bitwise rcmarl_dnc_aggregate's at H = 0 and, where n_in >= 3,
+ * multi-Krum's at H = 0.  H = n - 1 with no flagged row gives x_0 bitwise (a -0 coordinate comes out +0, as the sum
+ * starts from 0): every criterion is 0 and rank 0 is {0}.  The rule may drop the receiver's own message.  Rows of +-inf
+ * are never selected while fewer than n_in rows hold them, and rows of 1e30, at most H of them, get weight 0 while the
+ * other rows lie far closer together (a 1e30 row is at a squared distance of about 1e60 from each of them).  NaN inputs
+ * are not supported.  At most C(16, 8) = 12 870 candidates per job; one CTA per job, fixed summation orders, no
+ * atomics: bitwise reproducible, independent of the job order and of how jobs are split over launches.  dst[0:n] = out.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst and weights_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null
+ * dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, a rule other than RCMARL_SUBSET_MDA and
+ * RCMARL_SUBSET_SMEA, H outside [0, n_in), n_in * n > RCMARL_SUBSET_MAX_FLOATS (the staging bound: the messages are
+ * staged in shared memory), a dst or weights_out that overlaps an in-node row of any job of the launch, and two written
+ * ranges (dsts, weights_outs) of the launch that overlap. */
+#define RCMARL_SUBSET_MAX_FLOATS (48 * 1024)
+typedef enum { RCMARL_SUBSET_MDA = 0, RCMARL_SUBSET_SMEA = 1 } rcmarl_subset_rule;
+int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
 /* Nearest-neighbour mixing (rcmarl_nnm_mix): the pre-aggregation step of Allouah, Farhadkhani, Guerraoui, Gupta, Pinot
  * & Stephan, "Fixing by Mixing: A Recipe for Optimal Byzantine ML under Heterogeneity" (AISTATS 2023).  It replaces each
  * message a receiver hears by the mean of its n - H nearest received messages (itself among them); the receiver's own

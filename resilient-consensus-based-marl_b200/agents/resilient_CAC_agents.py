@@ -5,8 +5,8 @@ Same constructor and method names, argument meaning and mutation conventions as 
   *_update_local            return (message copy, loss) and leave the agent's own networks untouched (:113,120)
   resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166), or
                                  their trimmed / W-MSR mean with aggregation="trim" / "wmsr", or the hidden layers
-                                 of a distance-based ("krum", "mkrum", "scclip", "gmed") or divide-and-conquer
-                                 ("dnc") aggregate of whole messages
+                                 of a distance-based ("krum", "mkrum", "scclip", "gmed"), divide-and-conquer
+                                 ("dnc") or exact subset-selection ("mda", "smea") aggregate of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
                                  With mixing="nnm", every consensus step first replaces each received message by the
                                  mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix); with
@@ -35,8 +35,9 @@ class RPBCAC_agent():
         self.H = H
         # resilient aggregation rule of every consensus step: "clip" (the reference's), "trim" or "wmsr"
         # (include/rcmarl.h, rcmarl_agg_rule), or a distance-based rule over whole messages: "krum", "mkrum", "scclip"
-        # or "gmed" (rcmarl_vector_rule), or the spectral rule "dnc" (divide-and-conquer, rcmarl_dnc_aggregate)
-        if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation)):
+        # or "gmed" (rcmarl_vector_rule), the spectral rule "dnc" (divide-and-conquer, rcmarl_dnc_aggregate), or the
+        # exact subset-selection rules "mda" and "smea" (rcmarl_subset_aggregate)
+        if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation) or L.is_subset_rule(aggregation)):
             L.agg_rule(aggregation)
         self.aggregation = aggregation
         # pre-aggregation mixing of the received messages: None, "nnm", "bucket" or ("bucket", s) (rcmarl_mixing_rule)
@@ -88,17 +89,22 @@ class RPBCAC_agent():
         return out
 
     def _whole_messages(self):
-        """True if the rule aggregates whole messages (a distance-based rule or dnc)."""
-        return L.is_vector_rule(self.aggregation) or L.is_spectral_rule(self.aggregation)
+        """True if the rule aggregates whole messages (a distance-based rule, dnc, mda or smea)."""
+        return (L.is_vector_rule(self.aggregation) or L.is_spectral_rule(self.aggregation)
+                or L.is_subset_rule(self.aggregation))
 
     def _with_aggregate(self, stack):
-        """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based or
-        dnc rule."""
+        """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based, dnc,
+        mda or smea rule."""
         n, P = stack.shape
         out = torch.cat([stack, torch.empty(1, P, dtype=stack.dtype, device=stack.device)])
         if L.is_spectral_rule(self.aggregation):
             L.check_spectral_rule(self.H, n)
             ops.dnc_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, L.SPECTRAL_DNC)])
+        elif L.is_subset_rule(self.aggregation):
+            L.check_subset_rule(self.H, n)
+            ops.subset_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H,
+                                                 L.SUBSET_RULES[self.aggregation])])
         else:
             L.check_vector_rule(self.aggregation, self.H, n)
             ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
@@ -106,7 +112,7 @@ class RPBCAC_agent():
 
     def _consensus_inputs(self, stack, net, round):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
-        distance-based or dnc rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
+        distance-based, dnc, mda or smea rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
         Trainer.  An agent that mixes does so first (a bucketing agent with the draws of (net, round))."""
         stack = self._mixed(stack, net, round)
         if self._whole_messages():

@@ -13,6 +13,8 @@
 //                   median; rcmarl_vector_aggregate)
 //   dnc_agg_kernel  divide-and-conquer: removes the messages furthest along the top principal direction
 //                   (rcmarl_dnc_aggregate)
+//   subset_agg_kernel  exact subset selection (MDA, SMEA): averages the n - H messages that agree most as a set
+//                   (rcmarl_subset_aggregate)
 //   nnm_mix_kernel  nearest-neighbour mixing: each message becomes the mean of its n - H nearest (rcmarl_nnm_mix)
 //   bucket_mix_kernel  randomized bucketing: the received messages are shuffled into buckets of s and replaced by the
 //                   bucket means (rcmarl_bucket_mix)
@@ -586,6 +588,56 @@ __device__ __forceinline__ double warp_sum_f64(double v) {
     return v;
 }
 
+// Cyclic Jacobi on the symmetric m x m fp64 matrix A (m <= RCMARL_MAX_NEIGHBOURS, row stride RCMARL_MAX_NEIGHBOURS) in
+// shared memory, run by the calling warp, lane k owning row k, every lane computing each rotation identically: pairs
+// p < q in row order; a rotation is skipped, and A_pq set to 0, when 100 |A_pq| is below the rounding of |A_pp| and of
+// |A_qq|; at most RCMARL_DNC_SWEEPS sweeps, ending early after a sweep without a rotation.  The eigenvalues are left on
+// the diagonal.  V, when not null, is set to the identity and accumulates the rotations: column c is the eigenvector
+// of A_cc.  The rule of include/rcmarl.h for DnC's and SMEA's eigen-solves.
+__device__ __forceinline__ void warp_jacobi(double* A, double* V, int m) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    const int k = threadIdx.x & 31;
+    if (V && k < m)
+        for (int c = 0; c < m; ++c) V[k * MAXN + c] = c == k ? 1.0 : 0.0;
+    __syncwarp();
+    for (int sweep = 0; sweep < RCMARL_DNC_SWEEPS; ++sweep) {
+        bool rotated = false;
+        for (int p = 0; p < m - 1; ++p) {
+            for (int q = p + 1; q < m; ++q) {
+                const double apq = A[p * MAXN + q], app = A[p * MAXN + p], aqq = A[q * MAXN + q];
+                const double g = 100.0 * fabs(apq);
+                __syncwarp();                                       // every lane has read them
+                if (apq == 0.0 || (fabs(app) + g == fabs(app) && fabs(aqq) + g == fabs(aqq))) {
+                    if (k == 0) { A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0; }
+                    __syncwarp();
+                    continue;
+                }
+                rotated = true;
+                const double theta = (aqq - app) / (2.0 * apq);
+                const double tt = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + hypot(theta, 1.0));
+                const double c = 1.0 / sqrt(fma(tt, tt, 1.0)), s = tt * c;
+                if (k < m && k != p && k != q) {
+                    const double akp = A[k * MAXN + p], akq = A[k * MAXN + q];
+                    const double nkp = c * akp - s * akq, nkq = s * akp + c * akq;
+                    A[k * MAXN + p] = nkp; A[p * MAXN + k] = nkp;
+                    A[k * MAXN + q] = nkq; A[q * MAXN + k] = nkq;
+                } else if (k == p) {
+                    A[p * MAXN + p] = app - tt * apq;
+                    A[q * MAXN + q] = aqq + tt * apq;
+                    A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0;
+                }
+                if (V && k < m) {
+                    const double vkp = V[k * MAXN + p], vkq = V[k * MAXN + q];
+                    V[k * MAXN + p] = c * vkp - s * vkq;
+                    V[k * MAXN + q] = s * vkp + c * vkq;
+                }
+                __syncwarp();
+            }
+        }
+        if (!rotated) break;
+    }
+}
+
 // Divide-and-conquer (rcmarl_dnc_aggregate, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The fp32
 // messages and the fp64 mean of the unflagged ones are staged in shared memory; every Gram entry is summed by ONE warp
 // (lane-strided fp64 fma partials, then the fixed xor butterfly), so its value does not depend on which warp takes it.
@@ -647,45 +699,7 @@ __device__ __forceinline__ void dnc_rule(const Row& row, int n, int nin, int H, 
         __syncthreads();
         if (warp == 0) {
             const int k = lane;
-            if (k < m)
-                for (int c = 0; c < m; ++c) V[k * MAXN + c] = c == k ? 1.0 : 0.0;
-            __syncwarp();
-            for (int sweep = 0; sweep < RCMARL_DNC_SWEEPS; ++sweep) {
-                bool rotated = false;
-                for (int p = 0; p < m - 1; ++p) {
-                    for (int q = p + 1; q < m; ++q) {
-                        const double apq = A[p * MAXN + q], app = A[p * MAXN + p], aqq = A[q * MAXN + q];
-                        const double g = 100.0 * fabs(apq);
-                        __syncwarp();                               // every lane has read them
-                        if (apq == 0.0 || (fabs(app) + g == fabs(app) && fabs(aqq) + g == fabs(aqq))) {
-                            if (k == 0) { A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0; }
-                            __syncwarp();
-                            continue;
-                        }
-                        rotated = true;
-                        const double theta = (aqq - app) / (2.0 * apq);
-                        const double tt = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + hypot(theta, 1.0));
-                        const double c = 1.0 / sqrt(fma(tt, tt, 1.0)), s = tt * c;
-                        if (k < m && k != p && k != q) {
-                            const double akp = A[k * MAXN + p], akq = A[k * MAXN + q];
-                            const double nkp = c * akp - s * akq, nkq = s * akp + c * akq;
-                            A[k * MAXN + p] = nkp; A[p * MAXN + k] = nkp;
-                            A[k * MAXN + q] = nkq; A[q * MAXN + k] = nkq;
-                        } else if (k == p) {
-                            A[p * MAXN + p] = app - tt * apq;
-                            A[q * MAXN + q] = aqq + tt * apq;
-                            A[p * MAXN + q] = 0.0; A[q * MAXN + p] = 0.0;
-                        }
-                        if (k < m) {
-                            const double vkp = V[k * MAXN + p], vkq = V[k * MAXN + q];
-                            V[k * MAXN + p] = c * vkp - s * vkq;
-                            V[k * MAXN + q] = s * vkp + c * vkq;
-                        }
-                        __syncwarp();
-                    }
-                }
-                if (!rotated) break;
-            }
+            warp_jacobi(A, V, m);
             // lambda = the largest diagonal entry (ties to the lower index), score of U position a = lambda * u_a^2
             int top = 0;
             for (int c = 1; c < m; ++c)
@@ -735,6 +749,183 @@ __global__ void __launch_bounds__(VEC_THREADS) dnc_agg_kernel(const __grid_const
     }
     __syncthreads();
     dnc_rule(StagedRows{xs, n}, n, nin, job.H, mu, job.dst, S);
+    if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
+}
+
+// Exact subset selection (rcmarl_subset_aggregate, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The
+// messages are staged in shared memory, rows holding +-inf are flagged as in dnc_rule, and every fp64 distance of a
+// pair of U positions is summed by ONE warp (lane-strided fma partials, then the fixed xor butterfly).  A candidate is
+// a bit mask over U positions; rank r is unranked by the combinatorial number system, so the walk below visits ranks in
+// a fixed order whatever the data.  MDA takes one thread per candidate (ranks tid, tid + VEC_THREADS, ...); SMEA one
+// warp per candidate (ranks warp, warp + NW, ...), lane a owning row a of B_S in the warp's own scratch, solved by
+// warp_jacobi without eigenvectors.  Each thread keeps its best (c, rank), the earlier rank on equal c; warp 0 then
+// reduces them to S* by the order (c, rank), and the output takes one thread per coordinate.
+struct SubsetShared {
+    double D[RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];                      // D over U positions, D_aa = 0
+    double B[VEC_THREADS / 32][RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];    // SMEA: B_S of each warp's candidate
+    double best_c[VEC_THREADS];
+    int best_r[VEC_THREADS];
+    int binom[RCMARL_MAX_NEIGHBOURS + 1][RCMARL_MAX_NEIGHBOURS + 1];             // C(a, b), 0 for b > a
+    int ulist[RCMARL_MAX_NEIGHBOURS];                                             // U in index order
+    int flagged[RCMARL_MAX_NEIGHBOURS];
+    float wt[RCMARL_MAX_NEIGHBOURS];
+    int m;
+};
+
+// The candidate of lexicographic rank r among the sz-subsets of m U positions, as a bit mask (bit a: position a).
+__device__ __forceinline__ unsigned subset_unrank(int r, int m, int sz, const int (*binom)[RCMARL_MAX_NEIGHBOURS + 1]) {
+    unsigned mask = 0u;
+    int a = 0;
+    for (int i = 0; i < sz; ++i) {
+        for (;;) {                                  // the subsets whose i-th element is a and that share the first i
+            const int c = binom[m - 1 - a][sz - 1 - i];
+            if (r < c) break;
+            r -= c;
+            ++a;
+        }
+        mask |= 1u << a;
+        ++a;
+    }
+    return mask;
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ SubsetShared S;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in, H = job.H;
+    const bool smea = job.rule == RCMARL_SUBSET_SMEA;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float* xs = smem;                              // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    for (int e = tid; e < (MAXN + 1) * (MAXN + 1); e += VEC_THREADS) {
+        const int a = e / (MAXN + 1), b = e % (MAXN + 1);
+        int c = b > a ? 0 : 1;
+        for (int i = 0; i < b && i < a; ++i) c = c * (a - i) / (i + 1);
+        S.binom[a][b] = c;
+    }
+    __syncthreads();
+    const StagedRows row{xs, n};
+    for (int k = warp; k < nin; k += NW) {
+        bool inf = false;
+        for (int p = lane; p < n; p += 32) inf |= isinf(row.at(k, p));
+        inf = __any_sync(0xffffffffu, inf);
+        if (lane == 0) S.flagged[k] = inf ? 1 : 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int m = 0;
+        for (int k = 0; k < nin; ++k)
+            if (!S.flagged[k]) S.ulist[m++] = k;
+        S.m = m;
+    }
+    __syncthreads();
+    const int m = S.m;
+    if (m > 0) {
+        for (int t = warp; t < m * (m - 1) / 2; t += NW) {          // pairs a < b of U positions
+            int a = 0, r = t;
+            while (r >= m - 1 - a) { r -= m - 1 - a; ++a; }
+            const int b = a + 1 + r;
+            const float* xa = row(S.ulist[a]);
+            const float* xb = row(S.ulist[b]);
+            double s = 0.0;
+            for (int p = lane; p < n; p += 32) {
+                const double d = (double)xa[p] - (double)xb[p];
+                s = fma(d, d, s);
+            }
+            s = warp_sum_f64(s);
+            if (lane == 0) { S.D[a * MAXN + b] = s; S.D[b * MAXN + a] = s; }
+        }
+        if (tid < m) S.D[tid * MAXN + tid] = 0.0;
+        __syncthreads();
+        const int sz = nin - max(nin - m, H);                        // >= 1
+        const int total = S.binom[m][sz];
+        double bc = INFINITY;
+        int br = 0x7fffffff;
+        if (sz == 1) {                                                // every criterion is 0: rank 0
+            bc = 0.0;
+            br = 0;
+        } else if (!smea) {
+            for (int r = tid; r < total; r += VEC_THREADS) {
+                const unsigned mask = subset_unrank(r, m, sz, S.binom);
+                double c = 0.0;
+                for (unsigned ma = mask; ma; ma &= ma - 1) {
+                    const int a = __ffs(ma) - 1;
+                    for (unsigned mb = ma & (ma - 1); mb; mb &= mb - 1) {
+                        const double d = S.D[a * MAXN + __ffs(mb) - 1];
+                        if (d > c) c = d;
+                    }
+                }
+                if (c < bc) { bc = c; br = r; }
+            }
+        } else {
+            double* B = S.B[warp];
+            for (int r = warp; r < total; r += NW) {
+                const unsigned mask = subset_unrank(r, m, sz, S.binom);
+                int pa = 0;                                           // lane a < sz: the a-th position of the subset
+                unsigned mm = mask;
+                for (int i = 0; i < lane && mm; ++i) mm &= mm - 1;
+                if (mm) pa = __ffs(mm) - 1;
+                double ra = 0.0;                                      // r_a = (sum_b D_ab, b in order) / s
+                for (int b = 0; b < sz; ++b) {
+                    const int pb = __shfl_sync(0xffffffffu, pa, b);
+                    if (lane < sz) ra += S.D[pa * MAXN + pb];
+                }
+                ra = ra / (double)sz;
+                double t = 0.0;                                       // t = (sum_a r_a, a in order) / s
+                for (int b = 0; b < sz; ++b) t += __shfl_sync(0xffffffffu, ra, b);
+                t = t / (double)sz;
+                for (int b = 0; b < sz; ++b) {                        // B_ab for a <= b, mirrored
+                    const int pb = __shfl_sync(0xffffffffu, pa, b);
+                    const double rb = __shfl_sync(0xffffffffu, ra, b);
+                    if (lane <= b) {
+                        const double v = -0.5 * (((S.D[pa * MAXN + pb] - ra) - rb) + t);
+                        B[lane * MAXN + b] = v;
+                        B[b * MAXN + lane] = v;
+                    }
+                }
+                __syncwarp();
+                warp_jacobi(B, nullptr, sz);
+                double c = B[0];
+                for (int a = 1; a < sz; ++a) c = fmax(c, B[a * MAXN + a]);
+                __syncwarp();                                         // every lane has read the diagonal
+                if (c < bc) { bc = c; br = r; }
+            }
+        }
+        S.best_c[tid] = bc;
+        S.best_r[tid] = br;
+        __syncthreads();
+        if (warp == 0) {                                              // argmin over (c, rank): a total order
+            for (int q = lane + 32; q < VEC_THREADS; q += 32) {
+                const double c = S.best_c[q];
+                const int r = S.best_r[q];
+                if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                const double c = __shfl_xor_sync(0xffffffffu, bc, o);
+                const int r = __shfl_xor_sync(0xffffffffu, br, o);
+                if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
+            }
+            const unsigned mask = subset_unrank(br, m, sz, S.binom);
+            if (lane < nin) S.wt[lane] = 0.f;
+            __syncwarp();
+            if (lane < m && ((mask >> lane) & 1u)) S.wt[S.ulist[lane]] = 1.f / (float)sz;
+        }
+    } else if (tid < nin) {
+        S.wt[tid] = tid == 0 ? 1.f : 0.f;                            // every row flagged: out = x_0
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = s (1 when every row is flagged)
+        float s = 0.f, cnt = 0.f;
+        for (int k = 0; k < nin; ++k)
+            if (S.wt[k] != 0.f) { s += row.at(k, p); cnt += 1.f; }
+        job.dst[p] = s / cnt;
+    }
     if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
 }
 
@@ -1994,6 +2185,46 @@ int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream
     if (int e = opt_in_smem((const void*)dnc_agg_kernel, (int)(sizeof(float) * RCMARL_DNC_MAX_FLOATS), opted)) return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     dnc_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if ((q.rule != RCMARL_SUBSET_MDA && q.rule != RCMARL_SUBSET_SMEA) || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)q.n_in * q.n;
+        if (floats > RCMARL_SUBSET_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+    }
+    // as rcmarl_vector_aggregate: no written range (a dst, a weights_out) may overlap an in-node row of any job of the
+    // launch or another written range
+    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
+        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
+        ++n_w;
+        if (jobs[j].weights_out) {
+            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
+            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
+    }
+    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)subset_agg_kernel, (int)(sizeof(float) * RCMARL_SUBSET_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    subset_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

@@ -46,6 +46,9 @@ SPECTRAL_DNC = 0                                  # rcmarl_spectral_rule
 SPECTRAL_RULES = {"dnc": SPECTRAL_DNC}
 DNC_SWEEPS = 32
 DNC_MAX_FLOATS = 48 * 1024
+SUBSET_MDA, SUBSET_SMEA = 0, 1                    # rcmarl_subset_rule
+SUBSET_RULES = {"mda": SUBSET_MDA, "smea": SUBSET_SMEA}
+SUBSET_MAX_FLOATS = 48 * 1024
 MIX_NNM = 0                                       # rcmarl_mixing_rule
 MIXING_RULES = {"nnm": MIX_NNM}
 NNM_MAX_FLOATS = 48 * 1024
@@ -176,6 +179,7 @@ SYMBOLS = [
     ("rcmarl_attack", C.c_int, [C.POINTER(AttackJob), C.c_int, c_fp]),
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_subset_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
@@ -287,6 +291,19 @@ def check_spectral_rule(H, n_in):
     if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
         raise RcmarlError(f"aggregation 'dnc' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
     return SPECTRAL_DNC
+
+
+def is_subset_rule(rule):
+    """True for the name of an exact subset-selection rule (rcmarl_subset_rule): "mda", "smea"."""
+    return isinstance(rule, str) and rule in SUBSET_RULES
+
+
+def check_subset_rule(H, n_in):
+    """Raise RcmarlError unless the subset-selection rules (rcmarl_subset_aggregate, include/rcmarl.h) allow H out of
+    n_in messages: 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  The names are SUBSET_RULES (see is_subset_rule)."""
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
+        raise RcmarlError(f"aggregation 'mda' / 'smea' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most "
+                          f"{MAX_NEIGHBOURS})")
 
 
 def mixing_entry(mixing):

@@ -457,6 +457,12 @@ def dnc_aggregate(jobs):
     L.check(L.lib().rcmarl_dnc_aggregate(a, len(a), _stream()), "rcmarl_dnc_aggregate")
 
 
+def subset_aggregate(jobs):
+    """rcmarl_subset_aggregate over rcmarl_vector_job jobs (vector_job(..., rule=L.SUBSET_MDA or L.SUBSET_SMEA, ...))."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_subset_aggregate(a, len(a), _stream()), "rcmarl_subset_aggregate")
+
+
 def nnm_mix(jobs):
     """rcmarl_nnm_mix over rcmarl_vector_job jobs (vector_job(dst, ..., rule=L.MIX_NNM, weights_out=[n_in * n_in])):
     mixed row k goes to dst + k * msg_stride."""

@@ -61,17 +61,21 @@ class Trainer:
         # A distance-based rule ("krum", "mkrum", "scclip", "gmed") aggregates whole messages into one extra message row
         # per such agent; its consensus and team jobs then read that row as their only in-node under clip, which returns
         # it exactly (the projection target phi.W3 + b3 is linear in the head).
-        # The spectral rule "dnc" (divide-and-conquer) does the same through a launch of its own.
+        # The spectral rule "dnc" (divide-and-conquer) does the same through a launch of its own, and so do the exact
+        # subset-selection rules "mda" and "smea" (rcmarl_subset_rule).
         self.vector_rule = [L.VECTOR_RULES[a] if L.is_vector_rule(a) else None for a in agg] + [None] * (NA - n_real)
         self.dnc = [L.is_spectral_rule(a) for a in agg] + [False] * (NA - n_real)
-        self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) or L.is_spectral_rule(a) else L.agg_rule(a) for a in agg] \
-            + [L.AGG_CLIP] * (NA - n_real)
+        self.subset_rule = [L.SUBSET_RULES[a] if L.is_subset_rule(a) else None for a in agg] + [None] * (NA - n_real)
+        self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) or L.is_spectral_rule(a) or L.is_subset_rule(a)
+                            else L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
 
         def check_rule(i, n):
             if self.vector_rule[i] is not None:
                 L.check_vector_rule(agg[i], self.H[i], n)
             elif self.dnc[i]:
                 L.check_spectral_rule(self.H[i], n)
+            elif self.subset_rule[i] is not None:
+                L.check_subset_rule(self.H[i], n)
             else:
                 L.check_aggregation(agg[i], self.H[i], n)
         for i in self.coop:
@@ -110,16 +114,25 @@ class Trainer:
             if self.mixing[j] is not None:
                 raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose mixing "
                                     f"{self.mixing[j]!r} the tailored attack does not model")
+        for e in self.tailor_pairs + self.pipe_pairs:   # neither attack models the subset-selection rules
+            b, j, _ = self.byz_pairs[e]
+            if self.subset_rule[j] is not None:
+                raise L.RcmarlError(f"Byzantine agent {b} runs a {'tailored' if e in self.tailor_pairs else 'pipeline'} "
+                                    f"attack against agent {j}, whose rule {agg[j]!r} the attack does not model")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
-        # that of each cooperative agent on dnc
+        # that of each cooperative agent on dnc, then that of each on mda / smea
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
         self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
         self.dnc_agents = [i for i in self.coop if self.dnc[i]]
         self.dnc_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + q for q, i in enumerate(self.dnc_agents)}
+        self.subset_agents = [i for i in self.coop if self.subset_rule[i] is not None]
+        self.subset_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + q
+                           for q, i in enumerate(self.subset_agents)}
         # then the mixed rows of each cooperative agent that mixes (n_in for nnm, n_out for bucketing): mixed row k at
         # mix_row[i] + k
         self.mix_agents = [i for i in self.coop if self.mixing[i] is not None]
-        self.mix_row, row = {}, NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
+        self.mix_row, row = {}, NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) \
+            + len(self.subset_agents)
         for i in self.mix_agents:
             self.mix_row[i] = row
             row += L.mixed_rows(self.mixing[i], len(self.in_nodes[i]))
@@ -153,9 +166,9 @@ class Trainer:
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
-        # vec_row[i] / dnc_row[i] the aggregate of cooperative agent i's distance-based / dnc rule; mix_row[i] + k its
-        # mixed message k
-        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) \
+        # vec_row[i] / dnc_row[i] / subset_row[i] the aggregate of cooperative agent i's distance-based / dnc / mda or
+        # smea rule; mix_row[i] + k its mixed message k
+        n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + len(self.subset_agents) \
             + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
@@ -163,6 +176,9 @@ class Trainer:
         self.vec_weights = torch.zeros(2 * len(self.vec_agents), L.MAX_NEIGHBOURS, **f32) if self.vec_agents else None
         # ... and of each dnc aggregate: row 2q critic, 2q + 1 TR of dnc_agents[q]
         self.dnc_weights = torch.zeros(2 * len(self.dnc_agents), L.MAX_NEIGHBOURS, **f32) if self.dnc_agents else None
+        # ... and of each mda / smea aggregate: row 2q critic, 2q + 1 TR of subset_agents[q]
+        self.subset_weights = (torch.zeros(2 * len(self.subset_agents), L.MAX_NEIGHBOURS, **f32)
+                               if self.subset_agents else None)
         # mixing matrix M (row-major [n_rows][n_in], n_rows = len(_rule_nodes(i))) of each agent that mixes: row 2q
         # critic, 2q + 1 TR of mix_agents[q]
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
@@ -282,13 +298,14 @@ class Trainer:
         return list(range(self.mix_row[j], self.mix_row[j] + L.mixed_rows(self.mixing[j], len(self.in_nodes[j]))))
 
     def neighbour_weights(self):
-        """{cooperative agent i with a distance-based or the dnc rule: float32 [2, n_in]}: the weight w_k its rule gave
-        each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message crafted for i) in
-        the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.  For an agent that
-        mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry is the effective
-        weight w M of each in-neighbour."""
+        """{cooperative agent i with a distance-based, the dnc or an mda / smea rule: float32 [2, n_in]}: the weight w_k
+        its rule gave each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message
+        crafted for i) in the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.
+        For an agent that mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry
+        is the effective weight w M of each in-neighbour."""
         out = {}
-        for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights)):
+        for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights),
+                                (self.subset_agents, self.subset_weights)):
             if not agents:
                 continue
             w = weights.cpu().numpy()
@@ -539,8 +556,9 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            if i in self.vec_row or i in self.dnc_row:   # the aggregate as the single in-node: clip returns it exactly
-                nodes, H, rule = [self.vec_row.get(i, self.dnc_row.get(i))], 0, L.AGG_CLIP
+            agg_row = self.vec_row.get(i, self.dnc_row.get(i, self.subset_row.get(i)))
+            if agg_row is not None:                        # the aggregate as the single in-node: clip returns it exactly
+                nodes, H, rule = [agg_row], 0, L.AGG_CLIP
             else:
                 nodes, H, rule = self._rule_nodes(i), self.H[i], self.aggregation[i]
             cons_jobs.append(ops.consensus_job(self.critic[i], self.msg_c, self.PC, nets.n_hidden_params(2 * NA), nodes, H, rule))
@@ -650,6 +668,14 @@ class Trainer:
                 dnc_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], L.SPECTRAL_DNC,
                                                weights_out=self.dnc_weights[2 * q + t]))
         dnc_jobs = ops.job_array(L.VectorJob, dnc_jobs) if dnc_jobs else None
+        # the mda / smea aggregates likewise, in one launch of their own
+        subset_jobs = []
+        for q, i in enumerate(self.subset_agents):
+            nodes, row = self._rule_nodes(i), self.subset_row[i]
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                subset_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], self.subset_rule[i],
+                                                  weights_out=self.subset_weights[2 * q + t]))
+        subset_jobs = ops.job_array(L.VectorJob, subset_jobs) if subset_jobs else None
 
         for epoch in range(self.n_epochs):                                 # :100
             # ---------------- I) local updates (:105-121)
@@ -708,6 +734,9 @@ class Trainer:
                 self.launches += 1
             if dnc_jobs is not None:
                 ops.dnc_aggregate(dnc_jobs)
+                self.launches += 1
+            if subset_jobs is not None:
+                ops.subset_aggregate(subset_jobs)
                 self.launches += 1
             # ---------------- II) resilient consensus (:125-145)
             if coop:

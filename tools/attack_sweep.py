@@ -1,24 +1,25 @@
 """Byzantine attacks against each resilient aggregation rule on the C2 team: 4 cooperative agents (H = 1) and agent 4
 Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (by default clip, trim, wmsr; any of the coordinate rules,
-the distance-based krum, mkrum, scclip, gmed and the divide-and-conquer dnc) x attack (alie, ipm, gauss) over the learning harness's seeds
+the distance-based krum, mkrum, scclip, gmed, the divide-and-conquer dnc and the exact subset-selection mda and smea)
+x attack (alie, ipm, gauss) over the learning harness's seeds
 (tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed; agent 4 keeps its weights
 and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the cooperative critics' estimate
-of it, means of the last 500 episodes, over the seeds; for a distance-based rule or dnc also the mean weight the receivers of
+of it, means of the last 500 episodes, over the seeds; for a distance-based rule, dnc, mda or smea also the mean weight the receivers of
 agent 4 gave its crafted message in the last epoch of the last round (Trainer.neighbour_weights, both nets), over the
 seeds.  The attack list (by default alie 1.0, ipm 0.5, gauss 0.3) may also name the min-max / min-sum attacks
 (rcmarl_adaptive_attack: minmax_uv, minmax_std, minmax_sgn, minsum_uv, minsum_std, minsum_sgn, scale 1 = the paper's
 attack) and the rule-aware attacks tuned against each receiver's own rule and H (rcmarl_tailored_attack: tailored_uv,
 tailored_std, tailored_sgn, range multiplier 2 by default); an entry is a name or name:param.  For those the table also
 reports the mean gamma (gamma_i* for a tailored attack) of agent 4's messages in the last epoch of the last round
-(Trainer.attack_gammas, both nets and every receiver), over the seeds.  The tailored attacks do not model dnc: those
-cells are marked refused.  A rule may be written nnm+<rule> (e.g. nnm+mkrum): every cooperative agent then mixes the
+(Trainer.attack_gammas, both nets and every receiver), over the seeds.  The tailored attacks do not model dnc, mda or
+smea: those cells are marked refused.  A rule may be written nnm+<rule> (e.g. nnm+mkrum): every cooperative agent then mixes the
 messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, and the weight reported for a
 whole-message rule is the effective weight w M of agent 4's message.  Likewise bucket+<rule> (s = 2) or
 bucket<s>+<rule> (e.g. bucket3+gmed) buckets the messages (rcmarl_bucket_mix) before the rule, which then reads the own
 row and ceil(3 / s) bucket means at C2; a rule that refuses that many rows at H = 1 (krum, mkrum at s = 2) is marked
 refused.  The tailored attacks do not model mixing either; the pipeline-aware attacks (rcmarl_pipeline_attack:
 pipeline_uv, pipeline_std, pipeline_sgn, range multiplier 2 by default) model the receiver's mixing step and every rule,
-dnc included, and are never refused (their gamma is reported as the tailored attacks').
+dnc included, but not mda or smea, whose cells are marked refused (their gamma is reported as the tailored attacks').
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -27,7 +28,8 @@ agent 4 copied in the last epoch of the last round (Trainer.mimic_targets, criti
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
-and when it names dnc, on clip and dnc (all of them when it names both), alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
+and when it names dnc, mda or smea, on clip and each of those it names (all of them when it names several),
+alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
 tailored_std (every cooperative agent on clip) against gauss, when it names a pipeline attack, the round on
 pipeline_std against gauss, and when it names mimic, the round on mimic against gauss.
@@ -73,7 +75,8 @@ def split_rule(rule):
 
 BASES = tuple(split_rule(r)[1] for r in RULES)
 VECTOR = ("krum", "mkrum", "scclip", "gmed")
-WHOLE = VECTOR + ("dnc",)                       # the rules that report neighbour weights
+SUBSET = ("mda", "smea")
+WHOLE = VECTOR + ("dnc",) + SUBSET              # the rules that report neighbour weights
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
 TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
 PIPELINE = ("pipeline_uv", "pipeline_std", "pipeline_sgn")
@@ -118,9 +121,10 @@ def timing():
 
 
 def timed_rules():
-    """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc if listed."""
+    """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc, mda and
+    smea where listed."""
     return (("clip",) + (("gmed", "mkrum") if any(r in VECTOR for r in BASES) else ())
-            + (("dnc",) if "dnc" in BASES else ()))
+            + tuple(r for r in ("dnc",) + SUBSET if r in BASES))
 
 
 def rule_timing():
@@ -252,7 +256,7 @@ for rule in RULES:
                 tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
                              desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=base,
                              attack=attack, mixing=mixing, **bench.HYPER)
-            except RcmarlError as ex:                   # e.g. a tailored attack against dnc or mixing
+            except RcmarlError as ex:                   # e.g. a tailored attack against dnc, mda or mixing
                 refused = str(ex)
                 break
             t, e = [], []

@@ -1,16 +1,19 @@
 """Compare the outputs of the distance-based rules (rcmarl_vector_aggregate), the min-max / min-sum attacks
 (rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
-(rcmarl_bucket_mix) and the tailored attacks (rcmarl_tailored_attack) between two builds of librcmarl.so, bit for bit.
-Their kernels share their bodies with tailored_attack_kernel and pipeline_attack_kernel (vector_rule, adaptive_gamma,
-dnc_rule, nnm_rows, bucket_draw / bucket_means and the candidate search in csrc/train_kernels.cu), so a change there
-may change their register allocation and SASS; this shows whether it changed anything they compute.
+(rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack) and the subset-selection rules MDA / SMEA
+(rcmarl_subset_aggregate) between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with
+tailored_attack_kernel and pipeline_attack_kernel (vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows,
+bucket_draw / bucket_means and the candidate search in csrc/train_kernels.cu), so a change there may change their
+register allocation and SASS; this shows whether it changed anything they compute.
 
 Each build runs in its own process (RCMARL_LIB selects the library) on the same inputs: 24 messages of 1421 parameters
 around a common centre, four of them 1e3 times larger and one holding 1e30; every vector rule at n_in 1 .. 16 (H drawn
 per job, repeated in-nodes) with the weights, every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
 gamma), DnC, nnm and bucketing (s = 1, 2, 3) at n_in 1 .. 16 with their weights or mixing matrices, and every tailored
-attack x rule at n_in 2 .. 16 (scale 2, with gamma), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a build
-from before rcmarl_tailored_attack existed loads too.
+attack x rule at n_in 2 .. 16 (scale 2, with gamma), and MDA and SMEA at n_in 1 .. 16 (H drawn per job, with the
+weights), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a
+build from before rcmarl_tailored_attack existed loads too; the outputs of an entry point only one build exports are
+listed and not compared.
 
     python tools/compare_builds.py LIB_A LIB_B [out_dir]     -> prints whether every output is bitwise equal
     (e.g. build the parent commit with `git archive HEAD~1 | tar -x -C DIR && make -C DIR/resilient-consensus-based-marl_b200/csrc`)
@@ -100,7 +103,19 @@ if hasattr(lib, "rcmarl_bucket_mix"):
                 dsts.append(d)
             ops.tailored_attack(jobs)
             outs += [d.cpu().numpy() for d in dsts]
-np.savez(sys.argv[1], *outs)
+named = {}
+if hasattr(lib, "rcmarl_subset_aggregate"):
+    for rule in ("mda", "smea"):
+        jobs, dsts = [], []
+        for n_in in range(1, 17):
+            d = torch.full((P + 16,), float("nan"), device="cuda")
+            nodes = [int(x) for x in rs.choice(24, size=n_in)]
+            jobs.append(ops.vector_job(d[:P], msgs, P, PC[n_in % 4], nodes, int(rs.randint(0, n_in)),
+                                       L.SUBSET_RULES[rule], weights_out=d[P:]))
+            dsts.append(d)
+        ops.subset_aggregate(jobs)
+        named.update({f"subset_{rule}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
+np.savez(sys.argv[1], *outs, **named)
 '''
 
 
@@ -117,11 +132,14 @@ def main():
     out_dir = sys.argv[3] if len(sys.argv) > 3 else tempfile.mkdtemp()
     a = dump(sys.argv[1], os.path.join(out_dir, "outputs_a.npz"))
     b = dump(sys.argv[2], os.path.join(out_dir, "outputs_b.npz"))
-    diff = [k for k in a.files if a[k].tobytes() != b[k].tobytes()]
-    print(f"{len(a.files)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix and "
-          "tailored_attack outputs): "
-          + ("bitwise equal" if not diff and a.files == b.files else f"{len(diff)} differ: {diff[:8]}"))
-    sys.exit(1 if diff or a.files != b.files else 0)
+    common = [k for k in a.files if k in b.files]
+    only = sorted(set(a.files) ^ set(b.files))
+    diff = [k for k in common if a[k].tobytes() != b[k].tobytes()]
+    print(f"{len(common)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix, "
+          "tailored_attack and subset_aggregate outputs): "
+          + ("bitwise equal" if not diff else f"{len(diff)} differ: {diff[:8]}")
+          + (f"; {len(only)} from an entry point only one build exports, not compared" if only else ""))
+    sys.exit(1 if diff or not common else 0)
 
 
 if __name__ == "__main__":
