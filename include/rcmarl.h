@@ -485,7 +485,7 @@ int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void
  * memory), a written range (the n_in dst rows, the n_in^2 weights) that overlaps an in-node row of any job of the
  * launch, and two written ranges of the launch that overlap. */
 #define RCMARL_NNM_MAX_FLOATS (48 * 1024)
-typedef enum { RCMARL_MIX_NNM = 0, RCMARL_MIX_BUCKET = 1 } rcmarl_mixing_rule;
+typedef enum { RCMARL_MIX_NNM = 0, RCMARL_MIX_BUCKET = 1, RCMARL_MIX_MOMENTUM = 2 } rcmarl_mixing_rule;
 int rcmarl_nnm_mix(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
 /* Randomized bucketing (rcmarl_bucket_mix): the pre-aggregation step of Karimireddy, He & Jaggi, "Byzantine-robust
@@ -529,6 +529,45 @@ typedef struct {
     uint32_t receiver, net, round, epoch;   /* Philox counter words */
 } rcmarl_bucket_job;
 int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs_host, int n_jobs, void* stream);
+
+/* Per-neighbour momentum (rcmarl_momentum_mix): the stateful pre-aggregation step of Karimireddy, He & Jaggi, "Learning
+ * from History for Byzantine Robust Optimization" (ICML 2021).  The receiver keeps, for every slot it hears, an
+ * exponential moving average of that slot's update against its own net, and its rule reads the averages instead of the
+ * latest messages: honest noise averages out, a bias repeated every round builds up into an outlier.  Momentum is
+ * linear in what the receiver hears, so the receiver computes it itself; what agents send is unchanged.  One job is one
+ * (receiver, net): n = n_in message slots x_k = msgs + in_nodes[k] * msg_stride (x_0 the receiver's own; repeats in
+ * in_nodes count as separate slots), each of P = job.n floats; the reference c = ref[0:P] (the receiver's net after its
+ * previous consensus step); the state M, n_in rows at momentum + k * momentum_stride, read and written; beta in [0, 1)
+ * and first in {0, 1}.  For each slot k and coordinate p, in fp32 with every operation rounded on its own (no FMA):
+ *   u       = x_k,p - c_p
+ *   M_k,p   = u                             if first, or if M_k,p is finite and u is not
+ *           = M_k,p                         if M_k,p is +-inf and not first (a poisoned coordinate stays poisoned)
+ *           = beta * M_k,p + (1 - beta) * u otherwise ((1 - beta) one fp32 subtraction)
+ *   row_k,p = c_p + M_k,p                   written to dst + k * msg_stride.
+ * The rows are full packed nets (row 0 the own slot's), read by every rule as the mixed rows of rcmarl_nnm_mix are.  A
+ * +-inf or 1e30 message poisons its own slot's row only, so at most H poisoned inputs give at most H poisoned rows.  At
+ * beta = 0, row_k = (x_k - c) + c: x_k up to one rounding.  first = 1 ignores the old M (it is not read).  NaN inputs
+ * are not supported.  One thread per coordinate and slot, no reductions, no atomics: bitwise reproducible, independent
+ * of the job order and of how jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, every dst row and every M row untouched): n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null dst, msgs, ref or momentum, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative
+ * in-node, a beta that is not finite or lies outside [0, 1), first other than 0 or 1, a written range (the n_in dst
+ * rows, the n_in M rows) that overlaps an in-node row or a ref of any job of the launch, two written ranges of the
+ * launch that overlap, and a ref that overlaps an in-node row of any job of the launch. */
+typedef struct {
+    float* dst;                 /* n_in rows at dst + k * msg_stride */
+    const float* msgs;          /* base of the message stack */
+    int64_t msg_stride;
+    const float* ref;           /* [n]: c */
+    float* momentum;            /* n_in rows at momentum + k * momentum_stride: M, read and written */
+    int64_t momentum_stride;
+    int32_t n;                  /* parameters per message */
+    int32_t n_in;
+    int32_t in_nodes[RCMARL_MAX_NEIGHBOURS];
+    float beta;                 /* 0 <= beta < 1 */
+    int32_t first;              /* 1: M = u (the slot's first step) */
+} rcmarl_momentum_job;
+int rcmarl_momentum_mix(const rcmarl_momentum_job* jobs_host, int n_jobs, void* stream);
 
 /* Pipeline-aware Byzantine messages (rcmarl_pipeline_attack): the AGR-tailored attack of rcmarl_tailored_attack against
  * the receiver's whole aggregation pipeline -- its mixing step (none, rcmarl_nnm_mix or rcmarl_bucket_mix), then its rule,

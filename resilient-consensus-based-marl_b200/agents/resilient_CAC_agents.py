@@ -11,7 +11,9 @@ Same constructor and method names, argument meaning and mutation conventions as 
                                  With mixing="nnm", every consensus step first replaces each received message by the
                                  mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix); with
                                  mixing="bucket" or ("bucket", s) it keeps its own message and replaces the others by
-                                 the means of random buckets of s (randomized bucketing, rcmarl_bucket_mix)
+                                 the means of random buckets of s (randomized bucketing, rcmarl_bucket_mix); with
+                                 momentum=beta it replaces slot k's message by its net plus the moving average of
+                                 slot k's update against its net (per-neighbour momentum, rcmarl_momentum_mix)
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
 Tensors may be NumPy arrays, torch tensors or facade Tensors; they are moved to the GPU.  Calling these methods one
@@ -27,7 +29,8 @@ from rcmarl import nets, ops
 
 
 class RPBCAC_agent():
-    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip", mixing=None):
+    def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip", mixing=None,
+                 momentum=None):
         self.actor = actor
         self.critic = critic
         self.TR = team_reward
@@ -48,6 +51,17 @@ class RPBCAC_agent():
         # with receiver 0 and epoch 0; the round is a per-net count of hidden consensus calls (0 critic, 1 team reward)
         self._bucket_seed = tensorflow.random.seed
         self._consensus_calls = [0, 0]
+        # per-neighbour momentum at beta (rcmarl_momentum_mix), or None.  Per net (0 critic, 1 team reward): the state M
+        # [n_in, P], created at the first hidden consensus call, and the momentum rows of the last hidden call, which
+        # the estimate consensus reuses.  The reference c of a step is the net at its hidden call: the net at the end
+        # of the previous consensus round (at construction, for the first).
+        if momentum is not None:
+            momentum = L.check_momentum(momentum)
+            if self.mixing is not None:
+                raise L.RcmarlError(f"momentum and mixing {self.mixing!r} together: at most one pre-aggregation step")
+        self.momentum = momentum
+        self._momentum_M = [None, None]
+        self._momentum_rows = [None, None]
         self.n_actions = self.actor.output_shape[1]
         self.fast_lr = fast_lr
         self.slow_lr = slow_lr
@@ -86,6 +100,22 @@ class RPBCAC_agent():
             return out
         out = torch.empty_like(stack)
         ops.nnm_mix([ops.vector_job(out, stack, P, P, list(range(n)), self.H, L.MIX_NNM)])
+        return out
+
+    def _momentum_step(self, stack, ref, net):
+        """[n, P] device stack (own = row 0) -> its n momentum rows against the reference net `ref`, one momentum step
+        of net `net` (the first step of each net starts its state)."""
+        n, P = stack.shape
+        M = self._momentum_M[net]
+        first = M is None
+        if first:
+            M = self._momentum_M[net] = torch.empty_like(stack)
+        elif M.shape != stack.shape:
+            raise L.RcmarlError(f"momentum keeps one state per slot: this agent's net {net} has heard {M.shape[0]} "
+                                f"messages of {M.shape[1]} parameters per round, now {n} of {P}")
+        out = torch.empty_like(stack)
+        ops.momentum_mix([ops.momentum_job(out, stack, P, P, list(range(n)), ref, M, P, self.momentum, first)])
+        self._momentum_rows[net] = out
         return out
 
     def _whole_messages(self):
@@ -157,8 +187,10 @@ class RPBCAC_agent():
         dev = model.flat.device
         round = self._consensus_calls[net]
         self._consensus_calls[net] += 1
-        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]),
-                                                       net, round)
+        stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
+        if self.momentum is not None:                 # against the net before this round's consensus overwrites it
+            stack = self._momentum_step(stack, model.flat, net)
+        stack, nodes, H, rule = self._consensus_inputs(stack, net, round)
         ops.consensus_hidden([ops.consensus_job(model.flat, stack, stack.shape[1], nets.n_hidden_params(model.d_in_k),
                                                 nodes, H, rule)])
 
@@ -173,8 +205,14 @@ class RPBCAC_agent():
         # the round of the last hidden consensus of this net: both see the same buckets, as in one Trainer epoch
         rows, kind, xf = A.rows_for(x, self.n_agents)
         dev = xf.device
-        stack, nodes, H, rule = self._consensus_inputs(torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes]),
-                                                       net, max(self._consensus_calls[net] - 1, 0))
+        if self.momentum is None:
+            stack = torch.stack([A.as_flat(m, dev, model.d_in_k) for m in msgs_innodes])
+        elif self._momentum_rows[net] is None:
+            raise L.RcmarlError("an agent with momentum takes its momentum step at the hidden consensus call: call "
+                                "resilient_consensus_*_hidden first")
+        else:                                         # the momentum rows of this round's hidden call
+            stack = self._momentum_rows[net]
+        stack, nodes, H, rule = self._consensus_inputs(stack, net, max(self._consensus_calls[net] - 1, 0))
         agg = torch.empty(xf.shape[0], dtype=torch.float32, device=dev)
         ops.team(rows, [ops.team_job(model.flat, kind, stack, stack.shape[1], nodes, H, agg_out=agg, rule=rule)])
         return Tensor(agg.reshape(-1, 1))

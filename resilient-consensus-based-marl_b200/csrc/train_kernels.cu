@@ -30,7 +30,9 @@
 //
 // Reference semantics: agents/resilient_CAC_agents.py, agents/adversarial_CAC_agents.py,
 // training/train_agents.py:86-163 (cited per entry point in include/rcmarl.h).
+#include <algorithm>
 #include <cmath>
+#include <utility>
 #include "common.cuh"
 #include "grad_kernel.cuh"
 #include "comm.cuh"
@@ -1453,6 +1455,27 @@ __global__ void __launch_bounds__(256) dissensus_attack_kernel(const __grid_cons
     job.dst[i] = c == 0.f ? x : fmaf(-c, delta, x);
 }
 
+// Per-neighbour momentum (rcmarl_momentum_mix, include/rcmarl.h): one thread per coordinate, blockIdx.z the slot.  Every
+// operation is rounded on its own (__f*_rn), so no FMA is contracted and an fp32 NumPy restatement matches bitwise.
+struct MomentumParams { rcmarl_momentum_job jobs[RCMARL_MAX_JOBS]; };
+__global__ void __launch_bounds__(256) momentum_mix_kernel(const __grid_constant__ MomentumParams P) {
+    const rcmarl_momentum_job& job = P.jobs[blockIdx.y];
+    const int k = blockIdx.z;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= job.n_in || i >= job.n) return;
+    const float c = __ldg(job.ref + i);
+    const float u = __fsub_rn(__ldg(job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride + i), c);
+    float* m = job.momentum + (int64_t)k * job.momentum_stride + i;
+    float v = u;
+    if (!job.first) {
+        const float old = *m;
+        if (isinf(old)) v = old;
+        else if (isfinite(u)) v = __fadd_rn(__fmul_rn(job.beta, old), __fmul_rn(__fsub_rn(1.f, job.beta), u));
+    }
+    *m = v;
+    job.dst[(int64_t)k * job.msg_stride + i] = __fadd_rn(c, v);
+}
+
 // Mimic messages (rcmarl_mimic_attack, include/rcmarl.h): one CTA of 256 threads per job.  The honest rows are staged
 // in shared memory and centred in place (mu as attack_kernel), next to mu, z and u.  Every sum over p is taken by ONE
 // warp (warp_dot), so its value does not depend on which warp takes it; the per-row sums are spread over the warps, the
@@ -2297,6 +2320,68 @@ int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs, int n_jobs, void* stream) {
     }
     if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
     bucket_mix_kernel<<<n_jobs, VEC_THREADS, 0, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+// writes_overlap for the many ranges of rcmarl_momentum_mix (up to 1024 written, 544 read): the written ranges sorted by
+// start, so the check takes O((n_w + n_r) log n_w) comparisons instead of one per pair
+static bool sorted_writes_overlap(const uintptr_t* w0, const uintptr_t* w1, int n_w, const uintptr_t* r0,
+                                  const uintptr_t* r1, int n_r) {
+    std::pair<uintptr_t, uintptr_t> w[2 * RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
+    for (int a = 0; a < n_w; ++a) w[a] = {w0[a], w1[a]};
+    std::sort(w, w + n_w);
+    for (int a = 0; a + 1 < n_w; ++a)
+        if (w[a].second > w[a + 1].first) return true;
+    // the written ranges are now disjoint and sorted by start, hence by end too: of them only the first one that ends
+    // after r0 can overlap [r0, r1)
+    for (int r = 0; r < n_r; ++r) {
+        const auto* it = std::upper_bound(w, w + n_w, r0[r], [](uintptr_t x, const std::pair<uintptr_t, uintptr_t>& q) {
+            return x < q.second;
+        });
+        if (it != w + n_w && it->first < r1[r]) return true;
+    }
+    return false;
+}
+
+int rcmarl_momentum_mix(const rcmarl_momentum_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    MomentumParams P;
+    int maxn = 0, max_in = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_momentum_job& q = jobs[j];
+        if (!q.dst || !q.msgs || !q.ref || !q.momentum || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS)
+            return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (!std::isfinite(q.beta) || q.beta < 0.f || q.beta >= 1.f || (q.first != 0 && q.first != 1))
+            return RCMARL_ERR_ARG;
+        P.jobs[j] = q;
+        if (q.n > maxn) maxn = q.n;
+        if (q.n_in > max_in) max_in = q.n_in;
+    }
+    // a thread reads its coordinate of x_k, c and M_k before it writes M_k and row k, but other CTAs run concurrently:
+    // no written range (a dst row, an M row) may overlap an in-node row or a ref of any job of the launch or another
+    // written range, and no ref may overlap an in-node row
+    constexpr int MAX_W = 2 * RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS, MAX_R = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1);
+    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R], c0[RCMARL_MAX_JOBS], c1[RCMARL_MAX_JOBS];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_momentum_job& q = jobs[j];
+        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
+        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.momentum, k, q.momentum_stride, q.n, w0[n_w], w1[n_w]);
+        for (int k = 0; k < q.n_in; ++k, ++n_r) float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+        float_range(q.ref, 0, 0, q.n, c0[j], c1[j]);
+    }
+    for (int j = 0; j < n_jobs; ++j)
+        for (int r = 0; r < n_r; ++r)
+            if (c0[j] < r1[r] && r0[r] < c1[j]) return RCMARL_ERR_ARG;
+    for (int j = 0; j < n_jobs; ++j, ++n_r) {
+        r0[n_r] = c0[j];
+        r1[n_r] = c1[j];
+    }
+    if (sorted_writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    momentum_mix_kernel<<<dim3((maxn + 255) / 256, n_jobs, max_in), 256, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

@@ -55,6 +55,7 @@ NNM_MAX_FLOATS = 48 * 1024
 MIX_BUCKET = 1                                    # rcmarl_mixing_rule: randomized bucketing, ("bucket", s)
 BUCKET_DEFAULT_S = 2                              # the bucket size of a plain "bucket" entry
 BUCKET_MAX_S = 2 ** 31 - 1
+MIX_MOMENTUM = 2                                  # rcmarl_mixing_rule: per-neighbour momentum at beta, 0 <= beta < 1
 # pipeline-aware attacks (rcmarl_pipeline_attack): rcmarl_pipeline_mixing, the staging bound, the most shuffle samples
 # and the samples the trainer draws; the names are PIPELINE_ATTACKS
 PIPE_NONE, PIPE_NNM, PIPE_BUCKET = 0, 1, 2
@@ -124,6 +125,12 @@ class BucketJob(C.Structure):
                 ("receiver", C.c_uint32), ("net", C.c_uint32), ("round", C.c_uint32), ("epoch", C.c_uint32)]
 
 
+class MomentumJob(C.Structure):
+    _fields_ = [("dst", c_fp), ("msgs", c_fp), ("msg_stride", C.c_int64), ("ref", c_fp), ("momentum", c_fp),
+                ("momentum_stride", C.c_int64), ("n", C.c_int32), ("n_in", C.c_int32),
+                ("in_nodes", C.c_int32 * MAX_NEIGHBOURS), ("beta", C.c_float), ("first", C.c_int32)]
+
+
 class ValueJob(C.Structure):
     _fields_ = [("w", c_fp * MAX_TERMS), ("kind", C.c_int32 * MAX_TERMS), ("scale", C.c_float * MAX_TERMS),
                 ("n_terms", C.c_int32), ("n_out", C.c_int32), ("softmax", C.c_int32), ("add_off", C.c_int32),
@@ -182,6 +189,7 @@ SYMBOLS = [
     ("rcmarl_subset_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
+    ("rcmarl_momentum_mix", C.c_int, [C.POINTER(MomentumJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, c_fp]),
@@ -348,6 +356,17 @@ def mixed_rows(mixing, n_in):
     if entry is None or entry == "nnm":
         return n_in
     return 1 + -(-(n_in - 1) // entry[1])
+
+
+def check_momentum(beta):
+    """Raise RcmarlError unless beta is a real number that rcmarl_momentum_mix accepts (include/rcmarl.h): finite, in
+    [0, 1) once rounded to fp32.  Returns it as a float."""
+    if isinstance(beta, bool) or not isinstance(beta, numbers.Real):
+        raise RcmarlError(f"momentum needs a real beta in [0, 1), got {beta!r}")
+    b = float(C.c_float(float(beta)).value)
+    if not (math.isfinite(b) and 0.0 <= b < 1.0):
+        raise RcmarlError(f"momentum needs a real beta in [0, 1), got {beta!r}")
+    return float(beta)
 
 
 def is_adaptive_attack(name):

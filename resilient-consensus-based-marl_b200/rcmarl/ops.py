@@ -470,6 +470,28 @@ def nnm_mix(jobs):
     L.check(L.lib().rcmarl_nnm_mix(a, len(a), _stream()), "rcmarl_nnm_mix")
 
 
+def momentum_job(dst, msgs, msg_stride, n, in_nodes, ref, momentum, momentum_stride, beta, first):
+    """rcmarl_momentum_job: in_nodes the receiver's message rows (own first); ref the reference c [>= n]; momentum the
+    state M, row k at momentum + k * momentum_stride; beta in [0, 1); first 1 for the slots' first step
+    (include/rcmarl.h).  Limits are checked by the library."""
+    j = L.MomentumJob()
+    j.dst, j.msgs, j.msg_stride, j.n = dst.data_ptr(), msgs.data_ptr(), msg_stride, n
+    j.ref, j.momentum, j.momentum_stride = ref.data_ptr(), momentum.data_ptr(), momentum_stride
+    j.n_in = len(in_nodes)
+    for k, v in enumerate(in_nodes[:L.MAX_NEIGHBOURS]):
+        j.in_nodes[k] = v
+    j.beta, j.first = beta, int(first)
+    j._keep = (dst, msgs, ref, momentum)
+    return j
+
+
+def momentum_mix(jobs):
+    """rcmarl_momentum_mix over momentum_job jobs: row k of the n_in output rows goes to dst + k * msg_stride, and M
+    is updated in place."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.MomentumJob, jobs)
+    L.check(L.lib().rcmarl_momentum_mix(a, len(a), _stream()), "rcmarl_momentum_mix")
+
+
 def reward_mix(r, agents, out=None, scale=1.0):
     """r: [rows, n_agents]; out[row] = scale * sum_k r[row, agents[k]] / len(agents) in list order."""
     n_rows, n_agents = r.shape

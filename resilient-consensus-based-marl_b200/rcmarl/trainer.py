@@ -29,7 +29,7 @@ class Trainer:
                  common_reward=False, mu=0.1, seed=0, device=None, rank=0, world=1, group=None,
                  perm_source=None, local_steps=5, mb_epochs=10, mb_times=32, actor_mb_times=200,
                  capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip",
-                 attack=None, mixing=None):
+                 attack=None, mixing=None, momentum=None):
         L.lib()
         # Any team size up to 16 (main.py:26): the kernels are instantiated for 5 and 16 agents, a team of n_real agents
         # runs on the next instantiation with the extra agent slots zero (inputs and W1 rows, rcmarl/nets.py) -- exactly the
@@ -105,7 +105,28 @@ class Trainer:
                                             f"{self.mixing[i]!r}): {ex}") from None
             else:                                  # only cooperative agents aggregate: the name alone is checked
                 L.check_mixing(mix[i], 0, 1)
+        # Per-neighbour momentum (rcmarl_momentum_mix) before a cooperative agent's rule, which then reads n_in momentum
+        # rows, one per slot, with the same H: None, one beta for every agent or one entry per agent
+        mom = [momentum] * n_real if momentum is None or np.isscalar(momentum) else list(momentum)
+        if len(mom) != n_real:
+            raise L.RcmarlError("momentum must be None, one beta or one entry per agent")
+        self.momentum = [None] * NA
+        for i in range(n_real):
+            if mom[i] is None:
+                continue
+            beta = L.check_momentum(mom[i])
+            if i not in self.coop:                 # only cooperative agents aggregate: beta alone is checked
+                continue
+            if self.mixing[i] is not None:
+                raise L.RcmarlError(f"agent {i} takes both momentum and mixing {self.mixing[i]!r}: at most one "
+                                    "pre-aggregation step per agent")
+            self.momentum[i] = beta
         self._init_attacks(attack)
+        for e in self.tailor_pairs + self.pipe_pairs:   # neither attack models the receiver's history
+            b, j, _ = self.byz_pairs[e]
+            if self.momentum[j] is not None:
+                raise L.RcmarlError(f"Byzantine agent {b} runs a {'tailored' if e in self.tailor_pairs else 'pipeline'} "
+                                    f"attack against agent {j}, whose momentum the attack does not model")
         for e in self.tailor_pairs:                # rcmarl_tailored_attack models neither the DnC rule nor mixing
             b, j, _ = self.byz_pairs[e]
             if self.dnc[j]:
@@ -136,6 +157,12 @@ class Trainer:
         for i in self.mix_agents:
             self.mix_row[i] = row
             row += L.mixed_rows(self.mixing[i], len(self.in_nodes[i]))
+        # then the momentum rows of each cooperative agent with momentum: slot k's row at mom_row[i] + k
+        self.mom_agents = [i for i in self.coop if self.momentum[i] is not None]
+        self.mom_row = {}
+        for i in self.mom_agents:
+            self.mom_row[i] = row
+            row += len(self.in_nodes[i])
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -167,9 +194,10 @@ class Trainer:
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
         # vec_row[i] / dnc_row[i] / subset_row[i] the aggregate of cooperative agent i's distance-based / dnc / mda or
-        # smea rule; mix_row[i] + k its mixed message k
+        # smea rule; mix_row[i] + k its mixed message k; mom_row[i] + k its momentum row of slot k
         n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + len(self.subset_agents) \
-            + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents)
+            + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents) \
+            + sum(len(self.in_nodes[i]) for i in self.mom_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
@@ -190,6 +218,11 @@ class Trainer:
         self.mimic_target = (torch.zeros(len(self.mimic_pairs), 2, dtype=torch.int32, device=self.dev)
                              if self.mimic_pairs else None)
         self.mimic_steps = [0] * len(self.mimic_pairs)
+        # the momentum state M of each agent with momentum (row q = mom_agents[q]; [q, 0, k, :PC] critic slot k, [q, 1]
+        # TR), and the momentum steps each has taken (host; its first step ignores M)
+        self.momentum_M = (torch.zeros(len(self.mom_agents), 2, L.MAX_NEIGHBOURS, self.PT, **f32)
+                           if self.mom_agents else None)
+        self.momentum_steps = [0] * len(self.mom_agents)
         self.adam_m = torch.zeros(NA, self.PA, **f32)
         self.adam_v = torch.zeros(NA, self.PA, **f32)
         self.adam_t = [0] * NA
@@ -292,7 +325,10 @@ class Trainer:
         return [row.get(k, k) for k in self.in_nodes[j]]
 
     def _rule_nodes(self, j):
-        """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, else _receiver_nodes(j)."""
+        """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, its momentum rows if it has
+        momentum, else _receiver_nodes(j)."""
+        if self.momentum[j] is not None:
+            return list(range(self.mom_row[j], self.mom_row[j] + len(self.in_nodes[j])))
         if self.mixing[j] is None:
             return self._receiver_nodes(j)
         return list(range(self.mix_row[j], self.mix_row[j] + L.mixed_rows(self.mixing[j], len(self.in_nodes[j]))))
@@ -302,7 +338,8 @@ class Trainer:
         its rule gave each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message
         crafted for i) in the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.
         For an agent that mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry
-        is the effective weight w M of each in-neighbour."""
+        is the effective weight w M of each in-neighbour.  For an agent with momentum, entry k is the weight of slot k's
+        momentum row."""
         out = {}
         for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights),
                                 (self.subset_agents, self.subset_weights)):
@@ -649,6 +686,14 @@ class Trainer:
                     mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i),
                                                    self.H[i], L.MIX_NNM, weights_out=self.mix_weights[2 * q + t]))
         mix_jobs = ops.job_array(L.VectorJob, mix_jobs) if mix_jobs else None
+        # the momentum rows of the agents with momentum against their nets after the last consensus step (critic[i] /
+        # tr[i], which Phase I leaves untouched): at most 16 cooperative agents x 2 nets, so one launch per epoch
+        mom_jobs = []
+        for q, i in enumerate(self.mom_agents):
+            for t, (msgs, P, ref) in enumerate(((self.msg_c, self.PC, self.critic[i]), (self.msg_t, self.PT, self.tr[i]))):
+                mom_jobs.append(ops.momentum_job(msgs[self.mom_row[i]], msgs, P, P, self._receiver_nodes(i), ref,
+                                                 self.momentum_M[q, t], self.PT, self.momentum[i], 0))
+        mom_jobs = ops.job_array(L.MomentumJob, mom_jobs) if mom_jobs else None
         bucket_groups = [ops.job_array(L.BucketJob, bucket_jobs[g:g + L.MAX_JOBS])
                          for g in range(0, len(bucket_jobs), L.MAX_JOBS)]
         # distance-based aggregates over the messages each receiver hears (or their mixed rows): at most 16
@@ -729,6 +774,12 @@ class Trainer:
                     job.epoch = epoch
                 ops.bucket_mix(g)
                 self.launches += 1
+            if mom_jobs is not None:                                       # job 2q + t belongs to mom_agents[q]
+                for k, job in enumerate(mom_jobs):
+                    job.first = int(self.momentum_steps[k // 2] == 0)
+                ops.momentum_mix(mom_jobs)
+                self.launches += 1
+                self.momentum_steps = [s + 1 for s in self.momentum_steps]
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)
                 self.launches += 1
@@ -847,6 +898,8 @@ class Trainer:
             sd.update(sa=self.sa[:T].cpu(), ns=self.ns[:T].cpu(), r=self.r[:T].cpu())
         if self.mimic_pairs:                       # the mimic attack's state carries over between rounds
             sd.update(mimic_z=self.mimic_z.cpu(), mimic_steps=list(self.mimic_steps))
+        if getattr(self, "mom_agents", None):      # so does the momentum of the agents with momentum
+            sd.update(momentum_M=self.momentum_M.cpu(), momentum_steps=list(self.momentum_steps))
         return sd
 
     def load_state_dict(self, sd):
@@ -858,6 +911,14 @@ class Trainer:
             if tuple(sd["mimic_z"].shape) != tuple(self.mimic_z.shape) or len(sd["mimic_steps"]) != len(self.mimic_steps):
                 raise L.RcmarlError(f"checkpointed mimic state of shape {tuple(sd['mimic_z'].shape)} does not match "
                                     f"this trainer's {tuple(self.mimic_z.shape)}")
+        mom = getattr(self, "mom_agents", None)    # (state_dict and load_state_dict read only the attributes they need)
+        if mom:
+            if "momentum_M" not in sd or "momentum_steps" not in sd:
+                raise L.RcmarlError("checkpoint holds no momentum state, and this trainer has agents with momentum")
+            if (tuple(sd["momentum_M"].shape) != tuple(self.momentum_M.shape)
+                    or len(sd["momentum_steps"]) != len(self.momentum_steps)):
+                raise L.RcmarlError(f"checkpointed momentum state of shape {tuple(sd['momentum_M'].shape)} does not "
+                                    f"match this trainer's {tuple(self.momentum_M.shape)}")
         for name in ("actor", "critic", "tr", "critic_local", "adam_m", "adam_v"):
             getattr(self, name).copy_(sd[name])
         self.adam_t = [int(t) for t in sd["adam_t"]]
@@ -866,6 +927,9 @@ class Trainer:
         if self.mimic_pairs:
             self.mimic_z.copy_(sd["mimic_z"])
             self.mimic_steps = [int(s) for s in sd["mimic_steps"]]
+        if mom:
+            self.momentum_M.copy_(sd["momentum_M"])
+            self.momentum_steps = [int(s) for s in sd["momentum_steps"]]
         self.t_filled = 0
         if "sa" in sd:
             T = int(sd["t_filled"]) * self.N

@@ -42,6 +42,7 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
     aggregation = [getattr(ag, 'aggregation', 'clip') for ag in agents]
     attack = [getattr(ag, 'attack', None) for ag in agents]                # Byzantine_CAC_agent
     mixing = [getattr(ag, 'mixing', None) for ag in agents]                # RPBCAC_agent: None, "nnm" or ("bucket", s)
+    momentum = [getattr(ag, 'momentum', None) for ag in agents]            # RPBCAC_agent: None or beta
     adam = [(ag.adam.m, ag.adam.v, ag.adam.t) if getattr(ag, 'adam', None) is not None and ag.adam.m is not None else None
             for ag in agents]
     rank, world = _dist_info()
@@ -52,7 +53,8 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
               n_envs=getattr(env, 'n_envs', 1), nrow=env.nrow, ncol=env.ncol, gamma=args['gamma'], H=H, fast_lr=fast, slow_lr=slow_lr, max_ep_len=args['max_ep_len'],
               n_ep_fixed=args['n_ep_fixed'], n_epochs=args['n_epochs'], buffer_size=args['buffer_size'],
               common_reward=bool(args['common_reward']), seed=int(args.get('random_seed', 0)), adam_state=adam,
-              rank=rank, world=world, aggregation=aggregation, attack=attack, mixing=mixing)
+              rank=rank, world=world, aggregation=aggregation, attack=attack, mixing=mixing,
+              momentum=momentum)
     kw.update(overrides)
     tr = Trainer(**kw)
     if exp_buffer:                                                             # :36-40

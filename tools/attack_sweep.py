@@ -17,7 +17,10 @@ messages it hears by nearest-neighbour mixing (rcmarl_nnm_mix) before its rule, 
 whole-message rule is the effective weight w M of agent 4's message.  Likewise bucket+<rule> (s = 2) or
 bucket<s>+<rule> (e.g. bucket3+gmed) buckets the messages (rcmarl_bucket_mix) before the rule, which then reads the own
 row and ceil(3 / s) bucket means at C2; a rule that refuses that many rows at H = 1 (krum, mkrum at s = 2) is marked
-refused.  The tailored attacks do not model mixing either; the pipeline-aware attacks (rcmarl_pipeline_attack:
+refused.  A rule may also be written m<beta>+<rule> (e.g. m0.9+scclip): every cooperative agent then keeps per-neighbour
+momentum at beta (rcmarl_momentum_mix) and its rule reads the momentum rows, one per in-neighbour; the weight reported
+for a whole-message rule is the weight of agent 4's momentum row.  The tailored attacks do not model mixing or momentum
+either, and the pipeline-aware attacks do not model momentum: those cells are marked refused; the pipeline-aware attacks (rcmarl_pipeline_attack:
 pipeline_uv, pipeline_std, pipeline_sgn, range multiplier 2 by default) model the receiver's mixing step and every rule,
 dnc included, but not mda or smea, whose cells are marked refused (their gamma is reported as the tailored attacks').
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
@@ -62,9 +65,18 @@ out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_ou
 RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
 
 
+def split_momentum(rule):
+    """(beta, the rest) of a rule name: "m0.9+scclip" -> (0.9, "scclip"), "scclip" -> (None, "scclip")."""
+    if rule.startswith("m") and "+" in rule and rule[1:2].isdigit():
+        beta, rest = rule[1:].split("+", 1)
+        return float(beta), rest
+    return None, rule
+
+
 def split_rule(rule):
     """(mixing, aggregation rule) of a rule name: "nnm+mkrum" -> ("nnm", "mkrum"), "bucket+gmed" -> (("bucket", 2),
-    "gmed"), "bucket3+gmed" -> (("bucket", 3), "gmed"), "mkrum" -> (None, "mkrum")."""
+    "gmed"), "bucket3+gmed" -> (("bucket", 3), "gmed"), "mkrum" -> (None, "mkrum"); a momentum prefix is dropped."""
+    rule = split_momentum(rule)[1]
     if rule.startswith("nnm+"):
         return "nnm", rule[4:]
     if rule.startswith("bucket") and "+" in rule:
@@ -255,7 +267,7 @@ for rule in RULES:
             try:
                 tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
                              desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=base,
-                             attack=attack, mixing=mixing, **bench.HYPER)
+                             attack=attack, mixing=mixing, momentum=split_momentum(rule)[0], **bench.HYPER)
             except RcmarlError as ex:                   # e.g. a tailored attack against dnc, mda or mixing
                 refused = str(ex)
                 break

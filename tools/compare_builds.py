@@ -1,7 +1,7 @@
 """Compare the outputs of the distance-based rules (rcmarl_vector_aggregate), the min-max / min-sum attacks
 (rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
-(rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack) and the subset-selection rules MDA / SMEA
-(rcmarl_subset_aggregate) between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with
+(rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack), the subset-selection rules MDA / SMEA
+(rcmarl_subset_aggregate) and per-neighbour momentum (rcmarl_momentum_mix) between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with
 tailored_attack_kernel and pipeline_attack_kernel (vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows,
 bucket_draw / bucket_means and the candidate search in csrc/train_kernels.cu), so a change there may change their
 register allocation and SASS; this shows whether it changed anything they compute.
@@ -10,8 +10,9 @@ Each build runs in its own process (RCMARL_LIB selects the library) on the same 
 around a common centre, four of them 1e3 times larger and one holding 1e30; every vector rule at n_in 1 .. 16 (H drawn
 per job, repeated in-nodes) with the weights, every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
 gamma), DnC, nnm and bucketing (s = 1, 2, 3) at n_in 1 .. 16 with their weights or mixing matrices, and every tailored
-attack x rule at n_in 2 .. 16 (scale 2, with gamma), and MDA and SMEA at n_in 1 .. 16 (H drawn per job, with the
-weights), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a
+attack x rule at n_in 2 .. 16 (scale 2, with gamma), MDA and SMEA at n_in 1 .. 16 (H drawn per job, with the
+weights), and momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), at the trainer's
+parameter counts.  Entry points a build does not export are skipped when loading it, so a
 build from before rcmarl_tailored_attack existed loads too; the outputs of an entry point only one build exports are
 listed and not compared.
 
@@ -115,6 +116,18 @@ if hasattr(lib, "rcmarl_subset_aggregate"):
             dsts.append(d)
         ops.subset_aggregate(jobs)
         named.update({f"subset_{rule}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
+if hasattr(lib, "rcmarl_momentum_mix"):
+    wide = torch.full((24, P + 256), float("nan"), device="cuda")
+    wide[:, :P] = msgs
+    ref = msgs[0] * 0.5
+    Ms = [torch.full((16, P), float("nan"), device="cuda") for _ in range(16)]
+    nodes = [[int(x) for x in rs.choice(24, size=n_in)] for n_in in range(1, 17)]
+    for step in range(3):
+        dsts = [torch.full((16, P + 256), float("nan"), device="cuda") for _ in range(16)]
+        ops.momentum_mix([ops.momentum_job(dsts[q], wide, P + 256, PC[(q + 1) % 4], nodes[q], ref, Ms[q], P, 0.9,
+                                           int(step == 0)) for q in range(16)])
+        named.update({f"momentum_{step}_{q}": np.concatenate([dsts[q].cpu().numpy().ravel(), Ms[q].cpu().numpy().ravel()])
+                      for q in range(16)})
 np.savez(sys.argv[1], *outs, **named)
 '''
 
@@ -136,7 +149,7 @@ def main():
     only = sorted(set(a.files) ^ set(b.files))
     diff = [k for k in common if a[k].tobytes() != b[k].tobytes()]
     print(f"{len(common)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix, "
-          "tailored_attack and subset_aggregate outputs): "
+          "tailored_attack, subset_aggregate and momentum_mix outputs): "
           + ("bitwise equal" if not diff else f"{len(diff)} differ: {diff[:8]}")
           + (f"; {len(only)} from an entry point only one build exports, not compared" if only else ""))
     sys.exit(1 if diff or not common else 0)
