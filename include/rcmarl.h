@@ -96,7 +96,9 @@ int rcmarl_grad_tile_map(int d_in, int n_out, int32_t* info, int32_t* params, in
  * K4 / C5.  Coordinate-wise clipped ("winsorised") mean over the neighbour axis,
  * own value = row 0.  Replaces tf.sort/minimum/maximum/clip_by_value/reduce_mean
  * in RPBCAC_agent._resilient_aggregation (agents/resilient_CAC_agents.py:42-58).
- * vals: [n][P] with row stride `row_stride` floats; out: [P].  One streaming read. */
+ * vals: [n][P] with row stride `row_stride` floats; out: [P].  One streaming read.  Refused (RCMARL_ERR_ARG, nothing
+ * launched, out untouched): a null vals or out, n < 1, P < 0, row_stride < P, H outside 0..RCMARL_MAX_H, H >= n.
+ * P == 0 launches nothing and returns RCMARL_OK. */
 int rcmarl_clip_mean(const float* vals, int n, int64_t P, int64_t row_stride, int H,
                      float* out, void* stream);
 
@@ -117,7 +119,9 @@ typedef enum { RCMARL_AGG_CLIP = 0, RCMARL_AGG_TRIM = 1, RCMARL_AGG_WMSR = 2 } r
  * Replaces resilient_consensus_critic_hidden / _TR_hidden
  * (agents/resilient_CAC_agents.py:142-166) incl. the neighbour gather at
  * training/train_agents.py:129-130.  The output layer of dst is left untouched (:153).
- * An unknown rule or an H the rule does not allow is refused (RCMARL_ERR_ARG) before anything is launched. */
+ * Refused (RCMARL_ERR_ARG, nothing launched, every dst untouched): a null jobs, n_jobs outside 1..RCMARL_MAX_JOBS, a
+ * null dst or msgs, n_hidden < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, H outside [0, n_in), an
+ * unknown rule, TRIM with 2H >= n_in. */
 typedef struct {
     float* dst;                 /* the agent's own network (packed) */
     const float* msgs;          /* base of the message stack [n_agents][msg_stride] */
@@ -737,7 +741,12 @@ int rcmarl_adam_apply(const rcmarl_adam_job* jobs_host, int n_jobs, void* stream
  * so that theta_out += sums / B reproduces train_on_batch with sample weights
  * 1/(2 lr (||phi||^2+1)).  Replaces resilient_consensus_critic/_TR and
  * critic_update_team/TR_update_team (agents/resilient_CAC_agents.py:60-84,168-206).
- * agg_out (optional) stores agg per absolute row; agg_in (optional) supplies it instead (msgs, n_in, H, rule unused). */
+ * agg_out (optional) stores agg per absolute row; agg_in (optional) supplies it instead (msgs, n_in, H, rule unused).
+ * Refused (RCMARL_ERR_ARG, nothing launched, every sums and agg_out untouched): a null rows, sa, ns or r, n_rows < 0,
+ * n_envs < 1, n_agents other than 5 and 16, a time_idx with n_rows not a multiple of n_envs, a null jobs, n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null w, an unknown kind, a job with neither sums nor agg_out; for a job without agg_in also a
+ * null msgs, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, H outside [0, n_in), an unknown rule, TRIM with
+ * 2H >= n_in.  A job with sums and a null or too small ws gives RCMARL_ERR_WORKSPACE. */
 typedef struct {
     const float* w;             /* agent's network: aggregated hidden + current own head */
     const float* msgs;          /* message stack base (heads are read at the W3/b3 offsets) */

@@ -2020,6 +2020,8 @@ int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs
         if (!q.w || q.kind < 0 || q.kind > 2) return RCMARL_ERR_ARG;
         if (!q.agg_in) {
             if (!q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+            for (int k = 0; k < q.n_in; ++k)
+                if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
             if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         }
         if (!q.sums && !q.agg_out) return RCMARL_ERR_ARG;
@@ -2072,6 +2074,8 @@ int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs, int n_jobs, void* 
         const rcmarl_consensus_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in || q.n_hidden < 1)
             return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
         if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         P.jobs[j] = q;
         if (q.n_hidden > maxn) maxn = q.n_hidden;
