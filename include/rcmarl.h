@@ -626,6 +626,64 @@ typedef struct {
 } rcmarl_pipeline_attack_job;
 int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* Momentum-aware Byzantine messages (rcmarl_history_attack): the pipeline attack without mixing, run in the momentum-row
+ * space of a receiver j with per-neighbour momentum (rcmarl_momentum_mix), then inverted through j's momentum step.
+ * Threat model: that of rcmarl_pipeline_attack, plus j's momentum: the attacker knows beta, j's reference net c, its
+ * state M and whether this is its first step -- functions of messages an omniscient attacker has already seen.  The
+ * attack is greedy per epoch; it does not plan across epochs.  One job is one (attacker, receiver j, net); `attack`
+ * holds the fields of rcmarl_tailored_attack_job with their meaning there.  All arithmetic is fp32 (DnC's centring and
+ * eigen-solve fp64, as in rcmarl_dnc_aggregate); every operation marked (+) (-) (*) (/) is rounded on its own, no FMA.
+ *   Step.    step_k(x) is rcmarl_momentum_mix's arithmetic for slot k (the same device code): u = x (-) c, M'_k = u if
+ *            first or where M_k is finite and u is not, M_k where M_k is +-inf, beta (*) M_k (+) (1 (-) beta) (*) u
+ *            elsewhere; step_k(x) = c (+) M'_k.  M is read only when first = 0.
+ *   Rows.    A real slot k has the row r_k = step_k(x_k) of its message x_k.  mu, d and gamma_mm are those of
+ *            rcmarl_tailored_attack (the same device code and summation orders) over the honest slots' rows r_k in slot
+ *            order (repeats count), and so are Gamma = scale * gamma_mm, the K + 1 candidates gamma_i and the targets
+ *            t_i = m(gamma_i).
+ *   Inversion.  The message that puts slot k's row at t: inv_k(t)_p = t_p if first or M_k,p is +-inf, else
+ *              c_p (+) (((t_p (-) c_p) (-) (beta (*) M_k,p)) (/) (1 (-) beta)).
+ *            The own slots (own_mask) all receive inv_k0(t_i), k0 the lowest own slot; every other crafted slot k is a
+ *            colluder, modelled as sending inv_k(t_i) with its own state.  Crafted slot k's modelled row is
+ *            a_k = step_k(the message it receives): the row j computes, not t_i.  A candidate is infeasible if one of
+ *            these crafted messages has a coordinate that is not finite: O_i = -inf.
+ *   Rule.    j's rule reads the n_in rows (r_k of the real slots, a_k of the crafted ones; own = row 0) with H: family
+ *            COORD resilient_mean per coordinate (rcmarl_consensus_hidden's arithmetic), VECTOR exactly
+ *            rcmarl_vector_aggregate's output, SPECTRAL (rule RCMARL_SPECTRAL_DNC) exactly rcmarl_dnc_aggregate's.
+ *   Objective.  O_i = sum_p (R(gamma_i)_p - mu_p)^2 as in rcmarl_tailored_attack (-inf if not finite), against the
+ *            honest rows' mu; i* = argmax_i O_i, ties to the smaller i, i* = 0 if every O_i is -inf.
+ *   Output.  dst[0:n] = inv_k0(t_i*), gamma_out (optional, one float) = gamma_i*, model_out (optional, n floats) =
+ *            R(gamma_i*): the receiver's aggregate as the attacker models it.  momentum and ref are never written.
+ * Exactness: when every colluder occupies one slot of j and runs a job with the same parameters, model_out is bitwise
+ * what j computes from the messages actually sent -- rcmarl_momentum_mix, then rcmarl_consensus_hidden over all n
+ * parameters (COORD; for the hidden layers exact only when j combines its head through rcmarl_team, as for the
+ * tailored attack), rcmarl_vector_aggregate (VECTOR) or rcmarl_dnc_aggregate (SPECTRAL).  With c = 0, first = 1,
+ * inputs free of -0 and finite targets, every row is the raw message and dst, gamma_out and model_out are bitwise those
+ * of rcmarl_pipeline_attack with mixing none.  NaN inputs are not supported.
+ * One CTA per job: the real slots' rows, mu, d, the target, the output row, one row per crafted slot and (DnC) the fp64
+ * mean staged in shared memory; the crafted slots' M rows are read from global memory for each candidate.  Fixed
+ * summation orders, no atomics -- bitwise reproducible, independent of the job order and of how jobs are split over
+ * launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, gamma_out and model_out untouched): everything rcmarl_tailored_attack
+ * refuses (family SPECTRAL with rule RCMARL_SPECTRAL_DNC excepted), a null ref or momentum, a beta that is not finite or
+ * lies outside [0, 1), first other than 0 or 1, an own_mask that is empty or has a bit on a real slot or at or past
+ * n_in, a staging size (n_in + 4 + (DnC ? 2 : 0)) * n above RCMARL_HISTORY_MAX_FLOATS (the bound admits the 16-agent
+ * team-reward net, 1421 parameters, at n_in = 16 under DnC), a written range (dst, gamma_out, model_out) that overlaps
+ * a real slot's row, a ref or one of the n_in M rows of any job of the launch, and two written ranges of the launch
+ * that overlap. */
+#define RCMARL_HISTORY_MAX_FLOATS (22 * 1421)
+typedef struct {
+    rcmarl_tailored_attack_job attack;   /* family COORD, VECTOR or SPECTRAL; slots, H and dev as for the tailored attack */
+    float* model_out;           /* optional [n]: R(gamma_i*), the receiver's aggregate as the attacker models it */
+    const float* ref;           /* [n]: c, the receiver's net after its previous consensus step */
+    const float* momentum;      /* n_in rows at momentum + k * momentum_stride: the receiver's M, read only */
+    int64_t momentum_stride;
+    float beta;                 /* 0 <= beta < 1 */
+    int32_t first;              /* 1: the receiver's first momentum step (M not read) */
+    uint32_t own_mask;          /* bit k: crafted slot k receives this job's dst */
+    int32_t reserved;
+} rcmarl_history_attack_job;
+int rcmarl_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

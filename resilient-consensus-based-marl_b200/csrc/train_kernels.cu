@@ -23,6 +23,8 @@
 //   tailored_attack_kernel  Byzantine messages tuned against the receiver's own rule and H (rcmarl_tailored_attack)
 //   pipeline_attack_kernel  the same search against the receiver's mixing step and rule, DnC included
 //                   (rcmarl_pipeline_attack)
+//   history_attack_kernel  the same search in the momentum rows of a receiver with momentum, inverted through its
+//                   momentum step (rcmarl_history_attack)
 //   dissensus_attack_kernel  Byzantine messages that cancel the receiver's honest pull (rcmarl_dissensus_attack)
 //   mimic_attack_kernel  copies of the honest message furthest along the tracked principal direction
 //                   (rcmarl_mimic_attack)
@@ -1266,11 +1268,10 @@ __device__ __forceinline__ void coord_rule(const Row& row, int n, int nrows, int
     }
 }
 
-// Stage a tailored job's real slots at xs (the honest ones first), point every crafted slot at cand (S.off), and
-// compute mu, d and Gamma = scale * gamma_mm, 0 if that fp32 product is not finite (a huge scale: dst = mu).  Called
-// by the whole CTA; returns Gamma in every thread.
-__device__ __forceinline__ float tailored_setup(const rcmarl_tailored_attack_job& job, int nh, float* xs, float* mu,
-                                                float* d, const float* cand, TailoredShared& S) {
+// Stage a tailored job's real slots at xs (the honest ones first) and point every crafted slot at cand (S.off).  Called
+// by the whole CTA; the caller synchronises before reading the rows.
+__device__ __forceinline__ void tailored_stage(const rcmarl_tailored_attack_job& job, int nh, float* xs, const float* cand,
+                                               TailoredShared& S) {
     const int n = job.n, nin = job.n_in, tid = threadIdx.x;
     if (tid == 0) {
         int h = 0, o = nh;
@@ -1286,12 +1287,26 @@ __device__ __forceinline__ float tailored_setup(const rcmarl_tailored_attack_job
         float* row = xs + S.off[k];
         for (int p = tid; p < n; p += ADA_THREADS) row[p] = __ldg(src + p);
     }
-    __syncthreads();
+}
+
+// mu, d and Gamma = scale * gamma_mm over the nh honest rows at xs, 0 if that fp32 product is not finite (a huge scale:
+// dst = mu).  Called by the whole CTA once the rows are staged; returns Gamma in every thread.
+__device__ __forceinline__ float tailored_range(const rcmarl_tailored_attack_job& job, int nh, const float* xs, float* mu,
+                                                float* d, TailoredShared& S) {
+    const int n = job.n;
     constexpr int kind = RCMARL_ADAPT_MINMAX;
     adaptive_gamma(xs, nh, n, kind, job.dev, mu, d, S.dist, S.ek, S.bk, S.scal, [&](float g) { S.scal[1] = g; });
     __syncthreads();
     const float prod = job.scale * S.scal[1];
     return isfinite(prod) ? prod : 0.f;
+}
+
+// tailored_stage, then tailored_range over the raw messages.  Called by the whole CTA; returns Gamma in every thread.
+__device__ __forceinline__ float tailored_setup(const rcmarl_tailored_attack_job& job, int nh, float* xs, float* mu,
+                                                float* d, const float* cand, TailoredShared& S) {
+    tailored_stage(job, nh, xs, cand, S);
+    __syncthreads();
+    return tailored_range(job, nh, xs, mu, d, S);
 }
 
 // The candidate search: for i = 0 .. K, cand = m(gamma_i), then for each sample q < nq eval(q) writes the modelled
@@ -1458,6 +1473,19 @@ __global__ void __launch_bounds__(256) dissensus_attack_kernel(const __grid_cons
 // Per-neighbour momentum (rcmarl_momentum_mix, include/rcmarl.h): one thread per coordinate, blockIdx.z the slot.  Every
 // operation is rounded on its own (__f*_rn), so no FMA is contracted and an fp32 NumPy restatement matches bitwise.
 struct MomentumParams { rcmarl_momentum_job jobs[RCMARL_MAX_JOBS]; };
+
+// One coordinate of one slot's momentum step: M' at u = x - c, the old M at *m (read only when !first).  Shared by
+// momentum_mix_kernel and history_attack_kernel, so that the attacker's model is the receiver's arithmetic.
+__device__ __forceinline__ float momentum_next(float u, const float* m, float beta, int first) {
+    float v = u;
+    if (!first) {
+        const float old = *m;
+        if (isinf(old)) v = old;
+        else if (isfinite(u)) v = __fadd_rn(__fmul_rn(beta, old), __fmul_rn(__fsub_rn(1.f, beta), u));
+    }
+    return v;
+}
+
 __global__ void __launch_bounds__(256) momentum_mix_kernel(const __grid_constant__ MomentumParams P) {
     const rcmarl_momentum_job& job = P.jobs[blockIdx.y];
     const int k = blockIdx.z;
@@ -1466,14 +1494,111 @@ __global__ void __launch_bounds__(256) momentum_mix_kernel(const __grid_constant
     const float c = __ldg(job.ref + i);
     const float u = __fsub_rn(__ldg(job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride + i), c);
     float* m = job.momentum + (int64_t)k * job.momentum_stride + i;
-    float v = u;
-    if (!job.first) {
-        const float old = *m;
-        if (isinf(old)) v = old;
-        else if (isfinite(u)) v = __fadd_rn(__fmul_rn(job.beta, old), __fmul_rn(__fsub_rn(1.f, job.beta), u));
-    }
+    const float v = momentum_next(u, m, job.beta, job.first);
     *m = v;
     job.dst[(int64_t)k * job.msg_stride + i] = __fadd_rn(c, v);
+}
+
+// Momentum-aware Byzantine messages (rcmarl_history_attack, include/rcmarl.h): pipeline_attack_kernel without mixing,
+// in momentum-row space.  The real slots are staged by tailored_stage and stepped in place before mu, d and gamma_mm
+// are taken; behind mu, d, the target and the output row come one row per crafted slot (colluders' rows differ), and
+// for DnC the fp64 mean sits in front, 8-byte aligned.  A crafted slot's M row is read from global memory for each
+// candidate.
+struct HistoryParams { rcmarl_history_attack_job jobs[RCMARL_MAX_JOBS]; };
+
+// the message that puts a slot's momentum row at t (include/rcmarl.h, Inversion); m is read only when !first
+__device__ __forceinline__ float momentum_invert(float t, float c, const float* m, float beta, int first) {
+    if (first) return t;
+    const float old = *m;
+    if (isinf(old)) return t;
+    return __fadd_rn(c, __fdiv_rn(__fsub_rn(__fsub_rn(t, c), __fmul_rn(beta, old)), __fsub_rn(1.f, beta)));
+}
+
+__global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __grid_constant__ HistoryParams P) {
+    extern __shared__ __align__(16) float smem[];
+    __shared__ TailoredShared S;
+    __shared__ DncShared D;
+    const rcmarl_history_attack_job& hj = P.jobs[blockIdx.x];
+    const rcmarl_tailored_attack_job& job = hj.attack;
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    int nh = 0, nr = 0;                            // honest slots, real slots
+    for (int k = 0; k < nin; ++k) {
+        nh += (job.honest_mask >> k) & 1u;
+        nr += job.slots[k] >= 0 ? 1 : 0;
+    }
+    const int k0 = __ffs(hj.own_mask) - 1;         // the lowest own slot
+    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC: [n]
+    float* xs = smem + (job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
+    float* mu = xs + (int64_t)nr * n;              // [n]
+    float* d = mu + n;                             // [n]
+    float* cand = d + n;                           // [n]: the target t(gamma_i)
+    float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
+    float* crafted = z + n;                        // [n_in - nr][n]: a_k of each crafted slot, in slot order
+    tailored_stage(job, nh, xs, cand, S);
+    if (tid == 0)                                  // each crafted slot to a row of its own
+        for (int k = 0, c = 0; k < nin; ++k)
+            if (job.slots[k] < 0) S.off[k] = (int)(crafted - xs) + n * c++;
+    __syncthreads();
+    const auto Mrow = [&](int k) { return hj.momentum + (int64_t)k * hj.momentum_stride; };
+    for (int k = 0; k < nin; ++k) {                // r_k = step_k(x_k) in place
+        if (job.slots[k] < 0) continue;
+        float* row = xs + S.off[k];
+        const float* m = Mrow(k);
+        for (int p = tid; p < n; p += ADA_THREADS) {
+            const float c = __ldg(hj.ref + p);
+            row[p] = __fadd_rn(c, momentum_next(__fsub_rn(row[p], c), m + p, hj.beta, hj.first));
+        }
+    }
+    __syncthreads();
+    const float range = tailored_range(job, nh, xs, mu, d, S);
+    const SlotRows rows{xs, S.off};
+    // a_k of every crafted slot for the target in cand, then the rule into z; returns whether every crafted message is
+    // finite (the same in every thread).  An infeasible candidate skips the rule unless `always`: its objective is -inf
+    // whatever the rule gives.
+    const auto model = [&](bool always) {
+        bool bad = false;
+        for (int k = 0; k < nin; ++k) {
+            if (job.slots[k] < 0) {
+                float* row = xs + S.off[k];
+                const float* m = Mrow(k);
+                const float* src = Mrow((hj.own_mask >> k) & 1u ? k0 : k);
+                for (int p = tid; p < n; p += ADA_THREADS) {
+                    const float c = __ldg(hj.ref + p);
+                    const float x = momentum_invert(cand[p], c, src + p, hj.beta, hj.first);
+                    bad = bad || !isfinite(x);
+                    row[p] = __fadd_rn(c, momentum_next(__fsub_rn(x, c), m + p, hj.beta, hj.first));
+                }
+            }
+        }
+        const bool ok = !__syncthreads_or(bad);    // the crafted rows complete
+        if (!ok && !always) return false;
+        if (job.family == RCMARL_TAILOR_COORD)
+            coord_rule(rows, n, nin, job.H, job.rule, z);
+        else if (job.family == RCMARL_TAILOR_VECTOR)
+            vector_rule(rows, n, nin, job.H, job.rule, z, z, S.dist, S.wt, S.score, S.total);
+        else
+            dnc_rule(rows, n, nin, job.H, mu64, z, D);
+        return ok;
+    };
+    const int best = tailored_search(mu, d, cand, z, n, range, 1, S, [&](int) {
+        // infeasible: a non-finite objective, O_i = -inf (z is not read before tailored_search's next barrier)
+        if (!model(false) && tid == 0) z[0] = INFINITY;
+    });
+    const float g = range * (float)best / (float)RCMARL_TAILORED_STEPS;
+    if (tid == 0 && job.gamma_out) *job.gamma_out = g;
+    const float* m0 = Mrow(k0);
+    for (int p = tid; p < n; p += ADA_THREADS) {
+        const float t = g == 0.f ? mu[p] : fmaf(g, d[p], mu[p]);
+        job.dst[p] = momentum_invert(t, __ldg(hj.ref + p), m0 + p, hj.beta, hj.first);
+        cand[p] = t;
+    }
+    if (hj.model_out) {                            // R(gamma_i*), the same for every thread of the CTA
+        __syncthreads();
+        model(true);
+        __syncthreads();
+        for (int p = tid; p < n; p += ADA_THREADS) hj.model_out[p] = z[p];
+    }
 }
 
 // Mimic messages (rcmarl_mimic_attack, include/rcmarl.h): one CTA of 256 threads per job.  The honest rows are staged
@@ -2548,6 +2673,53 @@ int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         return e;
     const size_t smem = sizeof(float) * (size_t)max_floats;
     pipeline_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
+int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    HistoryParams P;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_history_attack_job& hj = jobs[j];
+        const rcmarl_tailored_attack_job& q = hj.attack;
+        int n_real = 0;
+        if (bad_tailored_slots(q, n_real) || bad_receiver_rule(q.family, q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
+        if (!hj.ref || !hj.momentum) return RCMARL_ERR_ARG;
+        if (!std::isfinite(hj.beta) || hj.beta < 0.f || hj.beta >= 1.f || (hj.first != 0 && hj.first != 1))
+            return RCMARL_ERR_ARG;
+        if (hj.own_mask == 0u || (hj.own_mask >> q.n_in)) return RCMARL_ERR_ARG;
+        for (int k = 0; k < q.n_in; ++k)
+            if (((hj.own_mask >> k) & 1u) && q.slots[k] >= 0) return RCMARL_ERR_ARG;   // an own bit on a real slot
+        const int64_t floats = (int64_t)(q.n_in + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        if (floats > RCMARL_HISTORY_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = hj;
+    }
+    // as rcmarl_pipeline_attack, with every ref and M row among the read ranges; up to 33 read ranges per job, so the
+    // written ranges are checked by a sorted sweep as in rcmarl_momentum_mix
+    constexpr int MAX_R = RCMARL_MAX_JOBS * (2 * RCMARL_MAX_NEIGHBOURS + 1);
+    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[MAX_R], r1[MAX_R];
+    int n_w = 0, n_r = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_history_attack_job& hj = jobs[j];
+        tailored_ranges(hj.attack, w0, w1, n_w, r0, r1, n_r);
+        if (hj.model_out) {
+            float_range(hj.model_out, 0, 0, hj.attack.n, w0[n_w], w1[n_w]);
+            ++n_w;
+        }
+        float_range(hj.ref, 0, 0, hj.attack.n, r0[n_r], r1[n_r]);
+        ++n_r;
+        for (int k = 0; k < hj.attack.n_in; ++k, ++n_r)
+            float_range(hj.momentum, k, hj.momentum_stride, hj.attack.n, r0[n_r], r1[n_r]);
+    }
+    if (sorted_writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    static bool opted[64] = {};
+    if (int e = opt_in_smem((const void*)history_attack_kernel, (int)(sizeof(float) * RCMARL_HISTORY_MAX_FLOATS), opted))
+        return e;
+    const size_t smem = sizeof(float) * (size_t)max_floats;
+    history_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }

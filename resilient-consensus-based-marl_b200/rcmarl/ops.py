@@ -386,6 +386,37 @@ def pipeline_attack(jobs):
     L.check(L.lib().rcmarl_pipeline_attack(a, len(a), _stream()), "rcmarl_pipeline_attack")
 
 
+def history_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack, scale, ref, momentum, momentum_stride,
+                       beta, first, own, gamma_out=None, model_out=None):
+    """rcmarl_history_attack_job: slots, honest, rule, H and scale as pipeline_attack_job; attack: "history_uv",
+    "history_std", "history_sgn" or an rcmarl_adaptive_dev id; ref the receiver's reference c [>= n]; momentum its state
+    M, row k at momentum + k * momentum_stride (read only); beta in [0, 1); first 1 for the receiver's first step; own:
+    the crafted slot indices that receive dst; model_out [n]: R of the pick.  Names and own slots are checked here, ids
+    and limits by the library."""
+    if isinstance(attack, str):
+        if not L.is_history_attack(attack):
+            raise L.RcmarlError(f"unknown history attack {attack!r}: expected one of {sorted(L.HISTORY_ATTACKS)}")
+        attack = L.HISTORY_ATTACKS[attack]
+    if L.is_spectral_rule(rule):
+        rule = (L.TAILOR_SPECTRAL, L.SPECTRAL_RULES[rule])
+    bad = [k for k in own if not (isinstance(k, (int, np.integer)) and 0 <= k < len(slots))]
+    if bad:
+        raise L.RcmarlError(f"own slot indices {bad} are outside the slot list of {len(slots)}")
+    j = L.HistoryAttackJob()
+    j.attack = tailored_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, int(attack), scale, gamma_out)
+    j.model_out = ptr(model_out)
+    j.ref, j.momentum, j.momentum_stride = ref.data_ptr(), momentum.data_ptr(), momentum_stride
+    j.beta, j.first = beta, int(first)
+    j.own_mask = sum(1 << int(k) for k in set(own))
+    j._keep = (dst, msgs, gamma_out, model_out, ref, momentum)
+    return j
+
+
+def history_attack(jobs):
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.HistoryAttackJob, jobs)
+    L.check(L.lib().rcmarl_history_attack(a, len(a), _stream()), "rcmarl_history_attack")
+
+
 def dissensus_attack_job(dst, msgs, msg_stride, n, own, honest, n_byz, eps):
     """own: the receiver's message row; honest: the message rows of its honest set in list order; n_byz: the dissensus
     entries of its in_nodes (repeats included); eps >= 0 (include/rcmarl.h).  Limits are checked by the library."""

@@ -135,11 +135,12 @@ class Trainer:
             if self.mixing[j] is not None:
                 raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose mixing "
                                     f"{self.mixing[j]!r} the tailored attack does not model")
-        for e in self.tailor_pairs + self.pipe_pairs:   # neither attack models the subset-selection rules
+        for e in self.tailor_pairs + self.pipe_pairs + self.hist_pairs:   # none models the subset-selection rules
             b, j, _ = self.byz_pairs[e]
             if self.subset_rule[j] is not None:
-                raise L.RcmarlError(f"Byzantine agent {b} runs a {'tailored' if e in self.tailor_pairs else 'pipeline'} "
-                                    f"attack against agent {j}, whose rule {agg[j]!r} the attack does not model")
+                name = 'tailored' if e in self.tailor_pairs else 'pipeline' if e in self.pipe_pairs else 'history'
+                raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose rule "
+                                    f"{agg[j]!r} the attack does not model")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
         # that of each cooperative agent on dnc, then that of each on mda / smea
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
@@ -311,7 +312,11 @@ class Trainer:
         # models the receiver's mixing step and every rule, DnC included: a launch of their own, after the tailored one
         self.pipe_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                            if isinstance(self.attack[b][0], L.PipelineKind)]
-        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs
+        # the pairs whose attacker runs a momentum-aware attack (rcmarl_history_attack, kind L.HistoryKind): against a
+        # receiver with momentum a launch of their own, after the pipeline one; against one without, a pipeline job
+        self.hist_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                           if isinstance(self.attack[b][0], L.HistoryKind)]
+        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs
         # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
         # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
         # tailored one
@@ -372,10 +377,11 @@ class Trainer:
         return out
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored or a pipeline attack: float32 [2]}:
-        the gamma of the message b crafted for j in the last epoch of the last update round (include/rcmarl.h,
-        rcmarl_adaptive_attack; for a tailored or pipeline attack gamma_i*, rcmarl_tailored_attack /
-        rcmarl_pipeline_attack); entry 0 for the critic, 1 for the team-reward net."""
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline or a history attack:
+        float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
+        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline or history attack gamma_i*,
+        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack); entry 0 for the critic, 1 for the
+        team-reward net."""
         if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
@@ -402,6 +408,98 @@ class Trainer:
         slots = [-1 if r >= self.NA else r for r in self._receiver_nodes(j)]
         honest = [k for k, i in enumerate(self.in_nodes[j]) if self.labels[i] == COOP]
         return slots, honest
+
+    def _attack_job_groups(self):
+        """The job tables of the Byzantine messages update_round launches in every epoch, each in groups of MAX_JOBS:
+        (attack, adaptive, tailored, pipeline, history, dissensus, mimic groups), with the history groups and the mimic
+        groups as (index of their first job, group) pairs, hist_mom the momentum agent index of each history job, and
+        mimic_t0 each mimic pair's T0."""
+        NA, lab = self.NA, self.labels
+        # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
+        # (the min-max / min-sum pairs in a job list of their own, with the gamma of each message)
+        # (and the tailored pairs in a third, against their receiver's own rule and H)
+        # (and the pipeline pairs in a fourth, against their receiver's mixing step, rule and H)
+        # (and the history pairs in a fifth, through their receiver's momentum; a history pair whose receiver has no
+        # momentum joins the pipeline pairs with the same direction and scale)
+        # (then the dissensus pairs, and the mimic pairs with their direction states)
+        att_jobs, ada_jobs, tail_jobs, pipe_jobs, hist_jobs, diss_jobs, mimic_jobs = [], [], [], [], [], [], []
+        ada_row = {e: q for q, e in enumerate(self.adapt_pairs)}
+        tail_row = {e: len(self.adapt_pairs) + q for q, e in enumerate(self.tailor_pairs)}
+        pipe_row = {e: len(self.adapt_pairs) + len(self.tailor_pairs) + q for q, e in enumerate(self.pipe_pairs)}
+        n_before = len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs)
+        hist_row = {e: n_before + q for q, e in enumerate(self.hist_pairs)}
+        pipe_row.update({e: r for e, r in hist_row.items() if self.momentum[self.byz_pairs[e][1]] is None})
+        hist_row = {e: r for e, r in hist_row.items() if e not in pipe_row}
+        hist_mom = []                                  # the momentum agent index q of each history job
+        mom_index = {i: q for q, i in enumerate(self.mom_agents)}
+        diss_set = set(self.diss_pairs)
+        mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
+        for e, (b, j, honest) in enumerate(self.byz_pairs):
+            kind, param = self.attack[b]
+            if e in diss_set:
+                # colluding dissensus attackers of j split the cancellation: n_byz counts their entries of in_nodes[j]
+                n_byz = sum(isinstance(self.attack[k][0], L.DissensusKind) for k in self.in_nodes[j]
+                            if lab[k] == BYZANTINE)
+                for msgs, P in ((self.msg_c, self.PC), (self.msg_t, self.PT)):
+                    diss_jobs.append(ops.dissensus_attack_job(msgs[NA + e], msgs, P, P, j, honest, n_byz, param))
+                continue
+            if e in mimic_row:
+                # copying the receiver to itself only slows its consensus: the candidates are S_j without j's own
+                # entries, unless that leaves none
+                q = mimic_row[e]
+                cand = [k for k, i in enumerate(honest) if i != j] or list(range(len(honest)))
+                for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                    mimic_jobs.append(ops.mimic_attack_job(msgs[NA + e], msgs, P, P, honest, cand, self.mimic_z[q, t],
+                                                           0, target_out=self.mimic_target[q, t:t + 1]))
+                continue
+            if e in tail_row or e in pipe_row or e in hist_row:
+                slots, hon = self._tailored_slots(j)
+                rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
+                        else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
+                        else (L.TAILOR_COORD, self.aggregation[j]))
+            if e in hist_row:
+                q = mom_index[j]
+                own = [k for k, i in enumerate(self.in_nodes[j]) if i == b]
+                for t, (msgs, P, ref) in enumerate(((self.msg_c, self.PC, self.critic[j]),
+                                                    (self.msg_t, self.PT, self.tr[j]))):
+                    hist_jobs.append(ops.history_attack_job(
+                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, ref,
+                        self.momentum_M[q, t], self.PT, self.momentum[j], 0, own,
+                        gamma_out=self.att_gamma[hist_row[e], t:t + 1]))
+                    hist_mom.append(q)
+                continue
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                if e in pipe_row:
+                    pipe_jobs.append(ops.pipeline_attack_job(
+                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, mixing=self.mixing[j],
+                        n_perms=L.PIPELINE_PERMS, seed=self.seed, attacker=b, receiver=j, net=t,
+                        round=self.episodes_done & 0xFFFFFFFF, gamma_out=self.att_gamma[pipe_row[e], t:t + 1]))
+                elif e in tail_row:
+                    tail_jobs.append(ops.tailored_attack_job(msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind,
+                                                             param, gamma_out=self.att_gamma[tail_row[e], t:t + 1]))
+                elif e in ada_row:
+                    ada_jobs.append(ops.adaptive_attack_job(msgs[NA + e], msgs, P, P, honest, kind, param,
+                                                            gamma_out=self.att_gamma[ada_row[e], t:t + 1]))
+                else:
+                    att_jobs.append(ops.attack_job(msgs[NA + e], msgs, P, P, honest, kind, param, seed=self.seed,
+                                                   attacker=b, receiver=j, round=self.episodes_done & 0xFFFFFFFF))
+        att_groups = [ops.job_array(L.AttackJob, att_jobs[g:g + L.MAX_JOBS]) for g in range(0, len(att_jobs), L.MAX_JOBS)]
+        ada_groups = [ops.job_array(L.AdaptiveAttackJob, ada_jobs[g:g + L.MAX_JOBS])
+                      for g in range(0, len(ada_jobs), L.MAX_JOBS)]
+        tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(tail_jobs), L.MAX_JOBS)]
+        pipe_groups = [ops.job_array(L.PipelineAttackJob, pipe_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(pipe_jobs), L.MAX_JOBS)]
+        hist_groups = [(g, ops.job_array(L.HistoryAttackJob, hist_jobs[g:g + L.MAX_JOBS]))
+                       for g in range(0, len(hist_jobs), L.MAX_JOBS)]
+        diss_groups = [ops.job_array(L.DissensusJob, diss_jobs[g:g + L.MAX_JOBS])
+                       for g in range(0, len(diss_jobs), L.MAX_JOBS)]
+        # mimic job 2q + t belongs to pair mimic_pairs[q]; its T0 is the attacker's parameter
+        mimic_t0 = [int(self.attack[self.byz_pairs[e][0]][1]) for e in self.mimic_pairs]
+        mimic_groups = [(g, ops.job_array(L.MimicJob, mimic_jobs[g:g + L.MAX_JOBS]))
+                        for g in range(0, len(mimic_jobs), L.MAX_JOBS)]
+        return (att_groups, ada_groups, tail_groups, pipe_groups, hist_groups, hist_mom, diss_groups, mimic_t0,
+                mimic_groups)
 
     def _try_peer_comm(self):
         """Set up the peer-memory exchange on every rank, or on none: the ranks agree (MIN all-reduce of a success
@@ -607,68 +705,9 @@ class Trainer:
         cons_jobs, team_jobs = ops.job_array(L.ConsensusJob, cons_jobs), ops.job_array(L.TeamJob, team_jobs)
         team_apply = ops.job_array(L.SgdJob, team_apply)
 
-        # Byzantine messages: per (attacker, receiver) pair one critic and one TR job, crafted anew in every epoch
-        # (the min-max / min-sum pairs in a job list of their own, with the gamma of each message)
-        # (and the tailored pairs in a third, against their receiver's own rule and H)
-        # (and the pipeline pairs in a fourth, against their receiver's mixing step, rule and H)
-        # (then the dissensus pairs, and the mimic pairs with their direction states)
-        att_jobs, ada_jobs, tail_jobs, pipe_jobs, diss_jobs, mimic_jobs = [], [], [], [], [], []
-        ada_row = {e: q for q, e in enumerate(self.adapt_pairs)}
-        tail_row = {e: len(self.adapt_pairs) + q for q, e in enumerate(self.tailor_pairs)}
-        pipe_row = {e: len(self.adapt_pairs) + len(self.tailor_pairs) + q for q, e in enumerate(self.pipe_pairs)}
-        diss_set = set(self.diss_pairs)
-        mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
-        for e, (b, j, honest) in enumerate(self.byz_pairs):
-            kind, param = self.attack[b]
-            if e in diss_set:
-                # colluding dissensus attackers of j split the cancellation: n_byz counts their entries of in_nodes[j]
-                n_byz = sum(isinstance(self.attack[k][0], L.DissensusKind) for k in self.in_nodes[j]
-                            if lab[k] == BYZANTINE)
-                for msgs, P in ((self.msg_c, self.PC), (self.msg_t, self.PT)):
-                    diss_jobs.append(ops.dissensus_attack_job(msgs[NA + e], msgs, P, P, j, honest, n_byz, param))
-                continue
-            if e in mimic_row:
-                # copying the receiver to itself only slows its consensus: the candidates are S_j without j's own
-                # entries, unless that leaves none
-                q = mimic_row[e]
-                cand = [k for k, i in enumerate(honest) if i != j] or list(range(len(honest)))
-                for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
-                    mimic_jobs.append(ops.mimic_attack_job(msgs[NA + e], msgs, P, P, honest, cand, self.mimic_z[q, t],
-                                                           0, target_out=self.mimic_target[q, t:t + 1]))
-                continue
-            if e in tail_row or e in pipe_row:
-                slots, hon = self._tailored_slots(j)
-                rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
-                        else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
-                        else (L.TAILOR_COORD, self.aggregation[j]))
-            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
-                if e in pipe_row:
-                    pipe_jobs.append(ops.pipeline_attack_job(
-                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, mixing=self.mixing[j],
-                        n_perms=L.PIPELINE_PERMS, seed=self.seed, attacker=b, receiver=j, net=t,
-                        round=self.episodes_done & 0xFFFFFFFF, gamma_out=self.att_gamma[pipe_row[e], t:t + 1]))
-                elif e in tail_row:
-                    tail_jobs.append(ops.tailored_attack_job(msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind,
-                                                             param, gamma_out=self.att_gamma[tail_row[e], t:t + 1]))
-                elif e in ada_row:
-                    ada_jobs.append(ops.adaptive_attack_job(msgs[NA + e], msgs, P, P, honest, kind, param,
-                                                            gamma_out=self.att_gamma[ada_row[e], t:t + 1]))
-                else:
-                    att_jobs.append(ops.attack_job(msgs[NA + e], msgs, P, P, honest, kind, param, seed=self.seed,
-                                                   attacker=b, receiver=j, round=self.episodes_done & 0xFFFFFFFF))
-        att_groups = [ops.job_array(L.AttackJob, att_jobs[g:g + L.MAX_JOBS]) for g in range(0, len(att_jobs), L.MAX_JOBS)]
-        ada_groups = [ops.job_array(L.AdaptiveAttackJob, ada_jobs[g:g + L.MAX_JOBS])
-                      for g in range(0, len(ada_jobs), L.MAX_JOBS)]
-        tail_groups = [ops.job_array(L.TailoredAttackJob, tail_jobs[g:g + L.MAX_JOBS])
-                       for g in range(0, len(tail_jobs), L.MAX_JOBS)]
-        pipe_groups = [ops.job_array(L.PipelineAttackJob, pipe_jobs[g:g + L.MAX_JOBS])
-                       for g in range(0, len(pipe_jobs), L.MAX_JOBS)]
-        diss_groups = [ops.job_array(L.DissensusJob, diss_jobs[g:g + L.MAX_JOBS])
-                       for g in range(0, len(diss_jobs), L.MAX_JOBS)]
-        # mimic job 2q + t belongs to pair mimic_pairs[q]; its T0 is the attacker's parameter
-        mimic_t0 = [int(self.attack[self.byz_pairs[e][0]][1]) for e in self.mimic_pairs]
-        mimic_groups = [(g, ops.job_array(L.MimicJob, mimic_jobs[g:g + L.MAX_JOBS]))
-                        for g in range(0, len(mimic_jobs), L.MAX_JOBS)]
+        # the Byzantine messages' job tables (_attack_job_groups)
+        (att_groups, ada_groups, tail_groups, pipe_groups, hist_groups, hist_mom, diss_groups, mimic_t0,
+         mimic_groups) = self._attack_job_groups()
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
         # 16 cooperative agents x 2 nets, so one nnm launch and one bucketing launch per epoch.  A bucketing job draws
@@ -754,6 +793,11 @@ class Trainer:
                 for job in g:
                     job.epoch = epoch
                 ops.pipeline_attack(g)
+                self.launches += 1
+            for g0, g in hist_groups:                                      # M as it stands before this epoch's step
+                for k, job in enumerate(g):
+                    job.first = int(self.momentum_steps[hist_mom[g0 + k]] == 0)
+                ops.history_attack(g)
                 self.launches += 1
             for g in diss_groups:                                          # no epoch dependence either
                 ops.dissensus_attack(g)

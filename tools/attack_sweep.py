@@ -23,6 +23,9 @@ for a whole-message rule is the weight of agent 4's momentum row.  The tailored 
 either, and the pipeline-aware attacks do not model momentum: those cells are marked refused; the pipeline-aware attacks (rcmarl_pipeline_attack:
 pipeline_uv, pipeline_std, pipeline_sgn, range multiplier 2 by default) model the receiver's mixing step and every rule,
 dnc included, but not mda or smea, whose cells are marked refused (their gamma is reported as the tailored attacks').
+The momentum-aware attacks (rcmarl_history_attack: history_uv, history_std, history_sgn, range multiplier 2 by default)
+run the pipeline attack's search in a momentum receiver's momentum rows and invert its momentum step; against a
+receiver without momentum they are the pipeline attacks, and mda or smea cells are marked refused.
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -35,7 +38,8 @@ and when it names dnc, mda or smea, on clip and each of those it names (all of t
 alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
 tailored_std (every cooperative agent on clip) against gauss, when it names a pipeline attack, the round on
-pipeline_std against gauss, and when it names mimic, the round on mimic against gauss.
+pipeline_std against gauss, when it names a history attack, the round on history_std against gauss with every
+cooperative agent on m0.9+clip, and when it names mimic, the round on mimic against gauss.
 
     python tools/attack_sweep.py [n_blocks=40] [n_envs=256] [timed_rounds=10] [out_dir=attack_sweep_out]
                                  [rules=clip,trim,wmsr] [attacks=alie,ipm,gauss]
@@ -57,7 +61,8 @@ from rcmarl._lib import RcmarlError            # noqa: E402
 from rcmarl.trainer import Trainer             # noqa: E402
 
 PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0,
-          "pipeline_uv": 2.0, "pipeline_std": 2.0, "pipeline_sgn": 2.0, "dissensus": 1.0, "mimic": 50.0}
+          "pipeline_uv": 2.0, "pipeline_std": 2.0, "pipeline_sgn": 2.0, "history_uv": 2.0, "history_std": 2.0,
+          "history_sgn": 2.0, "dissensus": 1.0, "mimic": 50.0}
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -92,6 +97,7 @@ WHOLE = VECTOR + ("dnc",) + SUBSET              # the rules that report neighbou
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
 TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
 PIPELINE = ("pipeline_uv", "pipeline_std", "pipeline_sgn")
+HISTORY = ("history_uv", "history_std", "history_sgn")
 ATTACKS = tuple((a.split(":")[0], float(a.split(":")[1]) if ":" in a else PARAMS.get(a, 1.0))
                 for a in (sys.argv[6] if len(sys.argv) > 6 else "alie,ipm,gauss").split(","))
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
@@ -164,10 +170,10 @@ def rule_timing():
     return out
 
 
-def adaptive_timing(attack="minmax_std"):
+def adaptive_timing(attack="minmax_std", momentum=None):
     """ms per update round (median over rounds) with agent 4 Byzantine on gauss and on `attack`, at the benchmark's C2
-    shape, the two trainers alternated round by round."""
-    cfg = dict(bench.workload("C2", 0), labels=["Cooperative"] * 4 + ["Byzantine"])
+    shape (every cooperative agent with `momentum`), the two trainers alternated round by round."""
+    cfg = dict(bench.workload("C2", 0), labels=["Cooperative"] * 4 + ["Byzantine"], momentum=momentum)
     trs = {a: Trainer(**dict(cfg, attack=(a, PARAMS.get(a, 1.0)))) for a in ("gauss", attack)}
     ms = {k: [] for k in trs}
     for r in range(timed_rounds + 1):
@@ -188,7 +194,7 @@ def adaptive_timing(attack="minmax_std"):
 
 
 def mean_gamma(tr):
-    """Mean gamma of the adaptive and tailored messages of the last epoch (critic and TR nets, every receiver)."""
+    """Mean gamma of the adaptive, tailored, pipeline and history messages of the last epoch (critic and TR nets, every receiver)."""
     g = [x for v in tr.attack_gammas().values() for x in v.tolist()]
     return float(np.mean(g)) if g else None
 
@@ -217,9 +223,10 @@ def timing_line(rt):
                                                                for k in timed_rules()[1:]])
 
 
-adaptive = any(a in ADAPTIVE + TAILORED + PIPELINE for a, _ in ATTACKS)
+adaptive = any(a in ADAPTIVE + TAILORED + PIPELINE + HISTORY for a, _ in ATTACKS)
 tailored = any(a in TAILORED for a, _ in ATTACKS)
 pipeline = any(a in PIPELINE for a, _ in ATTACKS)
+history = any(a in HISTORY for a, _ in ATTACKS)
 mimic = any(a == "mimic" for a, _ in ATTACKS)
 if vector:
     result["rule_timing"] = rt = rule_timing()
@@ -236,6 +243,10 @@ if pipeline:
     result["pipeline_timing"] = pt = adaptive_timing("pipeline_std")
     print(f"update round with agent 4 Byzantine: gauss {pt['gauss']['median_ms']:.2f} ms, pipeline_std "
           f"{pt['pipeline_std']['median_ms']:.2f} ms ({pt['pipeline_std_added_ms']:+.3f})", flush=True)
+if history:
+    result["history_timing"] = ht = adaptive_timing("history_std", momentum=0.9)
+    print(f"update round with agent 4 Byzantine, receivers on m0.9+clip: gauss {ht['gauss']['median_ms']:.2f} ms, "
+          f"history_std {ht['history_std']['median_ms']:.2f} ms ({ht['history_std_added_ms']:+.3f})", flush=True)
 if mimic:
     result["mimic_timing"] = mt = adaptive_timing("mimic")
     print(f"update round with agent 4 Byzantine: gauss {mt['gauss']['median_ms']:.2f} ms, mimic "
@@ -291,7 +302,7 @@ for rule in RULES:
         if vector:
             cell["byz_weight"] = float(np.mean(byz)) if split_rule(rule)[1] in WHOLE else None
         if adaptive:
-            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED + PIPELINE else None
+            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED + PIPELINE + HISTORY else None
         if mimic:
             cell["copied"] = {str(j): ks for j, ks in copied.items()} if copied else None
         result["cells"].append(cell)
@@ -342,6 +353,11 @@ with open(os.path.join(out_dir, "attack_sweep.md"), "w") as f:
         f.write(f"\nC2 update round at {pt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "
                 f"gauss {pt['gauss']['median_ms']:.2f} ms, pipeline_std {pt['pipeline_std']['median_ms']:.2f} ms "
                 f"({pt['pipeline_std_added_ms']:+.3f} ms)\n")
+    if history:
+        ht = result["history_timing"]
+        f.write(f"\nC2 update round at {ht['n_envs']} environments, agent 4 Byzantine, receivers on m0.9+clip (median "
+                f"of {timed_rounds}, alternated): gauss {ht['gauss']['median_ms']:.2f} ms, history_std "
+                f"{ht['history_std']['median_ms']:.2f} ms ({ht['history_std_added_ms']:+.3f} ms)\n")
     if mimic:
         mt = result["mimic_timing"]
         f.write(f"\nC2 update round at {mt['n_envs']} environments, agent 4 Byzantine (median of {timed_rounds}, alternated): "

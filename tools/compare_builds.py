@@ -1,17 +1,21 @@
 """Compare the outputs of the distance-based rules (rcmarl_vector_aggregate), the min-max / min-sum attacks
 (rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
 (rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack), the subset-selection rules MDA / SMEA
-(rcmarl_subset_aggregate) and per-neighbour momentum (rcmarl_momentum_mix) between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with
-tailored_attack_kernel and pipeline_attack_kernel (vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows,
-bucket_draw / bucket_means and the candidate search in csrc/train_kernels.cu), so a change there may change their
-register allocation and SASS; this shows whether it changed anything they compute.
+(rcmarl_subset_aggregate), per-neighbour momentum (rcmarl_momentum_mix), the pipeline attacks
+(rcmarl_pipeline_attack) and the history attacks (rcmarl_history_attack) between two builds of librcmarl.so, bit for
+bit.  Their kernels share their bodies with tailored_attack_kernel, pipeline_attack_kernel and history_attack_kernel
+(vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows, bucket_draw / bucket_means, tailored_stage /
+tailored_range, the candidate search and the momentum step in csrc/train_kernels.cu), so a change there may change
+their register allocation and SASS; this shows whether it changed anything they compute.
 
 Each build runs in its own process (RCMARL_LIB selects the library) on the same inputs: 24 messages of 1421 parameters
 around a common centre, four of them 1e3 times larger and one holding 1e30; every vector rule at n_in 1 .. 16 (H drawn
 per job, repeated in-nodes) with the weights, every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
 gamma), DnC, nnm and bucketing (s = 1, 2, 3) at n_in 1 .. 16 with their weights or mixing matrices, and every tailored
 attack x rule at n_in 2 .. 16 (scale 2, with gamma), MDA and SMEA at n_in 1 .. 16 (H drawn per job, with the
-weights), and momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), at the trainer's
+weights), momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), every pipeline
+attack x rule (DnC included) x mixing (none, nnm, bucketing at s = 2 with 3 samples) at n_in 2 .. 16 with gamma and
+model_out, and history_std x rule at n_in 2 .. 16 for (beta, first) = (0.9, 0), (0.99, 0), (0.5, 1), at the trainer's
 parameter counts.  Entry points a build does not export are skipped when loading it, so a
 build from before rcmarl_tailored_attack existed loads too; the outputs of an entry point only one build exports are
 listed and not compared.
@@ -128,6 +132,58 @@ if hasattr(lib, "rcmarl_momentum_mix"):
                                            int(step == 0)) for q in range(16)])
         named.update({f"momentum_{step}_{q}": np.concatenate([dsts[q].cpu().numpy().ravel(), Ms[q].cpu().numpy().ravel()])
                       for q in range(16)})
+
+
+def attack_cases(rule):
+    """(slots, honest, H, P) of an attack job against `rule` at n_in 2 .. 16, 1-3 crafted slots."""
+    out = []
+    for n_in in range(2, 17):
+        if rule in ("krum", "mkrum") and n_in < 3:
+            continue
+        n_cr = 1 + n_in % 3 if n_in > 3 else 1
+        real = [int(x) for x in rs.choice(20, size=n_in - n_cr, replace=False)]
+        slots = real[:1] + [-1] * n_cr + real[1:]
+        honest = [k for k, s in enumerate(slots) if 0 <= s < 16] or [0]
+        top = n_in - 3 if rule in ("krum", "mkrum") else (n_in - 1) // 2 if rule == "trim" else n_in - 1
+        out.append((slots, honest, int(rs.randint(0, top + 1)), PC[n_in % 4]))
+    return out
+
+
+ATTACK_RULES = ("clip", "trim", "wmsr", "krum", "mkrum", "scclip", "gmed", "dnc")
+if hasattr(lib, "rcmarl_pipeline_attack"):
+    for rule in ATTACK_RULES:
+        for mixing in (None, "nnm", ("bucket", 2)):
+            for a in ("pipeline_uv", "pipeline_std", "pipeline_sgn"):
+                jobs, dsts = [], []
+                for slots, honest, H, n in attack_cases(rule):
+                    if rule in ("krum", "mkrum") and mixing is not None and len(slots) < 6:
+                        continue                                  # too few mixed rows for the rule at H
+                    if isinstance(mixing, tuple):
+                        n_rows = 1 + (len(slots) - 2) // 2 + 1
+                        H = min(H, n_rows - 3 if rule in ("krum", "mkrum") else (n_rows - 1) // 2 if rule == "trim"
+                                else n_rows - 1)
+                    d = torch.full((2 * P + 1,), float("nan"), device="cuda")
+                    jobs.append(ops.pipeline_attack_job(d[:P], msgs, P, n, slots, honest, rule, H, a, 2.0,
+                                                        mixing=mixing, n_perms=3, seed=11, attacker=len(slots),
+                                                        receiver=2, net=1, round=5, epoch=1, gamma_out=d[2 * P:],
+                                                        model_out=d[P:2 * P]))
+                    dsts.append(d)
+                ops.pipeline_attack(jobs)
+                named.update({f"pipeline_{rule}_{mixing}_{a}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
+if hasattr(lib, "rcmarl_history_attack"):
+    ref = msgs[0] * 0.5
+    M = (torch.randn(16, P, generator=torch.Generator().manual_seed(5)) * 0.3).cuda()
+    for rule in ATTACK_RULES:
+        for beta, first in ((0.9, 0), (0.99, 0), (0.5, 1)):
+            jobs, dsts = [], []
+            for slots, honest, H, n in attack_cases(rule):
+                d = torch.full((2 * P + 1,), float("nan"), device="cuda")
+                jobs.append(ops.history_attack_job(d[:P], msgs, P, n, slots, honest, rule, H, "history_std", 2.0, ref,
+                                                   M, P, beta, first, [slots.index(-1)], gamma_out=d[2 * P:],
+                                                   model_out=d[P:2 * P]))
+                dsts.append(d)
+            ops.history_attack(jobs)
+            named.update({f"history_{rule}_{beta}_{first}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
 np.savez(sys.argv[1], *outs, **named)
 '''
 
@@ -149,7 +205,7 @@ def main():
     only = sorted(set(a.files) ^ set(b.files))
     diff = [k for k in common if a[k].tobytes() != b[k].tobytes()]
     print(f"{len(common)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix, "
-          "tailored_attack, subset_aggregate and momentum_mix outputs): "
+          "tailored_attack, subset_aggregate, momentum_mix, pipeline_attack and history_attack outputs): "
           + ("bitwise equal" if not diff else f"{len(diff)} differ: {diff[:8]}")
           + (f"; {len(only)} from an entry point only one build exports, not compared" if only else ""))
     sys.exit(1 if diff or not common else 0)
