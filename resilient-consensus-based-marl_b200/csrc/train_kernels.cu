@@ -1949,6 +1949,84 @@ static int launch_mb_persist(const MbParams& P, int n_ctas, cudaStream_t st) {
     return launch_pdl(mb_persist_kernel<NA>, dim3(n_ctas), dim3(32 * NW), smem, st, P);
 }
 
+// [first, last) byte range, never empty
+struct Range {
+    uintptr_t first, last;
+};
+
+static bool overlap(const Range& a, const Range& b) { return a.first < b.last && b.first < a.last; }
+
+// up to CAP byte ranges
+template <int CAP>
+struct RangeList {
+    Range at[CAP];
+    int n = 0;
+    // n_bytes bytes at p
+    void bytes(const void* p, int64_t n_bytes) { at[n++] = {(uintptr_t)p, (uintptr_t)p + (uintptr_t)n_bytes}; }
+    // n_floats floats at p
+    void floats(const float* p, int64_t n_floats) { row(p, 0, 0, n_floats); }
+    // n_floats floats at base + r * stride floats
+    void row(const float* base, int64_t r, int64_t stride, int64_t n_floats) {
+        const uintptr_t first = (uintptr_t)base + (uintptr_t)(r * stride * (int64_t)sizeof(float));
+        at[n++] = {first, first + (uintptr_t)(n_floats * (int64_t)sizeof(float))};
+    }
+    // the rows r < n_rows
+    void rows(const float* base, int n_rows, int64_t stride, int64_t n_floats) {
+        for (int r = 0; r < n_rows; ++r) row(base, r, stride, n_floats);
+    }
+    // the rows nodes[k], k < n_nodes, except the crafted slots (-1)
+    void nodes(const float* base, const int32_t* nodes, int n_nodes, int64_t stride, int64_t n_floats) {
+        for (int k = 0; k < n_nodes; ++k)
+            if (nodes[k] >= 0) row(base, nodes[k], stride, n_floats);
+    }
+};
+
+// What the CTAs of one launch write (w) and read (r).  A CTA may read its inputs before it writes, but the CTAs of
+// other jobs run concurrently: a launch is refused when a written range overlaps another written range or a read range
+// of any job of the launch.  Read ranges may overlap each other.  Sized for the most ranges of one launch: the 2 x 16
+// written rows per job of rcmarl_momentum_mix and the 2 x 16 + 1 read ranges per job of rcmarl_history_attack.
+struct RangeSet {
+    RangeList<2 * RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS> w;
+    RangeList<RCMARL_MAX_JOBS * (2 * RCMARL_MAX_NEIGHBOURS + 1)> r;
+    // Sorts the written ranges by start, so the check takes O((w.n + r.n) log w.n) comparisons instead of one per pair.
+    bool overlaps() {
+        Range* const w0 = w.at;
+        Range* const w1 = w.at + w.n;
+        std::sort(w0, w1, [](const Range& a, const Range& b) {
+            return a.first < b.first || (a.first == b.first && a.last < b.last);
+        });
+        for (const Range* a = w0; a + 1 < w1; ++a)
+            if (a->last > a[1].first) return true;
+        // the written ranges are now disjoint and sorted by start, hence by end too: of them only the first one that
+        // ends after a read range's start can overlap it
+        for (int k = 0; k < r.n; ++k) {
+            const Range* it =
+                std::upper_bound(w0, w1, r.at[k].first, [](uintptr_t x, const Range& q) { return x < q.last; });
+            if (it != w1 && it->first < r.at[k].last) return true;
+        }
+        return false;
+    }
+};
+
+// One CTA of `threads` per job, staging up to `floats` floats (the largest job's) in dynamic shared memory.  The kernel
+// also has static shared memory, so the default 48 KB limit applies to static + dynamic: its limit is lifted to the
+// staging bound of `bound` floats once per device, before the kernel's first launch there (opted: the flags of this
+// Kernel), independent of any other launch.
+template <auto Kernel, typename Params>
+static int launch_staged(const Params& P, int n_jobs, int bound, int64_t floats, int threads, void* stream) {
+    static bool opted[64] = {};
+    int dev = 0;
+    RC_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64 || !opted[dev]) {
+        RC_CUDA(cudaFuncSetAttribute((const void*)Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float) * bound)));
+        if (dev >= 0 && dev < 64) opted[dev] = true;
+    }
+    Kernel<<<n_jobs, threads, sizeof(float) * (size_t)floats, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
+}
+
 }  // namespace rcmarl
 
 using namespace rcmarl;
@@ -2131,6 +2209,23 @@ static bool bad_rule(int rule, int H, int n_in) {
     return rule < RCMARL_AGG_CLIP || rule > RCMARL_AGG_WMSR || (rule == RCMARL_AGG_TRIM && 2 * H >= n_in);
 }
 
+// a receiver's rule: a known family and rule, and an H that rule allows for n_rows messages (COORD: the checks of
+// rcmarl_consensus_hidden)
+static bool bad_receiver_rule(int family, int rule, int H, int n_rows) {
+    if (H < 0 || H >= n_rows) return true;
+    if (family == RCMARL_TAILOR_COORD) return bad_rule(rule, H, n_rows);
+    if (family == RCMARL_TAILOR_SPECTRAL) return rule != RCMARL_SPECTRAL_DNC;
+    if (family != RCMARL_TAILOR_VECTOR || rule < RCMARL_VEC_KRUM || rule > RCMARL_VEC_GMED) return true;
+    return (rule == RCMARL_VEC_KRUM || rule == RCMARL_VEC_MKRUM) && n_rows < H + 3;
+}
+
+// a negative row among the first n of a node list (in-nodes or honest rows; callers have checked n)
+static bool bad_nodes(const int32_t* nodes, int n) {
+    for (int k = 0; k < n; ++k)
+        if (nodes[k] < 0) return true;
+    return false;
+}
+
 int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs, void* ws, int64_t ws_bytes,
                 void* stream) {
     if (int e = check_rows(rows)) return e;
@@ -2145,9 +2240,7 @@ int rcmarl_team(const rcmarl_rows* rows, const rcmarl_team_job* jobs, int n_jobs
         if (!q.w || q.kind < 0 || q.kind > 2) return RCMARL_ERR_ARG;
         if (!q.agg_in) {
             if (!q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
-            for (int k = 0; k < q.n_in; ++k)
-                if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
-            if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
+            if (bad_nodes(q.in_nodes, q.n_in) || bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         }
         if (!q.sums && !q.agg_out) return RCMARL_ERR_ARG;
         any_sums |= (q.sums != nullptr);
@@ -2199,9 +2292,7 @@ int rcmarl_consensus_hidden(const rcmarl_consensus_job* jobs, int n_jobs, void* 
         const rcmarl_consensus_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS || q.H < 0 || q.H >= q.n_in || q.n_hidden < 1)
             return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
-        if (bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in) || bad_rule(q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         P.jobs[j] = q;
         if (q.n_hidden > maxn) maxn = q.n_hidden;
     }
@@ -2217,8 +2308,7 @@ int rcmarl_attack(const rcmarl_attack_job* jobs, int n_jobs, void* stream) {
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_attack_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_honest; ++k)
-            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.honest, q.n_honest)) return RCMARL_ERR_ARG;
         if (q.kind < RCMARL_ATTACK_ALIE || q.kind > RCMARL_ATTACK_GAUSS || !std::isfinite(q.param)) return RCMARL_ERR_ARG;
         if (q.kind == RCMARL_ATTACK_GAUSS && q.param < 0.f) return RCMARL_ERR_ARG;
         if (q.attacker > 255u || q.receiver > 255u) return RCMARL_ERR_ARG;
@@ -2230,286 +2320,146 @@ int rcmarl_attack(const rcmarl_attack_job* jobs, int n_jobs, void* stream) {
     return RCMARL_OK;
 }
 
-// [first, last) byte range of n floats at base + row * stride floats
-static void float_range(const float* base, int64_t row, int64_t stride, int64_t n, uintptr_t& first, uintptr_t& last) {
-    first = (uintptr_t)base + (uintptr_t)(row * stride * (int64_t)sizeof(float));
-    last = first + (uintptr_t)(n * (int64_t)sizeof(float));
-}
-
-// true if a written range [w0, w1) overlaps another written range or a read range [r0, r1)
-static bool writes_overlap(const uintptr_t* w0, const uintptr_t* w1, int n_w, const uintptr_t* r0, const uintptr_t* r1,
-                           int n_r) {
-    for (int a = 0; a < n_w; ++a) {
-        for (int b = a + 1; b < n_w; ++b)
-            if (w0[a] < w1[b] && w0[b] < w1[a]) return true;
-        for (int r = 0; r < n_r; ++r)
-            if (w0[a] < r1[r] && r0[r] < w1[a]) return true;
-    }
-    return false;
-}
-
-// Lift a kernel's dynamic shared-memory limit to `bytes`, once per device (opted: that kernel's flags), before its first
-// launch there, independent of any other launch.
-static int opt_in_smem(const void* kernel, int bytes, bool (&opted)[64]) {
-    int dev = 0;
-    RC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !opted[dev]) {
-        RC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        if (dev >= 0 && dev < 64) opted[dev] = true;
-    }
-    return RCMARL_OK;
-}
-
 int rcmarl_vector_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     VectorParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_vector_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        if (q.rule < RCMARL_VEC_KRUM || q.rule > RCMARL_VEC_GMED || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
-        if ((q.rule == RCMARL_VEC_KRUM || q.rule == RCMARL_VEC_MKRUM) && q.n_in < q.H + 3) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_receiver_rule(RCMARL_TAILOR_VECTOR, q.rule, q.H, q.n_in) || bad_nodes(q.in_nodes, q.n_in))
+            return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)(q.n_in + 1) * q.n;
         if (floats > RCMARL_VECTOR_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst and weights_out, reads the in-node rows
+        S.w.floats(q.dst, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    // The CTAs stage their inputs before anything is written, but the CTAs of other jobs run concurrently: no written
-    // range (a dst, a weights_out) may overlap an in-node row of any job of the launch or another written range.
-    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (jobs[j].weights_out) {
-            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
-            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    // The kernel also has static shared memory, so the default 48 KB limit applies to static + dynamic: opt in to the
-    // largest staging size, once per device, before the first launch there (independent of any other launch).
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)vector_agg_kernel, (int)(sizeof(float) * RCMARL_VECTOR_MAX_FLOATS), opted)) return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    vector_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<vector_agg_kernel>(P, n_jobs, RCMARL_VECTOR_MAX_FLOATS, max_floats, VEC_THREADS, stream);
 }
 
 int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     VectorParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_vector_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        if (q.rule != RCMARL_SPECTRAL_DNC || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_receiver_rule(RCMARL_TAILOR_SPECTRAL, q.rule, q.H, q.n_in) || bad_nodes(q.in_nodes, q.n_in))
+            return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)(q.n_in + 2) * q.n;
         if (floats > RCMARL_DNC_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst and weights_out, reads the in-node rows
+        S.w.floats(q.dst, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate: no written range (a dst, a weights_out) may overlap an in-node row of any job of the
-    // launch or another written range
-    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (jobs[j].weights_out) {
-            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
-            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)dnc_agg_kernel, (int)(sizeof(float) * RCMARL_DNC_MAX_FLOATS), opted)) return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    dnc_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<dnc_agg_kernel>(P, n_jobs, RCMARL_DNC_MAX_FLOATS, max_floats, VEC_THREADS, stream);
 }
 
 int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     VectorParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_vector_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
         if ((q.rule != RCMARL_SUBSET_MDA && q.rule != RCMARL_SUBSET_SMEA) || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in)) return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)q.n_in * q.n;
         if (floats > RCMARL_SUBSET_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst and weights_out, reads the in-node rows
+        S.w.floats(q.dst, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate: no written range (a dst, a weights_out) may overlap an in-node row of any job of the
-    // launch or another written range
-    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (jobs[j].weights_out) {
-            float_range(jobs[j].weights_out, 0, 0, jobs[j].n_in, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < jobs[j].n_in; ++k, ++n_r)
-            float_range(jobs[j].msgs, jobs[j].in_nodes[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)subset_agg_kernel, (int)(sizeof(float) * RCMARL_SUBSET_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    subset_agg_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<subset_agg_kernel>(P, n_jobs, RCMARL_SUBSET_MAX_FLOATS, max_floats, VEC_THREADS, stream);
 }
 
 int rcmarl_nnm_mix(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     VectorParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_vector_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
         if (q.rule != RCMARL_MIX_NNM || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in)) return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)q.n_in * q.n;
         if (floats > RCMARL_NNM_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes the n_in dst rows and the n_in^2 weights, reads the in-node rows
+        S.w.rows(q.dst, q.n_in, q.msg_stride, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, (int64_t)q.n_in * q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate, with n_in dst rows per job: no written range (a dst row, a weights_out) may overlap an
-    // in-node row of any job of the launch or another written range
-    constexpr int MAX_W = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1), MAX_R = RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS;
-    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_vector_job& q = jobs[j];
-        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
-        if (q.weights_out) {
-            float_range(q.weights_out, 0, 0, (int64_t)q.n_in * q.n_in, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < q.n_in; ++k, ++n_r)
-            float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)nnm_mix_kernel, (int)(sizeof(float) * RCMARL_NNM_MAX_FLOATS), opted)) return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    nnm_mix_kernel<<<n_jobs, VEC_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<nnm_mix_kernel>(P, n_jobs, RCMARL_NNM_MAX_FLOATS, max_floats, VEC_THREADS, stream);
 }
 
 int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     BucketParams P;
+    RangeSet S;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_bucket_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
-        if (q.s < 1 || q.net > 1u || q.receiver > 255u) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in) || q.s < 1 || q.net > 1u || q.receiver > 255u) return RCMARL_ERR_ARG;
         P.jobs[j] = q;
-    }
-    // as rcmarl_nnm_mix, with n_out = 1 + ceil((n_in - 1) / s) dst rows per job: no written range (a dst row, a
-    // weights_out) may overlap an in-node row of any job of the launch or another written range
-    constexpr int MAX_W = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1), MAX_R = RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS;
-    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_bucket_job& q = jobs[j];
+        // writes the n_out = 1 + ceil((n_in - 1) / s) dst rows and the n_out * n_in weights, reads the in-node rows
         const int n_out = q.n_in == 1 ? 1 : 1 + (q.n_in - 2) / q.s + 1;
-        for (int k = 0; k < n_out; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
-        if (q.weights_out) {
-            float_range(q.weights_out, 0, 0, (int64_t)n_out * q.n_in, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < q.n_in; ++k, ++n_r)
-            float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
+        S.w.rows(q.dst, n_out, q.msg_stride, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, (int64_t)n_out * q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
     bucket_mix_kernel<<<n_jobs, VEC_THREADS, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
 }
 
-// writes_overlap for the many ranges of rcmarl_momentum_mix (up to 1024 written, 544 read): the written ranges sorted by
-// start, so the check takes O((n_w + n_r) log n_w) comparisons instead of one per pair
-static bool sorted_writes_overlap(const uintptr_t* w0, const uintptr_t* w1, int n_w, const uintptr_t* r0,
-                                  const uintptr_t* r1, int n_r) {
-    std::pair<uintptr_t, uintptr_t> w[2 * RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    for (int a = 0; a < n_w; ++a) w[a] = {w0[a], w1[a]};
-    std::sort(w, w + n_w);
-    for (int a = 0; a + 1 < n_w; ++a)
-        if (w[a].second > w[a + 1].first) return true;
-    // the written ranges are now disjoint and sorted by start, hence by end too: of them only the first one that ends
-    // after r0 can overlap [r0, r1)
-    for (int r = 0; r < n_r; ++r) {
-        const auto* it = std::upper_bound(w, w + n_w, r0[r], [](uintptr_t x, const std::pair<uintptr_t, uintptr_t>& q) {
-            return x < q.second;
-        });
-        if (it != w + n_w && it->first < r1[r]) return true;
-    }
-    return false;
-}
-
 int rcmarl_momentum_mix(const rcmarl_momentum_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     MomentumParams P;
+    RangeSet S;
     int maxn = 0, max_in = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_momentum_job& q = jobs[j];
         if (!q.dst || !q.msgs || !q.ref || !q.momentum || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS)
             return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_in; ++k)
-            if (q.in_nodes[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in)) return RCMARL_ERR_ARG;
         if (!std::isfinite(q.beta) || q.beta < 0.f || q.beta >= 1.f || (q.first != 0 && q.first != 1))
             return RCMARL_ERR_ARG;
         P.jobs[j] = q;
         if (q.n > maxn) maxn = q.n;
         if (q.n_in > max_in) max_in = q.n_in;
+        // writes the dst rows and the M rows, reads the in-node rows and (below) the ref
+        S.w.rows(q.dst, q.n_in, q.msg_stride, q.n);
+        S.w.rows(q.momentum, q.n_in, q.momentum_stride, q.n);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
     }
-    // a thread reads its coordinate of x_k, c and M_k before it writes M_k and row k, but other CTAs run concurrently:
-    // no written range (a dst row, an M row) may overlap an in-node row or a ref of any job of the launch or another
-    // written range, and no ref may overlap an in-node row
-    constexpr int MAX_W = 2 * RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS, MAX_R = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1);
-    uintptr_t w0[MAX_W], w1[MAX_W], r0[MAX_R], r1[MAX_R], c0[RCMARL_MAX_JOBS], c1[RCMARL_MAX_JOBS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_momentum_job& q = jobs[j];
-        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.dst, k, q.msg_stride, q.n, w0[n_w], w1[n_w]);
-        for (int k = 0; k < q.n_in; ++k, ++n_w) float_range(q.momentum, k, q.momentum_stride, q.n, w0[n_w], w1[n_w]);
-        for (int k = 0; k < q.n_in; ++k, ++n_r) float_range(q.msgs, q.in_nodes[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
-        float_range(q.ref, 0, 0, q.n, c0[j], c1[j]);
-    }
-    for (int j = 0; j < n_jobs; ++j)
-        for (int r = 0; r < n_r; ++r)
-            if (c0[j] < r1[r] && r0[r] < c1[j]) return RCMARL_ERR_ARG;
-    for (int j = 0; j < n_jobs; ++j, ++n_r) {
-        r0[n_r] = c0[j];
-        r1[n_r] = c1[j];
-    }
-    if (sorted_writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    // and no ref may overlap an in-node row of any job of the launch (two refs may coincide)
+    const int n_rows = S.r.n;
+    for (int j = 0; j < n_jobs; ++j) S.r.floats(jobs[j].ref, jobs[j].n);
+    for (int c = n_rows; c < S.r.n; ++c)
+        for (int k = 0; k < n_rows; ++k)
+            if (overlap(S.r.at[c], S.r.at[k])) return RCMARL_ERR_ARG;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
     momentum_mix_kernel<<<dim3((maxn + 255) / 256, n_jobs, max_in), 256, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
@@ -2518,12 +2468,12 @@ int rcmarl_momentum_mix(const rcmarl_momentum_job* jobs, int n_jobs, void* strea
 int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     AdaptiveParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_adaptive_attack_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_honest; ++k)
-            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.honest, q.n_honest)) return RCMARL_ERR_ARG;
         if (q.kind < RCMARL_ADAPT_MINMAX || q.kind > RCMARL_ADAPT_MINSUM || q.dev < RCMARL_DEV_UV || q.dev > RCMARL_DEV_SGN)
             return RCMARL_ERR_ARG;
         if (!std::isfinite(q.scale) || q.scale < 0.f) return RCMARL_ERR_ARG;
@@ -2531,41 +2481,14 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs, int n_jobs, v
         if (floats > RCMARL_ADAPTIVE_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst and gamma_out, reads the honest rows
+        S.w.floats(q.dst, q.n);
+        if (q.gamma_out) S.w.floats(q.gamma_out, 1);
+        S.r.nodes(q.msgs, q.honest, q.n_honest, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate: no written range (a dst, a gamma_out) may overlap an honest row of any job of the launch
-    // or another written range
-    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        float_range(jobs[j].dst, 0, 0, jobs[j].n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (jobs[j].gamma_out) {
-            float_range(jobs[j].gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        for (int k = 0; k < jobs[j].n_honest; ++k, ++n_r)
-            float_range(jobs[j].msgs, jobs[j].honest[k], jobs[j].msg_stride, jobs[j].n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    // the staging bound is above the default 48 KB of dynamic shared memory
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)adaptive_attack_kernel, (int)(sizeof(float) * RCMARL_ADAPTIVE_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    adaptive_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
-}
-
-// the receiver's rule of a tailored or pipeline job: a known family and rule, and an H that rule allows for n_rows
-// messages (the checks of rcmarl_consensus_hidden, rcmarl_vector_aggregate and rcmarl_dnc_aggregate)
-static bool bad_receiver_rule(int family, int rule, int H, int n_rows) {
-    if (H < 0 || H >= n_rows) return true;
-    if (family == RCMARL_TAILOR_COORD) return bad_rule(rule, H, n_rows);
-    if (family == RCMARL_TAILOR_SPECTRAL) return rule != RCMARL_SPECTRAL_DNC;
-    if (family != RCMARL_TAILOR_VECTOR || rule < RCMARL_VEC_KRUM || rule > RCMARL_VEC_GMED) return true;
-    return (rule == RCMARL_VEC_KRUM || rule == RCMARL_VEC_MKRUM) && n_rows < H + 3;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<adaptive_attack_kernel>(P, n_jobs, RCMARL_ADAPTIVE_MAX_FLOATS, max_floats, ADA_THREADS,
+                                                 stream);
 }
 
 // the slot list, direction and scale of a tailored job (everything but its rule); n_real receives its real slots
@@ -2583,25 +2506,10 @@ static bool bad_tailored_slots(const rcmarl_tailored_attack_job& q, int& n_real)
     return !std::isfinite(q.scale) || q.scale < 0.f;
 }
 
-// the written ranges (dst, gamma_out) and the read ranges (the real slots' rows) of a tailored job
-static void tailored_ranges(const rcmarl_tailored_attack_job& q, uintptr_t* w0, uintptr_t* w1, int& n_w, uintptr_t* r0,
-                            uintptr_t* r1, int& n_r) {
-    float_range(q.dst, 0, 0, q.n, w0[n_w], w1[n_w]);
-    ++n_w;
-    if (q.gamma_out) {
-        float_range(q.gamma_out, 0, 0, 1, w0[n_w], w1[n_w]);
-        ++n_w;
-    }
-    for (int k = 0; k < q.n_in; ++k)
-        if (q.slots[k] >= 0) {
-            float_range(q.msgs, q.slots[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
-            ++n_r;
-        }
-}
-
 int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     TailoredParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_tailored_attack_job& q = jobs[j];
@@ -2612,27 +2520,20 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
         if (floats > RCMARL_TAILORED_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst and gamma_out, reads the real slots' rows
+        S.w.floats(q.dst, q.n);
+        if (q.gamma_out) S.w.floats(q.gamma_out, 1);
+        S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate: no written range (a dst, a gamma_out) may overlap a real slot's row of any job of the
-    // launch or another written range
-    uintptr_t w0[2 * RCMARL_MAX_JOBS], w1[2 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) tailored_ranges(jobs[j], w0, w1, n_w, r0, r1, n_r);
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    // the staging bound is above the default 48 KB of dynamic shared memory
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)tailored_attack_kernel, (int)(sizeof(float) * RCMARL_TAILORED_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    tailored_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<tailored_attack_kernel>(P, n_jobs, RCMARL_TAILORED_MAX_FLOATS, max_floats, ADA_THREADS,
+                                                 stream);
 }
 
 int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     PipelineParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_pipeline_attack_job& pj = jobs[j];
@@ -2655,31 +2556,21 @@ int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         if (floats > RCMARL_PIPELINE_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = pj;
+        // writes dst, gamma_out and model_out, reads the real slots' rows
+        S.w.floats(q.dst, q.n);
+        if (q.gamma_out) S.w.floats(q.gamma_out, 1);
+        if (pj.model_out) S.w.floats(pj.model_out, q.n);
+        S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
     }
-    // as rcmarl_tailored_attack, with model_out among the written ranges
-    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        tailored_ranges(jobs[j].attack, w0, w1, n_w, r0, r1, n_r);
-        if (jobs[j].model_out) {
-            float_range(jobs[j].model_out, 0, 0, jobs[j].attack.n, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)pipeline_attack_kernel, (int)(sizeof(float) * RCMARL_PIPELINE_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    pipeline_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<pipeline_attack_kernel>(P, n_jobs, RCMARL_PIPELINE_MAX_FLOATS, max_floats, ADA_THREADS,
+                                                 stream);
 }
 
 int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     HistoryParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_history_attack_job& hj = jobs[j];
@@ -2696,61 +2587,37 @@ int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         if (floats > RCMARL_HISTORY_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = hj;
+        // writes dst, gamma_out and model_out, reads the real slots' rows, the ref and the n_in M rows
+        S.w.floats(q.dst, q.n);
+        if (q.gamma_out) S.w.floats(q.gamma_out, 1);
+        if (hj.model_out) S.w.floats(hj.model_out, q.n);
+        S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
+        S.r.floats(hj.ref, q.n);
+        S.r.rows(hj.momentum, q.n_in, hj.momentum_stride, q.n);
     }
-    // as rcmarl_pipeline_attack, with every ref and M row among the read ranges; up to 33 read ranges per job, so the
-    // written ranges are checked by a sorted sweep as in rcmarl_momentum_mix
-    constexpr int MAX_R = RCMARL_MAX_JOBS * (2 * RCMARL_MAX_NEIGHBOURS + 1);
-    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[MAX_R], r1[MAX_R];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_history_attack_job& hj = jobs[j];
-        tailored_ranges(hj.attack, w0, w1, n_w, r0, r1, n_r);
-        if (hj.model_out) {
-            float_range(hj.model_out, 0, 0, hj.attack.n, w0[n_w], w1[n_w]);
-            ++n_w;
-        }
-        float_range(hj.ref, 0, 0, hj.attack.n, r0[n_r], r1[n_r]);
-        ++n_r;
-        for (int k = 0; k < hj.attack.n_in; ++k, ++n_r)
-            float_range(hj.momentum, k, hj.momentum_stride, hj.attack.n, r0[n_r], r1[n_r]);
-    }
-    if (sorted_writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)history_attack_kernel, (int)(sizeof(float) * RCMARL_HISTORY_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    history_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<history_attack_kernel>(P, n_jobs, RCMARL_HISTORY_MAX_FLOATS, max_floats, ADA_THREADS, stream);
 }
 
 int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     DissensusParams P;
+    RangeSet S;
     int maxn = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_dissensus_job& q = jobs[j];
         if (!q.dst || !q.msgs || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS || q.own < 0)
             return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_honest; ++k)
-            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.honest, q.n_honest)) return RCMARL_ERR_ARG;
         if (q.n_byz < 1 || q.n_byz > RCMARL_MAX_NEIGHBOURS || !std::isfinite(q.eps) || q.eps < 0.f) return RCMARL_ERR_ARG;
         P.jobs[j] = q;
         if (q.n > maxn) maxn = q.n;
+        // writes dst, reads the own and honest rows
+        S.w.floats(q.dst, q.n);
+        S.r.nodes(q.msgs, &q.own, 1, q.msg_stride, q.n);
+        S.r.nodes(q.msgs, q.honest, q.n_honest, q.msg_stride, q.n);
     }
-    // one thread per coordinate reads every row it needs before it writes, but other CTAs run concurrently: no dst may
-    // overlap an honest or own row of any job of the launch or another dst
-    constexpr int MAX_R = RCMARL_MAX_JOBS * (RCMARL_MAX_NEIGHBOURS + 1);
-    uintptr_t w0[RCMARL_MAX_JOBS], w1[RCMARL_MAX_JOBS], r0[MAX_R], r1[MAX_R];
-    int n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_dissensus_job& q = jobs[j];
-        float_range(q.dst, 0, 0, q.n, w0[j], w1[j]);
-        float_range(q.msgs, q.own, q.msg_stride, q.n, r0[n_r], r1[n_r]);
-        ++n_r;
-        for (int k = 0; k < q.n_honest; ++k, ++n_r) float_range(q.msgs, q.honest[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_jobs, r0, r1, n_r)) return RCMARL_ERR_ARG;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
     dissensus_attack_kernel<<<dim3((maxn + 255) / 256, n_jobs), 256, 0, (cudaStream_t)stream>>>(P);
     RC_CUDA(cudaGetLastError());
     return RCMARL_OK;
@@ -2759,47 +2626,27 @@ int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* 
 int rcmarl_mimic_attack(const rcmarl_mimic_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     MimicParams P;
+    RangeSet S;
     int64_t max_floats = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const rcmarl_mimic_job& q = jobs[j];
         if (!q.dst || !q.msgs || !q.z || q.n < 1 || q.n_honest < 1 || q.n_honest > RCMARL_MAX_NEIGHBOURS)
             return RCMARL_ERR_ARG;
-        for (int k = 0; k < q.n_honest; ++k)
-            if (q.honest[k] < 0) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.honest, q.n_honest)) return RCMARL_ERR_ARG;
         if (q.candidate_mask == 0u || (q.candidate_mask >> q.n_honest) != 0u) return RCMARL_ERR_ARG;
         if (q.update != 0 && q.update != 1) return RCMARL_ERR_ARG;
         const int64_t floats = (int64_t)(q.n_honest + 3) * q.n;
         if (floats > RCMARL_MIMIC_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = q;
+        // writes dst, z and target_out (one int32), reads the honest rows
+        S.w.floats(q.dst, q.n);
+        S.w.floats(q.z, q.n);
+        if (q.target_out) S.w.bytes(q.target_out, sizeof(int32_t));
+        S.r.nodes(q.msgs, q.honest, q.n_honest, q.msg_stride, q.n);
     }
-    // as rcmarl_vector_aggregate: no written range (a dst, a z, a target_out) may overlap an honest row of any job of the
-    // launch or another written range
-    uintptr_t w0[3 * RCMARL_MAX_JOBS], w1[3 * RCMARL_MAX_JOBS], r0[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS],
-        r1[RCMARL_MAX_JOBS * RCMARL_MAX_NEIGHBOURS];
-    int n_w = 0, n_r = 0;
-    for (int j = 0; j < n_jobs; ++j) {
-        const rcmarl_mimic_job& q = jobs[j];
-        float_range(q.dst, 0, 0, q.n, w0[n_w], w1[n_w]);
-        ++n_w;
-        float_range(q.z, 0, 0, q.n, w0[n_w], w1[n_w]);
-        ++n_w;
-        if (q.target_out) {
-            w0[n_w] = (uintptr_t)q.target_out;
-            w1[n_w] = w0[n_w] + sizeof(int32_t);
-            ++n_w;
-        }
-        for (int k = 0; k < q.n_honest; ++k, ++n_r) float_range(q.msgs, q.honest[k], q.msg_stride, q.n, r0[n_r], r1[n_r]);
-    }
-    if (writes_overlap(w0, w1, n_w, r0, r1, n_r)) return RCMARL_ERR_ARG;
-    // the staging bound is above the default 48 KB of dynamic shared memory
-    static bool opted[64] = {};
-    if (int e = opt_in_smem((const void*)mimic_attack_kernel, (int)(sizeof(float) * RCMARL_MIMIC_MAX_FLOATS), opted))
-        return e;
-    const size_t smem = sizeof(float) * (size_t)max_floats;
-    mimic_attack_kernel<<<n_jobs, ADA_THREADS, smem, (cudaStream_t)stream>>>(P);
-    RC_CUDA(cudaGetLastError());
-    return RCMARL_OK;
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<mimic_attack_kernel>(P, n_jobs, RCMARL_MIMIC_MAX_FLOATS, max_floats, ADA_THREADS, stream);
 }
 
 int rcmarl_sgd_apply(const rcmarl_sgd_job* jobs, int n_jobs, void* stream) {
