@@ -114,13 +114,16 @@ __host__ __device__ constexpr int stage_floats_per_row(int din, bool is_sa_net) 
 // Bulk-copy input staging costs 64 x 3*NA x 4 bytes of shared memory per warp.  At n_agents = 5 (3.8 KB per warp) it fits
 // next to 8 tiles; at n_agents = 16 it would cut the CTA from 6 to 4 warps, so those instantiations keep per-lane loads.
 __host__ __device__ constexpr bool grad_use_tma(int na) { return na <= 5; }
+// per-warp target slot of the bulk-copy path: the 64 targets of the next staged chunk (256 bytes per warp)
+__host__ __device__ constexpr int tgt_slot_floats(int na) { return grad_use_tma(na) ? 64 : 0; }
 
 template <int DIN, int NOUT, bool SA_NET>
 constexpr int grad_warps_for() {
     using L = TileLayout<DIN, NOUT>;
     const int na = SA_NET ? DIN / 3 : DIN / 2;
     const int avail = GRAD_SMEM_BUDGET - 4 * (round4(param_count(DIN, NOUT)) + 16) - 128;
-    const int n = avail / (4 * L::ROWS * L::RS + (grad_use_tma(na) ? 4 * L::ROWS * stage_floats_per_row(DIN, SA_NET) : 0));
+    const int n = avail / (4 * L::ROWS * L::RS + 4 * tgt_slot_floats(na) +
+                           (grad_use_tma(na) ? 4 * L::ROWS * stage_floats_per_row(DIN, SA_NET) : 0));
     return n > 8 ? 8 : n;
 }
 template <int NA, int LOSS>
@@ -161,6 +164,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// ---- per-lane 4-byte asynchronous copies (SASS LDGSTS) of the next chunk's targets; completion is per thread ----
+__device__ __forceinline__ void cp_async4(float* dst, const float* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 struct GradParams {
     rcmarl_rows rows;
     rcmarl_grad_job jobs[RCMARL_MAX_JOBS];
@@ -186,11 +196,13 @@ struct GradCore {
     static constexpr int R = 2;
     static constexpr int SROW = 3 * NA;                                     // staged row = one sa row (ns rows are shorter)
     static constexpr int SWARP = grad_use_tma(NA) ? L::ROWS * SROW : 0;      // staging floats per warp
+    static constexpr int TWARP = tgt_slot_floats(NA);                       // target-slot floats per warp
 
     float* sw;          // staged network parameters (shared)
     float* tiles;       // [GRAD_WARPS][ROWS][RS]
     float* wt;          // this warp's tile
     float* stage;       // this warp's bulk-copy staging buffer
+    float* tslot;       // this warp's target slot [ROWS]
     uint64_t* bar;      // this warp's mbarrier
     int warp, lane;
     uint32_t phase;
@@ -228,7 +240,8 @@ struct GradCore {
         lane = threadIdx.x & 31;
         wt = tiles + warp * (L::ROWS * L::RS);
         stage = tiles + GRAD_WARPS * (L::ROWS * L::RS) + warp * SWARP;
-        bar = reinterpret_cast<uint64_t*>(tiles + GRAD_WARPS * (L::ROWS * L::RS) + GRAD_WARPS * SWARP) + warp;
+        tslot = tiles + GRAD_WARPS * (L::ROWS * L::RS + SWARP) + warp * TWARP;
+        bar = reinterpret_cast<uint64_t*>(tiles + GRAD_WARPS * (L::ROWS * L::RS + SWARP + TWARP)) + warp;
         phase = 0;
         if (lane == 0) {
             mbar_init(bar, 1);
@@ -278,39 +291,48 @@ struct GradCore {
     const int rowf = from_ns ? 2 * NA : 3 * NA;
     const float* in_base = from_ns ? Rw.ns : Rw.sa;
     const bool gather_ok = grad_use_tma(NA) && ((Rw.time_idx == nullptr) || (Rw.n_envs % L::ROWS == 0));
-    auto stage_src = [&](int64_t c, const float*& src) -> bool {
+    // a chunk that can be staged is full and lies inside one time row, so its rows are base + 0 .. 63
+    auto stage_src = [&](int64_t c, int64_t& base, const float*& src) -> bool {
         if (!gather_ok || (c + 1) * L::ROWS > Rw.n_rows) return false;
-        src = in_base + row_of(Rw, c * L::ROWS) * rowf;
+        base = row_of(Rw, c * L::ROWS);
+        src = in_base + base * rowf;
         return (reinterpret_cast<uintptr_t>(src) & 15) == 0;
     };
-    bool staged = false;
     // Chunk c of the job goes to (CTA y, warp w) with c = k * cstep + w * gy + y: warp-major, so that the last, partial
     // round leaves one or two busy warps on every SM (on different schedulers, so they run faster alone).  A CTA-major
     // order (c = k * cstep + y * GRAD_WARPS + w) would leave a few SMs with all warps busy and the others idle, and the
     // whole launch would wait for a full extra round on those SMs.
     const int64_t cstep = (int64_t)gy * GRAD_WARPS;
     const int64_t cfirst = (int64_t)warp * gy + y;
-    {
-        const int64_t c0 = cfirst;
-        const float* src = nullptr;
-        if (c0 * L::ROWS < Rw.n_rows) staged = stage_src(c0, src);
-        if (staged && lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic accesses of the buffer
-            bulk_load(stage, src, (uint32_t)(L::ROWS * rowf * sizeof(float)), bar);
-        }
-    }
     const int64_t nchunks = (Rw.n_rows + L::ROWS - 1) / L::ROWS;
+    // Start the copies of chunk c's inputs (bulk, lane 0) and targets (cp.async, every lane its own two rows) if the
+    // chunk can be staged.  The targets go to the warp's target slot, so that no global load waits inside phase 1.  A
+    // chunk reads its targets back and uses them before it prefetches the next one, and each lane reads back only the two
+    // entries it copied, so the slot needs no warp barrier.
+    auto prefetch = [&](int64_t c) -> bool {
+        int64_t base = 0;
+        const float* src = nullptr;
+        const bool st = c < nchunks && stage_src(c, base, src);
+        if (st) {
+            if (lane == 0) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads before async writes
+                bulk_load(stage, src, (uint32_t)(L::ROWS * rowf * sizeof(float)), bar);
+            }
+#pragma unroll
+            for (int r = 0; r < R; ++r)
+                cp_async4(tslot + lane + 32 * r, job.target + (base + lane + 32 * r) * job.target_stride);
+            cp_async_commit();
+        }
+        return st;
+    };
+    bool staged = prefetch(cfirst);
     for (int64_t c = cfirst; c < nchunks; c += cstep) {
         // ---------------- phase 1: two rows per lane (lane, lane + 32 of the chunk) ----------------
         {
             bool live[R];
-            int64_t row[R];
+            float tgt[R];                                                  // dead rows: 0
 #pragma unroll
-            for (int r = 0; r < R; ++r) {
-                const int64_t m = c * L::ROWS + lane + 32 * r;
-                live[r] = m < Rw.n_rows;
-                row[r] = row_of(Rw, live[r] ? m : 0);      // dead rows read row 0 and contribute zeros
-            }
+            for (int r = 0; r < R; ++r) live[r] = c * L::ROWS + lane + 32 * r < Rw.n_rows;
             float h1[R][HID], h2[R][HID];
             {
                 float x[R][DIN];
@@ -324,35 +346,34 @@ struct GradCore {
 #pragma unroll
                         for (int k = 0; k < DIN; ++k) x[r][k] = sp[k + skip * (k >> 1)];
                     }
-                } else {
+                } else {                                                   // per-lane loads, targets beside the inputs
 #pragma unroll
-                    for (int r = 0; r < R; ++r) load_x<NA, DIN>(Rw, job.kind, row[r], x[r]);
-                }
-                __syncwarp();
-                {                                                          // prefetch the next chunk of this warp
-                    const int64_t c2 = c + cstep;
-                    const float* src = nullptr;
-                    staged = (c2 < nchunks) && stage_src(c2, src);
-                    if (staged && lane == 0) {
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads before async writes
-                        bulk_load(stage, src, (uint32_t)(L::ROWS * rowf * sizeof(float)), bar);
+                    for (int r = 0; r < R; ++r) {
+                        const int64_t row = row_of(Rw, live[r] ? c * L::ROWS + lane + 32 * r : 0);   // dead rows read row 0
+                        load_x<NA, DIN>(Rw, job.kind, row, x[r]);
+                        tgt[r] = live[r] ? __ldg(job.target + row * job.target_stride) : 0.f;
                     }
                 }
+                __syncwarp();
                 dense20_rows<DIN, R>(sw, sw + off_b1(DIN), x, h1);
 #pragma unroll
                 for (int r = 0; r < R; ++r)
                     put_vec<DIN, true, L::TA, L::BA1 * L::SA, true>(wt + (lane + 32 * r) * L::RS + L::OA1, x[r]);
             }
             dense20_rows<HID, R>(sw + off_W2(DIN), sw + off_b2(DIN), h1, h2);
+            if (staged) {                                                  // a staged chunk is full: every row is live
+                cp_async_wait_all();                                       // copied one chunk ago
+#pragma unroll
+                for (int r = 0; r < R; ++r) tgt[r] = tslot[lane + 32 * r];
+            }
             float d2[R][HID];
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 float* rowp = wt + (lane + 32 * r) * L::RS;
                 put_vec<HID, true, L::TA, L::BA2 * L::SA, true>(rowp + L::OA2, h1[r]);
-                const float tgt = live[r] ? __ldg(job.target + row[r] * job.target_stride) : 0.f;
                 if constexpr (NOUT == 1) {
                     // Keras MSE (Appendix A.2): dLoss/dout = 2 (out - y) / B; the 2/B is applied by the caller
-                    const float e = live[r] ? head1<DIN>(sw, h2[r]) - tgt : 0.f;
+                    const float e = live[r] ? head1<DIN>(sw, h2[r]) - tgt[r] : 0.f;
                     loss = fmaf(e, e, loss);
 #pragma unroll
                     for (int j = 0; j < HID; ++j) {
@@ -364,14 +385,15 @@ struct GradCore {
                     // weighted sparse categorical cross-entropy on the logits (Appendix A.5)
                     float p[NACT], mx, lse, g[NACT];
                     head5<DIN>(sw, h2[r], p);
-                    const int a = (int)__ldg(Rw.sa + row[r] * (3 * NA) + 3 * job.action_agent + 2);
+                    const int64_t row = row_of(Rw, live[r] ? c * L::ROWS + lane + 32 * r : 0);
+                    const int a = (int)__ldg(Rw.sa + row * (3 * NA) + 3 * job.action_agent + 2);
                     float la = 0.f;
 #pragma unroll
                     for (int o = 0; o < NACT; ++o) la = (o == a) ? p[o] : la;
                     softmax5(p, mx, lse);
-                    loss = fmaf(tgt, (mx + lse) - la, loss);
+                    loss = fmaf(tgt[r], (mx + lse) - la, loss);
 #pragma unroll
-                    for (int o = 0; o < NACT; ++o) g[o] = (p[o] - (o == a ? 1.f : 0.f)) * tgt;
+                    for (int o = 0; o < NACT; ++o) g[o] = (p[o] - (o == a ? 1.f : 0.f)) * tgt[r];
                     put_vec<HID, true, L::TA, L::BA2 * L::SA, true>(rowp + L::OA3, h2[r]);
                     put_vec<NOUT, false, L::TD, L::BD3 * L::SD, true>(rowp + L::OD3, g);
 #pragma unroll
@@ -384,6 +406,8 @@ struct GradCore {
                 }
                 put_vec<HID, false, L::TD, L::BD * L::SD, true>(rowp + L::OD2, d2[r]);
             }
+            // the next chunk of this warp: its targets may now overwrite this chunk's, which are consumed
+            staged = prefetch(c + cstep);
             // delta1[i] = (W2[i][:] . delta2) * lrelu'(z1[i]) for both rows; each W2 quad feeds 8 FFMA.  Computed one
             // stored quad (TD-blocked slot layout) at a time; quads of padding only are left to write_pads().
             f2 d2p[R][HID / 2];
@@ -459,7 +483,6 @@ struct GradCore {
         }
         __syncwarp();
     }
-
     }
 
     // CTA reduction in fixed order (bitwise reproducible): store(i, v) receives this CTA's gradient sums for the packed
@@ -560,7 +583,8 @@ constexpr int grad_smem_floats() {
     constexpr int tiles = NW * L::ROWS * L::RS;
     constexpr int red = NW * 32 * L::ACC_STRIDE + NW * (HID + 2);
     static_assert(tiles >= red, "the CTA reduction buffer reuses the tile region");
-    constexpr int stage = (grad_use_tma(NA) ? NW * L::ROWS * 3 * NA : 0) + 2 * NW + 8;   // staged rows + one mbarrier per warp
+    // staged rows + target slots + one mbarrier per warp
+    constexpr int stage = (grad_use_tma(NA) ? NW * L::ROWS * 3 * NA : 0) + NW * tgt_slot_floats(NA) + 2 * NW + 8;
     return round4(param_count(DIN, NOUT)) + tiles + stage + 16;
 }
 
