@@ -489,8 +489,36 @@ int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void
  * memory), a written range (the n_in dst rows, the n_in^2 weights) that overlaps an in-node row of any job of the
  * launch, and two written ranges of the launch that overlap. */
 #define RCMARL_NNM_MAX_FLOATS (48 * 1024)
-typedef enum { RCMARL_MIX_NNM = 0, RCMARL_MIX_BUCKET = 1, RCMARL_MIX_MOMENTUM = 2 } rcmarl_mixing_rule;
+typedef enum { RCMARL_MIX_NNM = 0, RCMARL_MIX_BUCKET = 1, RCMARL_MIX_MOMENTUM = 2, RCMARL_MIX_ARC = 3 } rcmarl_mixing_rule;
 int rcmarl_nnm_mix(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
+/* Adaptive robust clipping (rcmarl_arc_clip): the pre-aggregation step of Allouah et al., "Boosting Robustness by
+ * Clipping Gradients in Distributed Learning" (2024).  Before the receiver's rule runs,
+ * the k_clip received messages furthest from its own are pulled in along the line to its own message, to the distance
+ * of the (k_clip + 1)-th furthest; k_clip follows from H alone.  The paper clips gradient norms around the origin; the
+ * messages here are parameters, so ARC clips each message's offset from the receiver's own row.  It takes
+ * rcmarl_vector_job with rule = RCMARL_MIX_ARC; one job is one (receiver, net): n = n_in slots x_k = msgs + in_nodes[k]
+ * * msg_stride (x_0 the receiver's own; repeats in in_nodes count as separate slots), each of P = job.n floats,
+ * 0 <= H < n_in.  In fp32:
+ *   d_k      = sqrtf(squared distance of x_k and x_0) for k >= 1, the squared distance summed exactly as
+ *            rcmarl_vector_aggregate sums scclip's (one warp, lane-strided partials, then the fixed xor butterfly), so
+ *            d_k is bitwise scclip's d_k; a d_k that is not finite counts as +inf.
+ *   k_clip   = (2 * H * (n - H)) / n in integer division: the paper's floor(2 (f/n) (n - f)) at f = H (n = 4, H = 1: 1).
+ *   tau      = the (k_clip + 1)-th largest of d_1 .. d_{n-1}, or 0 if k_clip >= n - 1.
+ *   c_k      c_0 = 1; c_k = 0 if d_k is not finite, 1 if d_k <= tau, else tau / d_k (one IEEE division, __fdiv_rn).
+ *   Output   row k at dst + k * msg_stride: x_k bitwise if c_k = 1 (row 0 always), x_0 bitwise if c_k = 0, else
+ *            x_0,p + c_k * (x_k,p - x_0,p) with every operation rounded on its own (no FMA).  weights_out, when not
+ *            NULL, receives c [n_in].
+ * H = 0 passes every row through bitwise.  At most k_clip finite rows change, and a changed row lies at distance tau
+ * from x_0 up to rounding.  A +-inf or 1e30 message becomes x_0, so poisoned inputs never give poisoned rows.  NaN
+ * inputs are not supported.  Nothing is staged in shared memory, so P has no bound of its own.  One CTA per job, fixed
+ * summation orders, no atomics: bitwise reproducible, independent of the job order and of how jobs are split over
+ * launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, every dst row and weights_out untouched): n_jobs outside
+ * 1..RCMARL_MAX_JOBS, a null dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, a rule
+ * other than RCMARL_MIX_ARC, H outside [0, n_in), a written range (the n_in dst rows, the n_in weights) that overlaps an
+ * in-node row of any job of the launch, and two written ranges of the launch that overlap. */
+int rcmarl_arc_clip(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
 /* Randomized bucketing (rcmarl_bucket_mix): the pre-aggregation step of Karimireddy, He & Jaggi, "Byzantine-robust
  * learning on heterogeneous datasets via bucketing" (ICLR 2022).  The messages a receiver hears are shuffled into

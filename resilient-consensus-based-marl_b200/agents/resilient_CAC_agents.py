@@ -13,7 +13,9 @@ Same constructor and method names, argument meaning and mutation conventions as 
                                  mixing="bucket" or ("bucket", s) it keeps its own message and replaces the others by
                                  the means of random buckets of s (randomized bucketing, rcmarl_bucket_mix); with
                                  momentum=beta it replaces slot k's message by its net plus the moving average of
-                                 slot k's update against its net (per-neighbour momentum, rcmarl_momentum_mix)
+                                 slot k's update against its net (per-neighbour momentum, rcmarl_momentum_mix);
+                                 with clipping="arc" it then pulls the k_clip messages furthest from its own in to
+                                 the distance of the next (adaptive robust clipping, rcmarl_arc_clip), before mixing
   *_update_team             projection step on the output layer only (:60-84)
   actor_update              one Keras-Adam step weighted by the team TD error (:86-101)
 Tensors may be NumPy arrays, torch tensors or facade Tensors; they are moved to the GPU.  Calling these methods one
@@ -30,7 +32,7 @@ from rcmarl import nets, ops
 
 class RPBCAC_agent():
     def __init__(self, actor, critic, team_reward, slow_lr, fast_lr, gamma=0.95, H=0, aggregation="clip", mixing=None,
-                 momentum=None):
+                 momentum=None, clipping=None):
         self.actor = actor
         self.critic = critic
         self.TR = team_reward
@@ -60,6 +62,9 @@ class RPBCAC_agent():
             if self.mixing is not None:
                 raise L.RcmarlError(f"momentum and mixing {self.mixing!r} together: at most one pre-aggregation step")
         self.momentum = momentum
+        # adaptive robust clipping of the stacked rows (rcmarl_arc_clip) after the momentum step, before mixing: None
+        # or "arc"
+        self.clipping = L.check_clipping(clipping)
         self._momentum_M = [None, None]
         self._momentum_rows = [None, None]
         self.n_actions = self.actor.output_shape[1]
@@ -74,7 +79,7 @@ class RPBCAC_agent():
     def _resilient_aggregation(self, values_innodes):
         v = ops.dev_f32(values_innodes)
         shape = v.shape[1:]
-        v = self._mixed(v.reshape(v.shape[0], -1).contiguous(), net=0, round=0)
+        v = self._mixed(self._clipped(v.reshape(v.shape[0], -1).contiguous()), net=0, round=0)
         if self._whole_messages():                # the rows as whole vectors: out = sum_k w_k v_k
             out = self._with_aggregate(v)[-1]
         elif L.agg_rule(self.aggregation) == L.AGG_CLIP:
@@ -100,6 +105,18 @@ class RPBCAC_agent():
             return out
         out = torch.empty_like(stack)
         ops.nnm_mix([ops.vector_job(out, stack, P, P, list(range(n)), self.H, L.MIX_NNM)])
+        return out
+
+    def _clipped(self, stack):
+        """[n, P] device stack (own = row 0) -> its n rows clipped by ARC at H if the agent clips; else the stack."""
+        if self.clipping is None:
+            return stack
+        n, P = stack.shape
+        if not (1 <= n <= L.MAX_NEIGHBOURS and 0 <= self.H < n):
+            raise L.RcmarlError(f"clipping 'arc' with H={self.H} needs 0 <= H < n_in (n_in={n}, at most "
+                                f"{L.MAX_NEIGHBOURS})")
+        out = torch.empty_like(stack)
+        ops.arc_clip([ops.vector_job(out, stack, P, P, list(range(n)), self.H, L.MIX_ARC)])
         return out
 
     def _momentum_step(self, stack, ref, net):
@@ -143,8 +160,9 @@ class RPBCAC_agent():
     def _consensus_inputs(self, stack, net, round):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
         distance-based, dnc, mda or smea rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
-        Trainer.  An agent that mixes does so first (a bucketing agent with the draws of (net, round))."""
-        stack = self._mixed(stack, net, round)
+        Trainer.  An agent that clips does so first, then an agent that mixes does so (a bucketing agent with the draws
+        of (net, round))."""
+        stack = self._mixed(self._clipped(stack), net, round)
         if self._whole_messages():
             return self._with_aggregate(stack), [stack.shape[0]], 0, "clip"
         return stack, list(range(stack.shape[0])), self.H, self.aggregation

@@ -16,6 +16,8 @@
 //   subset_agg_kernel  exact subset selection (MDA, SMEA): averages the n - H messages that agree most as a set
 //                   (rcmarl_subset_aggregate)
 //   nnm_mix_kernel  nearest-neighbour mixing: each message becomes the mean of its n - H nearest (rcmarl_nnm_mix)
+//   arc_clip_kernel  adaptive robust clipping: the k_clip messages furthest from the receiver's own are pulled in to
+//                   the distance of the next (rcmarl_arc_clip)
 //   bucket_mix_kernel  randomized bucketing: the received messages are shuffled into buckets of s and replaced by the
 //                   bucket means (rcmarl_bucket_mix)
 //   adaptive_attack_kernel  min-max / min-sum Byzantine messages scaled to the receiver's honest spread
@@ -1006,6 +1008,59 @@ __global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_const
         const unsigned mask = sel[tid / nin];
         job.weights_out[tid] = ((mask >> (tid % nin)) & 1u) ? 1.f / (float)__popc(mask) : 0.f;
     }
+}
+
+// Adaptive robust clipping (rcmarl_arc_clip, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  Nothing is
+// staged: each d_k is summed by ONE warp with warp_sqdist straight from global memory, in the order scclip's d_k takes
+// in vector_rule, so the two are bitwise equal.  tau and the factors run on warp 0, one lane per slot; the rows take one
+// thread per coordinate, every operation rounded on its own (no FMA).
+__global__ void __launch_bounds__(VEC_THREADS) arc_clip_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    __shared__ float dist[MAXN];
+    __shared__ float cf[MAXN];
+    __shared__ float tau_at;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    auto row = [&](int k) { return job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride; };
+    const float* x0 = row(0);
+    for (int k = 1 + warp; k < nin; k += NW) {
+        const float d = sqrtf(warp_sqdist(row(k), x0, n, lane));
+        if (lane == 0) dist[k] = d;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        const int k = lane, kc = 2 * job.H * (nin - job.H) / nin;
+        if (k >= 1 && k < nin && kc < nin - 1) {      // tau = the d_k of descending rank k_clip (ties to the lower index)
+            const float dk = dist[k];
+            int r = 0;
+            for (int q = 1; q < nin; ++q) r += (dist[q] > dk || (dist[q] == dk && q < k)) ? 1 : 0;
+            if (r == kc) tau_at = dk;
+        }
+        __syncwarp();
+        const float tau = kc < nin - 1 ? tau_at : 0.f;
+        if (k < nin) {
+            const float dk = k == 0 ? 0.f : dist[k];
+            cf[k] = !isfinite(dk) ? 0.f : (dk <= tau ? 1.f : __fdiv_rn(tau, dk));
+        }
+    }
+    __syncthreads();
+    for (int k = 0; k < nin; ++k) {
+        const float c = cf[k];
+        const float* xk = row(k);
+        float* out = job.dst + (int64_t)k * job.msg_stride;
+        if (c == 1.f || c == 0.f) {                   // a bitwise copy of x_k or x_0: one row read
+            const float* src = c == 1.f ? xk : x0;
+            for (int p = tid; p < n; p += VEC_THREADS) out[p] = __ldg(src + p);
+        } else {
+            for (int p = tid; p < n; p += VEC_THREADS) {
+                const float a = __ldg(x0 + p);
+                out[p] = __fadd_rn(a, __fmul_rn(c, __fsub_rn(__ldg(xk + p), a)));
+            }
+        }
+    }
+    if (job.weights_out && tid < nin) job.weights_out[tid] = cf[tid];
 }
 
 // Randomized bucketing (rcmarl_bucket_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  Thread 0 draws
@@ -2410,6 +2465,27 @@ int rcmarl_nnm_mix(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
     return launch_staged<nnm_mix_kernel>(P, n_jobs, RCMARL_NNM_MAX_FLOATS, max_floats, VEC_THREADS, stream);
+}
+
+int rcmarl_arc_clip(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    RangeSet S;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.rule != RCMARL_MIX_ARC || q.H < 0 || q.H >= q.n_in) return RCMARL_ERR_ARG;
+        if (bad_nodes(q.in_nodes, q.n_in)) return RCMARL_ERR_ARG;
+        P.jobs[j] = q;
+        // writes the n_in dst rows and the n_in factors, reads the in-node rows
+        S.w.rows(q.dst, q.n_in, q.msg_stride, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
+    }
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    arc_clip_kernel<<<n_jobs, VEC_THREADS, 0, (cudaStream_t)stream>>>(P);
+    RC_CUDA(cudaGetLastError());
+    return RCMARL_OK;
 }
 
 int rcmarl_bucket_mix(const rcmarl_bucket_job* jobs, int n_jobs, void* stream) {

@@ -56,6 +56,7 @@ MIX_BUCKET = 1                                    # rcmarl_mixing_rule: randomiz
 BUCKET_DEFAULT_S = 2                              # the bucket size of a plain "bucket" entry
 BUCKET_MAX_S = 2 ** 31 - 1
 MIX_MOMENTUM = 2                                  # rcmarl_mixing_rule: per-neighbour momentum at beta, 0 <= beta < 1
+MIX_ARC = 3                                       # rcmarl_mixing_rule: adaptive robust clipping, clipping="arc"
 # pipeline-aware attacks (rcmarl_pipeline_attack): rcmarl_pipeline_mixing, the staging bound, the most shuffle samples
 # and the samples the trainer draws; the names are PIPELINE_ATTACKS
 PIPE_NONE, PIPE_NNM, PIPE_BUCKET = 0, 1, 2
@@ -196,6 +197,7 @@ SYMBOLS = [
     ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_subset_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_arc_clip", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
     ("rcmarl_momentum_mix", C.c_int, [C.POINTER(MomentumJob), C.c_int, c_fp]),
     ("rcmarl_adaptive_attack", C.c_int, [C.POINTER(AdaptiveAttackJob), C.c_int, c_fp]),
@@ -376,6 +378,19 @@ def check_momentum(beta):
     if not (math.isfinite(b) and 0.0 <= b < 1.0):
         raise RcmarlError(f"momentum needs a real beta in [0, 1), got {beta!r}")
     return float(beta)
+
+
+def check_clipping(name):
+    """Raise RcmarlError unless `name` is a pre-aggregation clipping entry: None or "arc" (adaptive robust clipping,
+    rcmarl_arc_clip).  Returns it."""
+    if name is None or (isinstance(name, str) and name == "arc"):
+        return name
+    raise RcmarlError(f"unknown clipping {name!r}: expected None or 'arc'")
+
+
+def arc_count(H, n):
+    """k_clip of rcmarl_arc_clip: how many of n messages ARC may clip at H, (2 H (n - H)) // n (include/rcmarl.h)."""
+    return (2 * int(H) * (int(n) - int(H))) // int(n)
 
 
 def is_adaptive_attack(name):

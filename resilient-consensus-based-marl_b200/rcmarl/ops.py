@@ -501,6 +501,13 @@ def nnm_mix(jobs):
     L.check(L.lib().rcmarl_nnm_mix(a, len(a), _stream()), "rcmarl_nnm_mix")
 
 
+def arc_clip(jobs):
+    """rcmarl_arc_clip over rcmarl_vector_job jobs (vector_job(dst, ..., rule=L.MIX_ARC, weights_out=[n_in])): clipped
+    row k goes to dst + k * msg_stride, the factors c to weights_out."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_arc_clip(a, len(a), _stream()), "rcmarl_arc_clip")
+
+
 def momentum_job(dst, msgs, msg_stride, n, in_nodes, ref, momentum, momentum_stride, beta, first):
     """rcmarl_momentum_job: in_nodes the receiver's message rows (own first); ref the reference c [>= n]; momentum the
     state M, row k at momentum + k * momentum_stride; beta in [0, 1); first 1 for the slots' first step

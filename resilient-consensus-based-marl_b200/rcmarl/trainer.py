@@ -29,7 +29,7 @@ class Trainer:
                  common_reward=False, mu=0.1, seed=0, device=None, rank=0, world=1, group=None,
                  perm_source=None, local_steps=5, mb_epochs=10, mb_times=32, actor_mb_times=200,
                  capacity_times=None, adam_state=None, scaling=True, fixed_initial_state=None, aggregation="clip",
-                 attack=None, mixing=None, momentum=None):
+                 attack=None, mixing=None, momentum=None, clipping=None):
         L.lib()
         # Any team size up to 16 (main.py:26): the kernels are instantiated for 5 and 16 agents, a team of n_real agents
         # runs on the next instantiation with the extra agent slots zero (inputs and W1 rows, rcmarl/nets.py) -- exactly the
@@ -121,12 +121,28 @@ class Trainer:
                 raise L.RcmarlError(f"agent {i} takes both momentum and mixing {self.mixing[i]!r}: at most one "
                                     "pre-aggregation step per agent")
             self.momentum[i] = beta
+        # Adaptive robust clipping (rcmarl_arc_clip) after a cooperative agent's momentum step and before its mixing
+        # step and rule, which then read n_in clipped rows with the same H: None, "arc" or one entry per agent
+        clip = list(clipping) if isinstance(clipping, (list, tuple)) else [clipping] * n_real
+        if len(clip) != n_real:
+            raise L.RcmarlError("clipping must be None, 'arc' or one entry per agent")
+        self.clipping = [None] * NA
+        for i in range(n_real):
+            L.check_clipping(clip[i])
+            if i in self.coop:                     # only cooperative agents aggregate: the name alone is checked
+                self.clipping[i] = clip[i]
         self._init_attacks(attack)
         for e in self.tailor_pairs + self.pipe_pairs:   # neither attack models the receiver's history
             b, j, _ = self.byz_pairs[e]
             if self.momentum[j] is not None:
                 raise L.RcmarlError(f"Byzantine agent {b} runs a {'tailored' if e in self.tailor_pairs else 'pipeline'} "
                                     f"attack against agent {j}, whose momentum the attack does not model")
+        for e in self.tailor_pairs + self.pipe_pairs + self.hist_pairs:   # none models the receiver's clipping
+            b, j, _ = self.byz_pairs[e]
+            if self.clipping[j] is not None:
+                name = 'tailored' if e in self.tailor_pairs else 'pipeline' if e in self.pipe_pairs else 'history'
+                raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose clipping "
+                                    f"{self.clipping[j]!r} the attack does not model")
         for e in self.tailor_pairs:                # rcmarl_tailored_attack models neither the DnC rule nor mixing
             b, j, _ = self.byz_pairs[e]
             if self.dnc[j]:
@@ -164,6 +180,12 @@ class Trainer:
         for i in self.mom_agents:
             self.mom_row[i] = row
             row += len(self.in_nodes[i])
+        # then the clipped rows of each cooperative agent that clips: slot k's row at arc_row[i] + k
+        self.arc_agents = [i for i in self.coop if self.clipping[i] is not None]
+        self.arc_row = {}
+        for i in self.arc_agents:
+            self.arc_row[i] = row
+            row += len(self.in_nodes[i])
         self.slow_lr = [float(slow_lr)] * NA if np.isscalar(slow_lr) else [float(x) for x in slow_lr] + [0.0] * (NA - n_real)
         self.max_ep_len, self.n_ep_fixed, self.n_epochs = int(max_ep_len), int(n_ep_fixed), int(n_epochs)
         self.block = self.max_ep_len * self.n_ep_fixed                    # time rows per fixed-policy block
@@ -195,10 +217,11 @@ class Trainer:
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
         # vec_row[i] / dnc_row[i] / subset_row[i] the aggregate of cooperative agent i's distance-based / dnc / mda or
-        # smea rule; mix_row[i] + k its mixed message k; mom_row[i] + k its momentum row of slot k
+        # smea rule; mix_row[i] + k its mixed message k; mom_row[i] + k its momentum row of slot k; arc_row[i] + k its
+        # clipped row of slot k
         n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + len(self.subset_agents) \
             + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents) \
-            + sum(len(self.in_nodes[i]) for i in self.mom_agents)
+            + sum(len(self.in_nodes[i]) for i in self.mom_agents) + sum(len(self.in_nodes[i]) for i in self.arc_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
         self.msg_t = torch.zeros(n_rows, self.PT, **f32)
         # w_k of each distance-based aggregate of the last epoch: row 2q critic, 2q + 1 TR of vec_agents[q]
@@ -211,6 +234,8 @@ class Trainer:
         # mixing matrix M (row-major [n_rows][n_in], n_rows = len(_rule_nodes(i))) of each agent that mixes: row 2q
         # critic, 2q + 1 TR of mix_agents[q]
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
+        # clipping factors c of each agent that clips: row 2q critic, 2q + 1 TR of arc_agents[q]
+        self.arc_weights = torch.zeros(2 * len(self.arc_agents), L.MAX_NEIGHBOURS, **f32) if self.arc_agents else None
         # gamma of each adaptive, tailored or pipeline attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         # the mimic attack's direction state z of each mimic pair (row q = mimic_pairs[q]; [q, 0, :PC] critic, [q, 1] TR),
@@ -329,13 +354,25 @@ class Trainer:
         row = {b: self.NA + e for e, (b, r, _) in enumerate(self.byz_pairs) if r == j}
         return [row.get(k, k) for k in self.in_nodes[j]]
 
-    def _rule_nodes(self, j):
-        """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, its momentum rows if it has
-        momentum, else _receiver_nodes(j)."""
+    def _momentum_nodes(self, j):
+        """The message rows cooperative agent j's clipping step reads: its momentum rows if it has momentum, else
+        _receiver_nodes(j)."""
         if self.momentum[j] is not None:
             return list(range(self.mom_row[j], self.mom_row[j] + len(self.in_nodes[j])))
+        return self._receiver_nodes(j)
+
+    def _clipped_nodes(self, j):
+        """The message rows cooperative agent j's mixing step reads: its clipped rows if it clips, else
+        _momentum_nodes(j)."""
+        if self.clipping[j] is not None:
+            return list(range(self.arc_row[j], self.arc_row[j] + len(self.in_nodes[j])))
+        return self._momentum_nodes(j)
+
+    def _rule_nodes(self, j):
+        """The message rows cooperative agent j's rule reads: its mixed rows if it mixes, else its clipped rows if it
+        clips, else its momentum rows if it has momentum, else _receiver_nodes(j)."""
         if self.mixing[j] is None:
-            return self._receiver_nodes(j)
+            return self._clipped_nodes(j)
         return list(range(self.mix_row[j], self.mix_row[j] + L.mixed_rows(self.mixing[j], len(self.in_nodes[j]))))
 
     def neighbour_weights(self):
@@ -344,7 +381,8 @@ class Trainer:
         crafted for i) in the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.
         For an agent that mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry
         is the effective weight w M of each in-neighbour.  For an agent with momentum, entry k is the weight of slot k's
-        momentum row."""
+        momentum row.  For an agent that clips, with w' that weight and c its clipping factors (clipping_factors), entry
+        k >= 1 is w'_k c_k and entry 0 is w'_0 + sum_{k >= 1} w'_k (1 - c_k): a clipped row is x_0 + c_k (x_k - x_0)."""
         out = {}
         for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights),
                                 (self.subset_agents, self.subset_weights)):
@@ -358,7 +396,25 @@ class Trainer:
             for i in out:
                 if i in mix:
                     out[i] = np.einsum("tk,tkl->tl", out[i].astype(np.float64), mix[i]).astype(np.float32)
+        if any(self.clipping[i] is not None for i in out):
+            clip = self.clipping_factors()
+            for i in out:
+                if i in clip:
+                    w, c = out[i].astype(np.float64), clip[i].astype(np.float64)
+                    eff = w * c
+                    eff[:, 0] = w[:, 0] + (w[:, 1:] * (1.0 - c[:, 1:])).sum(1)
+                    out[i] = eff.astype(np.float32)
         return out
+
+    def clipping_factors(self):
+        """{cooperative agent i that clips: float32 [2, n_in]}: the factors c_k of its clipping step (rcmarl_arc_clip;
+        c_0 = 1, in_nodes[i] order) in the last epoch of the last update round; row 0 for the critic, row 1 for the
+        team-reward net."""
+        if not self.arc_agents:
+            return {}
+        c = self.arc_weights.cpu().numpy()
+        self.d2h_bytes += c.nbytes
+        return {i: c[2 * q:2 * q + 2, :len(self.in_nodes[i])].copy() for q, i in enumerate(self.arc_agents)}
 
     def mixing_matrices(self):
         """{cooperative agent i that mixes: float32 [2, n_out, n_in]}: the mixing matrix M of the last epoch of the last
@@ -717,12 +773,12 @@ class Trainer:
         for q, i in enumerate(self.mix_agents):
             for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
                 if L.is_bucket_mixing(self.mixing[i]):
-                    bucket_jobs.append(ops.bucket_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i),
+                    bucket_jobs.append(ops.bucket_job(msgs[self.mix_row[i]], msgs, P, P, self._clipped_nodes(i),
                                                       self.mixing[i][1], seed=self.seed, receiver=i, net=t,
                                                       round=self.episodes_done & 0xFFFFFFFF,
                                                       weights_out=self.mix_weights[2 * q + t]))
                 else:
-                    mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._receiver_nodes(i),
+                    mix_jobs.append(ops.vector_job(msgs[self.mix_row[i]], msgs, P, P, self._clipped_nodes(i),
                                                    self.H[i], L.MIX_NNM, weights_out=self.mix_weights[2 * q + t]))
         mix_jobs = ops.job_array(L.VectorJob, mix_jobs) if mix_jobs else None
         # the momentum rows of the agents with momentum against their nets after the last consensus step (critic[i] /
@@ -733,6 +789,22 @@ class Trainer:
                 mom_jobs.append(ops.momentum_job(msgs[self.mom_row[i]], msgs, P, P, self._receiver_nodes(i), ref,
                                                  self.momentum_M[q, t], self.PT, self.momentum[i], 0))
         mom_jobs = ops.job_array(L.MomentumJob, mom_jobs) if mom_jobs else None
+        # the clipped rows of the agents that clip, from their momentum rows or the messages they hear: at most 16
+        # cooperative agents x 2 nets, so one launch per epoch, after the momentum launch and before the mixing launches
+        arc_jobs = []
+        for q, i in enumerate(self.arc_agents):
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                arc_jobs.append(ops.vector_job(msgs[self.arc_row[i]], msgs, P, P, self._momentum_nodes(i), self.H[i],
+                                               L.MIX_ARC, weights_out=self.arc_weights[2 * q + t]))
+        arc_jobs = ops.job_array(L.VectorJob, arc_jobs) if arc_jobs else None
+
+        def momentum_step():
+            if mom_jobs is not None:                                       # job 2q + t belongs to mom_agents[q]
+                for k, job in enumerate(mom_jobs):
+                    job.first = int(self.momentum_steps[k // 2] == 0)
+                ops.momentum_mix(mom_jobs)
+                self.launches += 1
+                self.momentum_steps = [s + 1 for s in self.momentum_steps]
         bucket_groups = [ops.job_array(L.BucketJob, bucket_jobs[g:g + L.MAX_JOBS])
                          for g in range(0, len(bucket_jobs), L.MAX_JOBS)]
         # distance-based aggregates over the messages each receiver hears (or their mixed rows): at most 16
@@ -810,6 +882,12 @@ class Trainer:
                     ops.mimic_attack(g)
                     self.launches += 1
                 self.mimic_steps = [s + u for s, u in zip(self.mimic_steps, update)]
+            # momentum, clipping and mixing touch disjoint agents' rows except momentum -> clipping -> mixing of an
+            # agent that clips, so without one the momentum launch keeps its place after the mixing launches
+            if arc_jobs is not None:
+                momentum_step()
+                ops.arc_clip(arc_jobs)
+                self.launches += 1
             if mix_jobs is not None:
                 ops.nnm_mix(mix_jobs)
                 self.launches += 1
@@ -818,12 +896,8 @@ class Trainer:
                     job.epoch = epoch
                 ops.bucket_mix(g)
                 self.launches += 1
-            if mom_jobs is not None:                                       # job 2q + t belongs to mom_agents[q]
-                for k, job in enumerate(mom_jobs):
-                    job.first = int(self.momentum_steps[k // 2] == 0)
-                ops.momentum_mix(mom_jobs)
-                self.launches += 1
-                self.momentum_steps = [s + 1 for s in self.momentum_steps]
+            if arc_jobs is None:
+                momentum_step()
             if vec_jobs is not None:
                 ops.vector_aggregate(vec_jobs)
                 self.launches += 1

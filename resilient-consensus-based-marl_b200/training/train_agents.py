@@ -43,6 +43,7 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
     attack = [getattr(ag, 'attack', None) for ag in agents]                # Byzantine_CAC_agent
     mixing = [getattr(ag, 'mixing', None) for ag in agents]                # RPBCAC_agent: None, "nnm" or ("bucket", s)
     momentum = [getattr(ag, 'momentum', None) for ag in agents]            # RPBCAC_agent: None or beta
+    clipping = [getattr(ag, 'clipping', None) for ag in agents]            # RPBCAC_agent: None or "arc"
     adam = [(ag.adam.m, ag.adam.v, ag.adam.t) if getattr(ag, 'adam', None) is not None and ag.adam.m is not None else None
             for ag in agents]
     rank, world = _dist_info()
@@ -54,7 +55,7 @@ def build_trainer(env, agents, args, exp_buffer=None, **overrides):
               n_ep_fixed=args['n_ep_fixed'], n_epochs=args['n_epochs'], buffer_size=args['buffer_size'],
               common_reward=bool(args['common_reward']), seed=int(args.get('random_seed', 0)), adam_state=adam,
               rank=rank, world=world, aggregation=aggregation, attack=attack, mixing=mixing,
-              momentum=momentum)
+              momentum=momentum, clipping=clipping)
     kw.update(overrides)
     tr = Trainer(**kw)
     if exp_buffer:                                                             # :36-40

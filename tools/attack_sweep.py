@@ -26,6 +26,11 @@ dnc included, but not mda or smea, whose cells are marked refused (their gamma i
 The momentum-aware attacks (rcmarl_history_attack: history_uv, history_std, history_sgn, range multiplier 2 by default)
 run the pipeline attack's search in a momentum receiver's momentum rows and invert its momentum step; against a
 receiver without momentum they are the pipeline attacks, and mda or smea cells are marked refused.
+Any of these rule names may take an arc+ prefix (e.g. arc+mkrum, arc+nnm+mkrum, arc+m0.9+scclip): every cooperative
+agent then clips its k_clip = 1 furthest message (adaptive robust clipping, rcmarl_arc_clip) after its momentum step and
+before its mixing step, and the weight reported for a whole-message rule is agent 4's effective weight through the
+clipping factors (Trainer.neighbour_weights).  No tailored, pipeline or history attack models clipping: those cells are
+marked refused.
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -70,8 +75,17 @@ out_dir = os.path.abspath(sys.argv[4] if len(sys.argv) > 4 else "attack_sweep_ou
 RULES = tuple((sys.argv[5] if len(sys.argv) > 5 else "clip,trim,wmsr").split(","))
 
 
+def split_clipping(rule):
+    """(clipping, the rest) of a rule name: "arc+nnm+mkrum" -> ("arc", "nnm+mkrum"), "mkrum" -> (None, "mkrum")."""
+    if rule.startswith("arc+"):
+        return "arc", rule[4:]
+    return None, rule
+
+
 def split_momentum(rule):
-    """(beta, the rest) of a rule name: "m0.9+scclip" -> (0.9, "scclip"), "scclip" -> (None, "scclip")."""
+    """(beta, the rest) of a rule name: "m0.9+scclip" -> (0.9, "scclip"), "scclip" -> (None, "scclip"); an arc prefix
+    is dropped."""
+    rule = split_clipping(rule)[1]
     if rule.startswith("m") and "+" in rule and rule[1:2].isdigit():
         beta, rest = rule[1:].split("+", 1)
         return float(beta), rest
@@ -278,7 +292,8 @@ for rule in RULES:
             try:
                 tr = Trainer(labels=["Cooperative"] * 4 + ["Byzantine"], in_nodes=bench.IN_NODES5, weights=w,
                              desired=z[f"{tag}/desired"], n_envs=n_envs, H=1, seed=int(ss[1:]), aggregation=base,
-                             attack=attack, mixing=mixing, momentum=split_momentum(rule)[0], **bench.HYPER)
+                             attack=attack, mixing=mixing, momentum=split_momentum(rule)[0],
+                             clipping=split_clipping(rule)[0], **bench.HYPER)
             except RcmarlError as ex:                   # e.g. a tailored attack against dnc, mda or mixing
                 refused = str(ex)
                 break
