@@ -712,6 +712,42 @@ typedef struct {
 } rcmarl_history_attack_job;
 int rcmarl_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, void* stream);
 
+/* ARC-aware Byzantine messages (rcmarl_pipeline_arc_attack, rcmarl_history_arc_attack): the pipeline and history attacks
+ * against a receiver j that clips (rcmarl_arc_clip) before its mixing step and rule.  Threat model: that of the base
+ * attack, plus j's clipping step, whose only parameter is the job's H.  The jobs are rcmarl_pipeline_attack_job and
+ * rcmarl_history_attack_job with every field's meaning unchanged; ARC runs on the rows the base attack hands on:
+ *   rcmarl_pipeline_arc_attack   the slot list x(gamma_i), before the mixing step (received -> ARC -> [nnm | bucket]
+ *                                -> rule);
+ *   rcmarl_history_arc_attack    the momentum rows (r_k of the real slots, a_k of the crafted ones), before the rule
+ *                                (received -> momentum -> ARC -> rule).
+ *   ARC.     For each candidate gamma_i, rcmarl_arc_clip's arithmetic bit for bit over those n_in rows y_k (y_0 = row 0,
+ *            the receiver's own, which must be real): d_k = sqrtf(the squared distance of y_k and y_0, summed as in
+ *            rcmarl_arc_clip), k_clip = (2 * H * (n_in - H)) / n_in, tau and c_k by its rank rule (the same device code);
+ *            the clipped row k is y_k bitwise if c_k = 1, y_0 bitwise if c_k = 0, else y_0,p + c_k * (y_k,p - y_0,p)
+ *            with every operation rounded on its own.  The mixing step (or, without mixing, the rule) reads the clipped
+ *            rows in place of the y_k.  The real slots' d_k do not depend on gamma_i and are taken once per job; under
+ *            bucketing ARC runs once per candidate, before the n_perms shuffle samples.
+ *   Everything else is the base attack's: mu, d and gamma_mm over the honest rows before ARC (the raw messages in the
+ *   pipeline form, the momentum rows in the history form), O_i = sum_p (R(gamma_i)_p - mu_p)^2, the pick, dst and
+ *   gamma_out; model_out = R(gamma_i*) (R_0 under bucketing) taken through ARC.
+ * At H = 0 (k_clip = 0) with finite rows, ARC is the identity, so dst, gamma_out and model_out are bitwise those of the
+ * base attack.  Exactness: under the base attack's conditions, model_out is bitwise what j computes from the messages
+ * actually sent -- [rcmarl_momentum_mix] -> rcmarl_arc_clip -> [rcmarl_nnm_mix] -> rcmarl_consensus_hidden over all n
+ * parameters (COORD), rcmarl_vector_aggregate (VECTOR) or rcmarl_dnc_aggregate (SPECTRAL); under bucketing, with the
+ * attacker's sample 0 in place of j's secret shuffle.  +-inf or 1e30 real rows get c_k = 0 (they become y_0), as in
+ * rcmarl_arc_clip.  NaN inputs are not supported.  One CTA per job: the clipped rows (at most k_clip of them) are staged
+ * in shared memory behind the base attack's staging; fixed summation orders, no atomics -- bitwise reproducible,
+ * independent of the job order and of how jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, gamma_out and model_out untouched): everything the base entry point
+ * refuses, a crafted slot 0, and a job whose base staging size plus k_clip * n floats exceeds the base bound
+ * (RCMARL_PIPELINE_MAX_FLOATS / RCMARL_HISTORY_MAX_FLOATS).  At the 16-agent team-reward net (1421 parameters) with
+ * n_in = 16 and 15 real slots, those bounds admit: the pipeline form without mixing, and under bucketing with s >= 2,
+ * every H; under bucketing with s = 1 k_clip <= 3 (H <= 2) without DnC and k_clip <= 1 (H = 1) with DnC; under nnm
+ * k_clip <= 2 (H = 1) without DnC and no H >= 1 with DnC.  The history form: k_clip <= 2 (H = 1) without DnC and no
+ * H >= 1 with DnC.  Every shape of the 5-agent team (n_in <= 5, at most 761 parameters) is admitted. */
+int rcmarl_pipeline_arc_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, void* stream);
+int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, void* stream);
+
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]
  *                                              + sum_t scale_t * net_t(x_kind_t(row))

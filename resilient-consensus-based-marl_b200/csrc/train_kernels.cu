@@ -1010,6 +1010,25 @@ __global__ void __launch_bounds__(VEC_THREADS) nnm_mix_kernel(const __grid_const
     }
 }
 
+// ARC's factors (rcmarl_arc_clip, include/rcmarl.h) on one warp, lane k for slot k: tau = the d_k (dist[1 .. nin - 1])
+// of descending rank k_clip, ties to the lower index (0 if k_clip >= nin - 1), then cf[k] for k < nin.  tau_at is shared
+// scratch.  Shared by arc_clip_kernel and the ARC forms of the pipeline and history searches.
+__device__ __forceinline__ void arc_factors(const float* dist, int nin, int H, float& tau_at, float* cf, int lane) {
+    const int k = lane, kc = 2 * H * (nin - H) / nin;
+    if (k >= 1 && k < nin && kc < nin - 1) {
+        const float dk = dist[k];
+        int r = 0;
+        for (int q = 1; q < nin; ++q) r += (dist[q] > dk || (dist[q] == dk && q < k)) ? 1 : 0;
+        if (r == kc) tau_at = dk;
+    }
+    __syncwarp();
+    const float tau = kc < nin - 1 ? tau_at : 0.f;
+    if (k < nin) {
+        const float dk = k == 0 ? 0.f : dist[k];
+        cf[k] = !isfinite(dk) ? 0.f : (dk <= tau ? 1.f : __fdiv_rn(tau, dk));
+    }
+}
+
 // Adaptive robust clipping (rcmarl_arc_clip, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  Nothing is
 // staged: each d_k is summed by ONE warp with warp_sqdist straight from global memory, in the order scclip's d_k takes
 // in vector_rule, so the two are bitwise equal.  tau and the factors run on warp 0, one lane per slot; the rows take one
@@ -1030,21 +1049,7 @@ __global__ void __launch_bounds__(VEC_THREADS) arc_clip_kernel(const __grid_cons
         if (lane == 0) dist[k] = d;
     }
     __syncthreads();
-    if (warp == 0) {
-        const int k = lane, kc = 2 * job.H * (nin - job.H) / nin;
-        if (k >= 1 && k < nin && kc < nin - 1) {      // tau = the d_k of descending rank k_clip (ties to the lower index)
-            const float dk = dist[k];
-            int r = 0;
-            for (int q = 1; q < nin; ++q) r += (dist[q] > dk || (dist[q] == dk && q < k)) ? 1 : 0;
-            if (r == kc) tau_at = dk;
-        }
-        __syncwarp();
-        const float tau = kc < nin - 1 ? tau_at : 0.f;
-        if (k < nin) {
-            const float dk = k == 0 ? 0.f : dist[k];
-            cf[k] = !isfinite(dk) ? 0.f : (dk <= tau ? 1.f : __fdiv_rn(tau, dk));
-        }
-    }
+    if (warp == 0) arc_factors(dist, nin, job.H, tau_at, cf, lane);
     __syncthreads();
     for (int k = 0; k < nin; ++k) {
         const float c = cf[k];
@@ -1438,6 +1443,63 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) tailored_attack_kernel(const _
 struct PipelineParams { rcmarl_pipeline_attack_job jobs[RCMARL_MAX_JOBS]; };
 static_assert(ADA_THREADS == VEC_THREADS, "dnc_rule, nnm_rows, bucket_means and vector_rule stride by VEC_THREADS");
 
+// The receiver's ARC step inside the ARC forms of the pipeline and history searches (rcmarl_pipeline_arc_attack,
+// rcmarl_history_arc_attack): d_k and c_k of each slot, and the row the next stage reads for slot k at xs + off[k].
+struct ArcShared {
+    float dist[RCMARL_MAX_NEIGHBOURS], cf[RCMARL_MAX_NEIGHBOURS], tau;
+    int off[RCMARL_MAX_NEIGHBOURS];
+};
+
+// dist[k] = d_k = sqrtf(squared distance of slot k's row and slot 0's) for each slot k >= 1 of `mask`, each summed by
+// ONE warp with warp_sqdist as in arc_clip_kernel (slot k's row at xs + off[k]).  Called by the whole CTA; the caller
+// synchronises before reading dist.
+__device__ __forceinline__ void arc_dist(const float* xs, const int* off, int n, int nin, unsigned mask, float* dist) {
+    constexpr int NW = ADA_THREADS / 32;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int k = 1 + warp; k < nin; k += NW)
+        if ((mask >> k) & 1u) {
+            const float d = sqrtf(warp_sqdist(xs + off[k], xs + off[0], n, lane));
+            if (lane == 0) dist[k] = d;
+        }
+}
+
+// ARC of one candidate, called by the whole CTA once the slot rows (slot k at xs + off[k], slot 0 real) are complete and
+// A.dist holds d_k of every slot whose row does not depend on the candidate: d_k of the slots of `sum` is summed here,
+// each slot of `copy` takes d_from's; then the factors (arc_factors) and A.off[k]: slot k's own row if c_k = 1, slot 0's
+// if c_k = 0, else a row of its own in clip (at most k_clip of them), x_0 + c_k (x_k - x_0) with every operation rounded
+// on its own (arc_clip_kernel's arithmetic).  The clipped rows are complete on return.
+__device__ __forceinline__ void arc_rows(float* xs, const int* off, int n, int nin, int H, unsigned sum, unsigned copy,
+                                         int from, float* clip, ArcShared& A) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    arc_dist(xs, off, n, nin, sum, A.dist);
+    __syncthreads();
+    if (warp == 0) {
+        if (lane < nin && ((copy >> lane) & 1u)) A.dist[lane] = A.dist[from];
+        __syncwarp();
+        arc_factors(A.dist, nin, H, A.tau, A.cf, lane);
+        __syncwarp();
+        if (lane == 0)
+            for (int k = 0, c = 0; k < nin; ++k) {
+                const float ck = A.cf[k];
+                A.off[k] = ck == 1.f ? off[k] : ck == 0.f ? off[0] : (int)(clip - xs) + n * c++;
+            }
+    }
+    __syncthreads();
+    const float* x0 = xs + off[0];
+    for (int k = 1; k < nin; ++k) {
+        const float c = A.cf[k];
+        if (c == 1.f || c == 0.f) continue;
+        const float* xk = xs + off[k];
+        float* out = xs + A.off[k];
+        for (int p = tid; p < n; p += ADA_THREADS) {
+            const float a = x0[p];
+            out[p] = __fadd_rn(a, __fmul_rn(c, __fsub_rn(xk[p], a)));
+        }
+    }
+    __syncthreads();
+}
+
+template <bool ARC>
 __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const __grid_constant__ PipelineParams P) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     extern __shared__ __align__(16) float smem[];
@@ -1447,6 +1509,7 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
     __shared__ unsigned members[RCMARL_PIPELINE_MAX_PERMS * MAXN];   // bucketing: bucket b of sample q at [q * MAXN + b]
     __shared__ int pi[MAXN];
     __shared__ int roff[MAXN];                                       // the rule's row k at xs + roff[k]
+    __shared__ ArcShared A;                                          // ARC
     const rcmarl_pipeline_attack_job& pj = P.jobs[blockIdx.x];
     const rcmarl_tailored_attack_job& job = pj.attack;
     const int n = job.n, nin = job.n_in;
@@ -1465,7 +1528,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
     float* d = mu + n;                             // [n]
     float* cand = d + n;                           // [n]: m(gamma_i), every crafted slot
     float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
-    float* mixed = z + n;                          // nnm: [n_in][n]; bucketing: [nb][n]
+    float* mixed = z + n;                          // nnm: [n_in][n]; bucketing: [nb][n]; then ARC: [k_clip][n]
+    const int n_mixed = pj.mixing == RCMARL_PIPE_NNM ? nin : nb;
     if (tid == 0 && bucket)
         for (int q = 0; q < nq; ++q)
             bucket_draw(make_uint4((uint32_t)q << 2, pj.attacker | pj.receiver << 8 | pj.net << 16 | 0x10000000u,
@@ -1479,8 +1543,23 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
                     : k == 0 ? S.off[0] : base + (k - 1) * n;
     }
     __syncthreads();
-    const SlotRows slots{xs, S.off}, rows{xs, roff};
+    const int *soff = S.off, *ooff = roff;        // the rows the mixing step and the rule read
+    unsigned real = 0u;                           // ARC: the real slots, and the first crafted one
+    int from = 0;
+    if constexpr (ARC) {
+        for (int k = nin - 1; k >= 0; --k)
+            if (job.slots[k] >= 0) real |= 1u << k;
+            else from = k;
+        arc_dist(xs, S.off, n, nin, real, A.dist);  // the real slots' d_k, once per job
+        soff = A.off;
+        if (pj.mixing == RCMARL_PIPE_NONE) ooff = A.off;
+    }
+    const SlotRows slots{xs, soff}, rows{xs, ooff};
     const auto eval = [&](int q) {
+        if constexpr (ARC)                        // once per candidate: every crafted slot holds it, one d_k for all
+            if (q == 0)
+                arc_rows(xs, S.off, n, nin, job.H, 1u << from, ~real & ~(1u << from) & ((1u << nin) - 1u), from,
+                         mixed + (int64_t)n_mixed * n, A);
         if (pj.mixing == RCMARL_PIPE_NNM) {
             nnm_rows(slots, n, nin, job.H, S.dist, sel, [&](int k) { return mixed + k * n; });
             __syncthreads();                                          // the mixed rows complete
@@ -1569,10 +1648,12 @@ __device__ __forceinline__ float momentum_invert(float t, float c, const float* 
     return __fadd_rn(c, __fdiv_rn(__fsub_rn(__fsub_rn(t, c), __fmul_rn(beta, old)), __fsub_rn(1.f, beta)));
 }
 
+template <bool ARC>
 __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __grid_constant__ HistoryParams P) {
     extern __shared__ __align__(16) float smem[];
     __shared__ TailoredShared S;
     __shared__ DncShared D;
+    __shared__ ArcShared A;                        // ARC
     const rcmarl_history_attack_job& hj = P.jobs[blockIdx.x];
     const rcmarl_tailored_attack_job& job = hj.attack;
     const int n = job.n, nin = job.n_in;
@@ -1590,6 +1671,7 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
     float* cand = d + n;                           // [n]: the target t(gamma_i)
     float* z = cand + n;                           // [n]: the rule's output (and GMED's iterate)
     float* crafted = z + n;                        // [n_in - nr][n]: a_k of each crafted slot, in slot order
+    float* clip = crafted + (int64_t)(nin - nr) * n;   // ARC: [k_clip][n]
     tailored_stage(job, nh, xs, cand, S);
     if (tid == 0)                                  // each crafted slot to a row of its own
         for (int k = 0, c = 0; k < nin; ++k)
@@ -1606,8 +1688,13 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
         }
     }
     __syncthreads();
+    unsigned real = 0u;                            // ARC: the real slots
+    if constexpr (ARC) {
+        for (int k = 0; k < nin; ++k) real |= job.slots[k] >= 0 ? 1u << k : 0u;
+        arc_dist(xs, S.off, n, nin, real, A.dist); // the real slots' d_k, once per job
+    }
     const float range = tailored_range(job, nh, xs, mu, d, S);
-    const SlotRows rows{xs, S.off};
+    const SlotRows rows{xs, ARC ? A.off : S.off};
     // a_k of every crafted slot for the target in cand, then the rule into z; returns whether every crafted message is
     // finite (the same in every thread).  An infeasible candidate skips the rule unless `always`: its objective is -inf
     // whatever the rule gives.
@@ -1628,6 +1715,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
         }
         const bool ok = !__syncthreads_or(bad);    // the crafted rows complete
         if (!ok && !always) return false;
+        if constexpr (ARC)                         // one d_k per crafted slot: colluders' rows differ
+            arc_rows(xs, S.off, n, nin, job.H, ~real & ((1u << nin) - 1u), 0u, 0, clip, A);
         if (job.family == RCMARL_TAILOR_COORD)
             coord_rule(rows, n, nin, job.H, job.rule, z);
         else if (job.family == RCMARL_TAILOR_VECTOR)
@@ -2606,7 +2695,17 @@ int rcmarl_tailored_attack(const rcmarl_tailored_attack_job* jobs, int n_jobs, v
                                                  stream);
 }
 
-int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
+}  // extern "C"
+
+// ARC's staging in an ARC form of the pipeline or history search: k_clip rows, and slot 0 (the receiver's own) real
+static bool arc_staging(const rcmarl_tailored_attack_job& q, bool arc, int64_t& floats) {
+    if (!arc) return false;
+    floats += (int64_t)(2 * q.H * (q.n_in - q.H) / q.n_in) * q.n;
+    return q.slots[0] < 0;
+}
+
+template <bool ARC>
+static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     PipelineParams P;
     RangeSet S;
@@ -2628,8 +2727,8 @@ int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
             return RCMARL_ERR_ARG;
         }
         if (bad_receiver_rule(q.family, q.rule, q.H, n_rows)) return RCMARL_ERR_ARG;
-        const int64_t floats = (int64_t)(n_real + n_mixed + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
-        if (floats > RCMARL_PIPELINE_MAX_FLOATS) return RCMARL_ERR_ARG;
+        int64_t floats = (int64_t)(n_real + n_mixed + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        if (arc_staging(q, ARC, floats) || floats > RCMARL_PIPELINE_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = pj;
         // writes dst, gamma_out and model_out, reads the real slots' rows
@@ -2639,11 +2738,12 @@ int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<pipeline_attack_kernel>(P, n_jobs, RCMARL_PIPELINE_MAX_FLOATS, max_floats, ADA_THREADS,
-                                                 stream);
+    return launch_staged<pipeline_attack_kernel<ARC>>(P, n_jobs, RCMARL_PIPELINE_MAX_FLOATS, max_floats, ADA_THREADS,
+                                                      stream);
 }
 
-int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
+template <bool ARC>
+static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     HistoryParams P;
     RangeSet S;
@@ -2659,8 +2759,8 @@ int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         if (hj.own_mask == 0u || (hj.own_mask >> q.n_in)) return RCMARL_ERR_ARG;
         for (int k = 0; k < q.n_in; ++k)
             if (((hj.own_mask >> k) & 1u) && q.slots[k] >= 0) return RCMARL_ERR_ARG;   // an own bit on a real slot
-        const int64_t floats = (int64_t)(q.n_in + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
-        if (floats > RCMARL_HISTORY_MAX_FLOATS) return RCMARL_ERR_ARG;
+        int64_t floats = (int64_t)(q.n_in + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        if (arc_staging(q, ARC, floats) || floats > RCMARL_HISTORY_MAX_FLOATS) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = hj;
         // writes dst, gamma_out and model_out, reads the real slots' rows, the ref and the n_in M rows
@@ -2672,7 +2772,26 @@ int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         S.r.rows(hj.momentum, q.n_in, hj.momentum_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<history_attack_kernel>(P, n_jobs, RCMARL_HISTORY_MAX_FLOATS, max_floats, ADA_THREADS, stream);
+    return launch_staged<history_attack_kernel<ARC>>(P, n_jobs, RCMARL_HISTORY_MAX_FLOATS, max_floats, ADA_THREADS,
+                                                     stream);
+}
+
+extern "C" {
+
+int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
+    return pipeline_attack<false>(jobs, n_jobs, stream);
+}
+
+int rcmarl_pipeline_arc_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
+    return pipeline_attack<true>(jobs, n_jobs, stream);
+}
+
+int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
+    return history_attack<false>(jobs, n_jobs, stream);
+}
+
+int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
+    return history_attack<true>(jobs, n_jobs, stream);
 }
 
 int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* stream) {

@@ -204,6 +204,8 @@ SYMBOLS = [
     ("rcmarl_tailored_attack", C.c_int, [C.POINTER(TailoredAttackJob), C.c_int, c_fp]),
     ("rcmarl_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, c_fp]),
     ("rcmarl_history_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, c_fp]),
+    ("rcmarl_pipeline_arc_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, c_fp]),
+    ("rcmarl_history_arc_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, c_fp]),
     ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
     ("rcmarl_mimic_attack", C.c_int, [C.POINTER(MimicJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -448,6 +450,23 @@ def is_history_attack(name):
     return isinstance(name, str) and name in HISTORY_ATTACKS
 
 
+class ArcAttackKind(int):
+    """The kind check_attack gives an ARC-aware attack (rcmarl_pipeline_arc_attack / rcmarl_history_arc_attack): its
+    rcmarl_adaptive_dev, as a type of its own so that it is told apart from the pipeline and history attacks, which do
+    not model the receiver's clipping."""
+
+    def __repr__(self):
+        return f"ArcAttackKind({int(self)})"
+
+
+ARC_ATTACKS = {f"arc_{d}": ArcAttackKind(dev) for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+
+
+def is_arc_attack(name):
+    """True for the name of an ARC-aware attack: "arc_uv", "arc_std", "arc_sgn"."""
+    return isinstance(name, str) and name in ARC_ATTACKS
+
+
 class DissensusKind(int):
     """The kind check_attack gives the dissensus attack (rcmarl_dissensus_attack), a type of its own so that it is told
     apart from the other attacks' kinds; its parameter is eps >= 0."""
@@ -469,30 +488,33 @@ STATE_ATTACKS = {"dissensus": DissensusKind(0), "mimic": MimicKind(0)}
 
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss", the adaptive, the tailored, the pipeline and the history attacks and "dissensus" also >= 0; for "mimic" an
-    integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack /
-    rcmarl_pipeline_attack / rcmarl_history_attack / rcmarl_dissensus_attack / rcmarl_mimic_attack require
+    "gauss", the adaptive, the tailored, the pipeline, the history and the ARC attacks and "dissensus" also >= 0; for
+    "mimic" an integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack /
+    rcmarl_pipeline_attack / rcmarl_history_attack / rcmarl_pipeline_arc_attack / rcmarl_history_arc_attack /
+    rcmarl_dissensus_attack / rcmarl_mimic_attack require
     (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
     the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the
     paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, the PipelineKind of a pipeline
-    attack and the HistoryKind of a history attack, whose parameter is the range multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
+    attack, the HistoryKind of a history attack and the ArcAttackKind of an ARC attack, whose parameter is the range
+    multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
     and MimicKind for "mimic", whose parameter is T0 (the power steps each pair takes before its direction freezes)."""
     try:
         name, param = attack
         param = float(param)
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
-    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **PIPELINE_ATTACKS, **HISTORY_ATTACKS, **STATE_ATTACKS}
+    known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **PIPELINE_ATTACKS, **HISTORY_ATTACKS, **ARC_ATTACKS,
+             **STATE_ATTACKS}
     if not isinstance(name, str) or name not in known:
         names = sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(PIPELINE_ATTACKS) \
-            + sorted(HISTORY_ATTACKS) + sorted(STATE_ATTACKS)
+            + sorted(HISTORY_ATTACKS) + sorted(ARC_ATTACKS) + sorted(STATE_ATTACKS)
         raise RcmarlError(f"unknown attack {name!r}: expected one of {names}")
     if name == "mimic":
         if not (math.isfinite(param) and param == int(param) and 0 <= param <= MIMIC_MAX_T0):
             raise RcmarlError(f"attack 'mimic' needs an integer T0 in 0 .. {MIMIC_MAX_T0}, got {param}")
         return known[name], param
     nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS \
-        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS
+        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS or name in ARC_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
     return known[name], param

@@ -151,12 +151,21 @@ class Trainer:
             if self.mixing[j] is not None:
                 raise L.RcmarlError(f"Byzantine agent {b} runs a tailored attack against agent {j}, whose mixing "
                                     f"{self.mixing[j]!r} the tailored attack does not model")
-        for e in self.tailor_pairs + self.pipe_pairs + self.hist_pairs:   # none models the subset-selection rules
+        for e in self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs:   # none models mda / smea
             b, j, _ = self.byz_pairs[e]
             if self.subset_rule[j] is not None:
-                name = 'tailored' if e in self.tailor_pairs else 'pipeline' if e in self.pipe_pairs else 'history'
+                name = ('tailored' if e in self.tailor_pairs else 'pipeline' if e in self.pipe_pairs
+                        else 'history' if e in self.hist_pairs else 'ARC')
                 raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose rule "
                                     f"{agg[j]!r} the attack does not model")
+        for e in self.arc_pairs:                   # an ARC job stages k_clip clipped rows on top of its base job's
+            b, j, _ = self.byz_pairs[e]
+            n_real = sum(k >= 0 for k in self._tailored_slots(j)[0])
+            kc = L.arc_count(self.H[j], len(self.in_nodes[j])) if self.clipping[j] is not None else 0
+            floats, bound = self._arc_staging(j, n_real, kc)
+            if floats > bound:
+                raise L.RcmarlError(f"Byzantine agent {b} runs an ARC attack against agent {j}, whose job stages "
+                                    f"{floats} floats, more than the {bound} the library admits")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
         # that of each cooperative agent on dnc, then that of each on mda / smea
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
@@ -236,7 +245,8 @@ class Trainer:
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
         # clipping factors c of each agent that clips: row 2q critic, 2q + 1 TR of arc_agents[q]
         self.arc_weights = torch.zeros(2 * len(self.arc_agents), L.MAX_NEIGHBOURS, **f32) if self.arc_agents else None
-        # gamma of each adaptive, tailored or pipeline attack of the last epoch: row q = gamma_pairs[q], columns critic, TR
+        # gamma of each adaptive, tailored, pipeline, history or ARC attack of the last epoch: row q = gamma_pairs[q],
+        # columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         # the mimic attack's direction state z of each mimic pair (row q = mimic_pairs[q]; [q, 0, :PC] critic, [q, 1] TR),
         # the index into S_j each copied in the last epoch, and the power steps each has taken (host)
@@ -341,7 +351,12 @@ class Trainer:
         # receiver with momentum a launch of their own, after the pipeline one; against one without, a pipeline job
         self.hist_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                            if isinstance(self.attack[b][0], L.HistoryKind)]
-        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs
+        # the pairs whose attacker runs an ARC-aware attack (kind L.ArcAttackKind): the history or pipeline search
+        # through the receiver's whole chain, its clipping step included (rcmarl_history_arc_attack /
+        # rcmarl_pipeline_arc_attack); launches of their own, after the history ones (_arc_job_groups)
+        self.arc_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                          if isinstance(self.attack[b][0], L.ArcAttackKind)]
+        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs
         # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
         # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
         # tailored one
@@ -433,11 +448,11 @@ class Trainer:
         return out
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline or a history attack:
-        float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
-        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline or history attack gamma_i*,
-        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack); entry 0 for the critic, 1 for the
-        team-reward net."""
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline, a history or an ARC
+        attack: float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
+        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline, history or ARC attack gamma_i*,
+        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / their ARC forms); entry 0 for the
+        critic, 1 for the team-reward net."""
         if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
@@ -465,6 +480,62 @@ class Trainer:
         honest = [k for k, i in enumerate(self.in_nodes[j]) if self.labels[i] == COOP]
         return slots, honest
 
+    def _arc_staging(self, j, n_real, kc):
+        """(floats, bound) of the job an ARC pair against receiver j gets (include/rcmarl.h): the history form's
+        (n_in + 4 + (DnC ? 2 : 0) + k_clip) * PT if j has momentum, else the pipeline form's (n_real + n_mixed + 4 +
+        (DnC ? 2 : 0) + k_clip) * PT, with k_clip = kc (0 when j does not clip)."""
+        n_in, extra = len(self.in_nodes[j]), (2 if self.dnc[j] else 0) + 4 + kc
+        PT = L.param_count(3 * self.NA, 1)             # the TR net, the larger of the two
+        if self.momentum[j] is not None:
+            return (n_in + extra) * PT, L.HISTORY_MAX_FLOATS
+        mix = self.mixing[j]
+        n_mixed = 0 if mix is None else n_in if mix == "nnm" else L.mixed_rows(mix, n_in) - 1
+        return (n_real + n_mixed + extra) * PT, L.PIPELINE_MAX_FLOATS
+
+    def _arc_job_groups(self):
+        """The job tables of the ARC pairs' messages update_round launches in every epoch, after the history
+        launches: a list of (launch, group, mom), each group of at most MAX_JOBS jobs, with mom the momentum agent index
+        of each job of a history-form group (its `first` is set per epoch) and None for a pipeline-form group (its
+        `epoch` is set per epoch).  Per pair one critic and one TR job: against a receiver that clips, the history form
+        (momentum) or the pipeline form (with the receiver's mixing) through its clipping step; against one that does
+        not, exactly the job a history pair gets."""
+        NA = self.NA
+        mom_index = {i: q for q, i in enumerate(self.mom_agents)}
+        n_before = len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs) + len(self.hist_pairs)
+        tables = {}                                    # (history form, clips) -> ([jobs], [mom])
+        for q_pair, e in enumerate(self.arc_pairs):
+            b, j, _ = self.byz_pairs[e]
+            kind, param = self.attack[b]
+            slots, hon = self._tailored_slots(j)
+            rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
+                    else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
+                    else (L.TAILOR_COORD, self.aggregation[j]))
+            hist = self.momentum[j] is not None
+            jobs, moms = tables.setdefault((hist, self.clipping[j] is not None), ([], []))
+            for t, (msgs, P, ref) in enumerate(((self.msg_c, self.PC, self.critic[j]), (self.msg_t, self.PT, self.tr[j]))):
+                gamma_out = self.att_gamma[n_before + q_pair, t:t + 1]
+                if hist:
+                    q = mom_index[j]
+                    own = [k for k, i in enumerate(self.in_nodes[j]) if i == b]
+                    jobs.append(ops.history_attack_job(
+                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, ref,
+                        self.momentum_M[q, t], self.PT, self.momentum[j], 0, own, gamma_out=gamma_out))
+                    moms.append(q)
+                else:
+                    jobs.append(ops.pipeline_attack_job(
+                        msgs[NA + e], msgs, P, P, slots, hon, rule, self.H[j], kind, param, mixing=self.mixing[j],
+                        n_perms=L.PIPELINE_PERMS, seed=self.seed, attacker=b, receiver=j, net=t,
+                        round=self.episodes_done & 0xFFFFFFFF, gamma_out=gamma_out))
+        launch = {(True, True): ops.history_arc_attack, (True, False): ops.history_attack,
+                  (False, True): ops.pipeline_arc_attack, (False, False): ops.pipeline_attack}
+        cls = {True: L.HistoryAttackJob, False: L.PipelineAttackJob}
+        out = []
+        for (hist, clips), (jobs, moms) in sorted(tables.items(), reverse=True):
+            for g in range(0, len(jobs), L.MAX_JOBS):
+                out.append((launch[(hist, clips)], ops.job_array(cls[hist], jobs[g:g + L.MAX_JOBS]),
+                            moms[g:g + L.MAX_JOBS] if hist else None))
+        return out
+
     def _attack_job_groups(self):
         """The job tables of the Byzantine messages update_round launches in every epoch, each in groups of MAX_JOBS:
         (attack, adaptive, tailored, pipeline, history, dissensus, mimic groups), with the history groups and the mimic
@@ -490,7 +561,10 @@ class Trainer:
         mom_index = {i: q for q, i in enumerate(self.mom_agents)}
         diss_set = set(self.diss_pairs)
         mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
+        arc_set = set(self.arc_pairs)                  # their jobs are _arc_job_groups'
         for e, (b, j, honest) in enumerate(self.byz_pairs):
+            if e in arc_set:
+                continue
             kind, param = self.attack[b]
             if e in diss_set:
                 # colluding dissensus attackers of j split the cancellation: n_byz counts their entries of in_nodes[j]
@@ -764,6 +838,7 @@ class Trainer:
         # the Byzantine messages' job tables (_attack_job_groups)
         (att_groups, ada_groups, tail_groups, pipe_groups, hist_groups, hist_mom, diss_groups, mimic_t0,
          mimic_groups) = self._attack_job_groups()
+        arc_groups = self._arc_job_groups()
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
         # 16 cooperative agents x 2 nets, so one nnm launch and one bucketing launch per epoch.  A bucketing job draws
@@ -870,6 +945,14 @@ class Trainer:
                 for k, job in enumerate(g):
                     job.first = int(self.momentum_steps[hist_mom[g0 + k]] == 0)
                 ops.history_attack(g)
+                self.launches += 1
+            for launch, g, mom in arc_groups:                             # as the pipeline and history groups
+                for k, job in enumerate(g):
+                    if mom is None:
+                        job.epoch = epoch
+                    else:
+                        job.first = int(self.momentum_steps[mom[k]] == 0)
+                launch(g)
                 self.launches += 1
             for g in diss_groups:                                          # no epoch dependence either
                 ops.dissensus_attack(g)
