@@ -256,7 +256,10 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs_host, int n_jo
  * written ranges (dsts, gamma_outs) of the launch that overlap.  NaN inputs are not supported. */
 #define RCMARL_TAILORED_STEPS 32
 #define RCMARL_TAILORED_MAX_FLOATS (19 * 1536)
-typedef enum { RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1, RCMARL_TAILOR_SPECTRAL = 2 } rcmarl_tailored_family;
+typedef enum {
+    RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1, RCMARL_TAILOR_SPECTRAL = 2,
+    RCMARL_TAILOR_SUBSET = 3    /* rule: rcmarl_subset_rule; only the subset forms (rcmarl_subset_pipeline_attack) */
+} rcmarl_tailored_family;
 typedef struct {
     float* dst;                 /* the crafted message (packed network) */
     const float* msgs;          /* base of the message stack */
@@ -747,6 +750,49 @@ int rcmarl_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs
  * H >= 1 with DnC.  Every shape of the 5-agent team (n_in <= 5, at most 761 parameters) is admitted. */
 int rcmarl_pipeline_arc_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, void* stream);
 int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, void* stream);
+
+/* Subset-aware Byzantine messages (rcmarl_subset_pipeline_attack, rcmarl_subset_history_attack): the pipeline and
+ * history attacks, with or without ARC, against a receiver j whose rule is exact subset selection (MDA or SMEA,
+ * rcmarl_subset_aggregate).  Threat model: that of the base attack, plus j's rule.  The jobs are
+ * rcmarl_pipeline_attack_job and rcmarl_history_attack_job with every field's meaning unchanged, except that the family
+ * is RCMARL_TAILOR_SUBSET and the rule an rcmarl_subset_rule:
+ *   rcmarl_subset_pipeline_attack   received -> [ARC] -> [nnm | bucket] -> MDA / SMEA (the pipeline form; arc = 1:
+ *                                   rcmarl_pipeline_arc_attack's clipping step);
+ *   rcmarl_subset_history_attack    received -> momentum -> [ARC] -> MDA / SMEA (the history form; arc = 1:
+ *                                   rcmarl_history_arc_attack's clipping step).
+ *   Rule.    For each candidate gamma_i (and each shuffle sample q under bucketing), rcmarl_subset_aggregate's arithmetic
+ *            bit for bit over the n_rows rows the base attack's rule reads, at H (the same device code): the flagged
+ *            set F, the fp64 distances (one warp per pair, the fixed xor butterfly), the s-subsets of U in
+ *            lexicographic rank order, MDA's diameter or SMEA's lambda_max(B_S) by warp_jacobi, S* = argmin c(S) with
+ *            ties to the lower rank, and the fp32 mean of S* summed from 0.  The flags and pairwise distances of rows
+ *            that do not depend on gamma_i (the real slots in the pipeline form without mixing or ARC and in the
+ *            history form without ARC) are taken once per job by the same warp code; every other distance is summed
+ *            per candidate.  No subset is skipped.
+ *   Everything else is the base attack's: mu, d, Gamma, the K + 1 candidates, O_i, the pick, dst, gamma_out and
+ *   model_out = R(gamma_i*) (R_0 under bucketing), with ARC (arc = 1) exactly where the ARC forms put it.
+ * At H = 0 with finite rows, the rule is the plain mean, bitwise rcmarl_dnc_aggregate's at H = 0, so dst, gamma_out and
+ * model_out are bitwise those of the base entry point with family SPECTRAL (DnC) at H = 0 (rcmarl_pipeline_attack,
+ * rcmarl_history_attack, or their ARC forms when arc = 1).  Exactness: under the base attack's conditions, model_out is
+ * bitwise what j computes from the messages actually sent -- [rcmarl_momentum_mix] -> [rcmarl_arc_clip] ->
+ * [rcmarl_nnm_mix] -> rcmarl_subset_aggregate; under bucketing, with the attacker's sample 0 in place of j's secret
+ * shuffle.  NaN inputs are not supported.  Each candidate runs a full subset search, up to C(16, 8) = 12 870 subsets:
+ * at n_in = 16 and H >= 5 under SMEA a job takes seconds.  One CTA per job, the staging of the base attack (no fp64
+ * mean) in shared memory; fixed summation orders, no atomics -- bitwise reproducible, independent of the job order and
+ * of how jobs are split over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, gamma_out and model_out untouched): everything the base entry point
+ * (arc = 1: its ARC form) refuses except the family -- a family other than RCMARL_TAILOR_SUBSET, a rule other than
+ * RCMARL_SUBSET_MDA and RCMARL_SUBSET_SMEA, H outside [0, n_rows) -- arc other than 0 or 1, with arc = 1 a crafted slot
+ * 0, and a staging size above RCMARL_SUBSET_ATTACK_MAX_FLOATS: (n_real + n_mixed + 4 + k_clip) * n in the pipeline form
+ * and (n_in + 4 + k_clip) * n in the history form (n_real, n_mixed as for rcmarl_pipeline_attack; k_clip =
+ * (2 * H * (n_in - H)) / n_in with arc = 1, else 0).  The bound admits every shape of the 5-agent team (n_in <= 5, at
+ * most 761 parameters) in all four forms and, at the 16-agent team-reward net (1421 parameters) with n_in = 16 and 15
+ * real slots: the pipeline form without mixing (19 rows) and under bucketing with s >= 2 (at most 27 rows), with ARC at
+ * every H (k_clip <= 8); under bucketing with s = 1 (34 rows) with ARC at H <= 1; under nnm (35 rows) without ARC
+ * (with ARC at H = 0 only); the history form (20 rows), with ARC at every H (at most 28 rows).  Static shared memory
+ * plus the bound stays under the 227 KB a CTA may opt in to (ptxas -v: at most 27 760 bytes static). */
+#define RCMARL_SUBSET_ATTACK_MAX_FLOATS (35 * 1421)
+int rcmarl_subset_pipeline_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, int arc, void* stream);
+int rcmarl_subset_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, int arc, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]

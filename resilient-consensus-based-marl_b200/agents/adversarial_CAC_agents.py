@@ -85,7 +85,10 @@ class Byzantine_CAC_agent(Faulty_CAC_agent):
     its momentum step, ("history_uv" | "history_std" | "history_sgn", s), at rcmarl_history_attack (against a receiver
     without momentum it is the pipeline attack in the same direction); or that history / pipeline search through the
     receiver's adaptive robust clipping as well, ("arc_uv" | "arc_std" | "arc_sgn", s), at rcmarl_history_arc_attack /
-    rcmarl_pipeline_arc_attack (against a receiver that does not clip it is the history attack); or the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
+    rcmarl_pipeline_arc_attack (against a receiver that does not clip it is the history attack); or that search through
+    an mda / smea receiver's exact subset selection as well, ("subset_uv" | "subset_std" | "subset_sgn", s), at
+    rcmarl_subset_history_attack / rcmarl_subset_pipeline_attack (against a receiver on any other rule it is the ARC
+    attack); or the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
     with eps >= 0, at rcmarl_dissensus_attack; or the mimic attack that copies the honest neighbour furthest along the
     honest messages' principal direction, ("mimic", T0) with T0 the number of power steps, an integer in 0 .. 2^31 - 1,
     after which the direction is frozen, at rcmarl_mimic_attack).

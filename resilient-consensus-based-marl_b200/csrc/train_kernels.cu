@@ -795,32 +795,103 @@ __device__ __forceinline__ unsigned subset_unrank(int r, int m, int sz, const in
     return mask;
 }
 
-__global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_constant__ VectorParams P) {
+// C(a, b) for a, b <= RCMARL_MAX_NEIGHBOURS into S.binom; called by the whole CTA, the caller synchronises.
+__device__ __forceinline__ void subset_binom(SubsetShared& S) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
-    constexpr int NW = VEC_THREADS / 32;
-    extern __shared__ __align__(16) float smem[];
-    __shared__ SubsetShared S;
-    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
-    const int n = job.n, nin = job.n_in, H = job.H;
-    const bool smea = job.rule == RCMARL_SUBSET_SMEA;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    float* xs = smem;                              // [n_in][n]
-    for (int k = 0; k < nin; ++k) {
-        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
-        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
-    }
-    for (int e = tid; e < (MAXN + 1) * (MAXN + 1); e += VEC_THREADS) {
+    for (int e = threadIdx.x; e < (MAXN + 1) * (MAXN + 1); e += VEC_THREADS) {
         const int a = e / (MAXN + 1), b = e % (MAXN + 1);
         int c = b > a ? 0 : 1;
         for (int i = 0; i < b && i < a; ++i) c = c * (a - i) / (i + 1);
         S.binom[a][b] = c;
     }
+}
+
+// Whether row xa holds +-inf, in every lane of the calling warp (the flag of rcmarl_subset_aggregate and dnc_rule).
+__device__ __forceinline__ bool warp_has_inf(const float* xa, int n, int lane) {
+    bool inf = false;
+    for (int p = lane; p < n; p += 32) inf |= isinf(xa[p]);
+    return __any_sync(0xffffffffu, inf);
+}
+
+// The fp64 squared distance of two rows in every lane of the calling warp: lane-strided fma partials, then the fixed
+// xor butterfly (rcmarl_subset_aggregate's D_kl).
+__device__ __forceinline__ double warp_sqdist_f64(const float* xa, const float* xb, int n, int lane) {
+    double s = 0.0;
+    for (int p = lane; p < n; p += 32) {
+        const double d = (double)xa[p] - (double)xb[p];
+        s = fma(d, d, s);
+    }
+    return warp_sum_f64(s);
+}
+
+// The argmin over (c, rank), a total order, of (bc, br) of the calling lane and S.best_c / S.best_r of every thread
+// past warp 0, into (bc, br) of every lane of warp 0.
+__device__ __forceinline__ void subset_argmin(const SubsetShared& S, double& bc, int& br, int lane) {
+    for (int q = lane + 32; q < VEC_THREADS; q += 32) {
+        const double c = S.best_c[q];
+        const int r = S.best_r[q];
+        if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        const double c = __shfl_xor_sync(0xffffffffu, bc, o);
+        const int r = __shfl_xor_sync(0xffffffffu, br, o);
+        if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
+    }
+}
+
+// The rows of `known` whose flags and pairwise distances subset_rule reads from a cache instead of its rows: flag[k]
+// for k in known, DK[k * MAXN + l] (row indices) for k != l both in known and unflagged.  Called by the whole CTA; the
+// caller synchronises.
+template <class Row>
+__device__ __forceinline__ void subset_known(const Row& row, int n, int nin, unsigned known, int* flag, double* DK) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int k = warp; k < nin; k += NW)
+        if ((known >> k) & 1u) {
+            const bool inf = warp_has_inf(row(k), n, lane);
+            if (lane == 0) flag[k] = inf ? 1 : 0;
+        }
     __syncthreads();
-    const StagedRows row{xs, n};
+    for (int t = warp; t < nin * nin; t += NW) {
+        const int k = t / nin, l = t % nin;
+        if (k < l && ((known >> k) & (known >> l) & 1u) && !flag[k] && !flag[l]) {
+            const double s = warp_sqdist_f64(row(k), row(l), n, lane);
+            if (lane == 0) { DK[k * MAXN + l] = s; DK[l * MAXN + k] = s; }
+        }
+    }
+}
+
+// The best (criterion, rank) over the candidates that hold only rows of `known`, for the U (as a row mask) it was
+// taken with; urows = 0 until it is taken.
+struct SubsetKnownBest {
+    double c;
+    int r;
+    unsigned urows;
+};
+
+// The body of rcmarl_subset_aggregate over nin rows row(0) .. row(nin - 1) of n floats in shared memory (S.binom
+// filled): writes the aggregate to out[0:n] and leaves w_k in S.wt (the caller synchronises before reading either).
+// The rows of `known` take their flags from kflag and the distances of their pairs from DK (subset_known, the same
+// warp code), so only the pairs with a row outside `known` are summed here.  With kb, the candidates that hold only
+// rows of `known` are searched once: the first call takes their best (c, rank) into kb besides the full search, and a
+// later call with the same U skips them and merges kb's -- the same criteria from the same numbers, and (c, rank) is a
+// total order, so the selection is the full search's.  Called by the whole CTA of VEC_THREADS threads; Row maps a row
+// index to its staged row.
+template <class Row>
+__device__ __forceinline__ void subset_rule(const Row& row, int n, int nin, int H, int rule, float* out, SubsetShared& S,
+                                            unsigned known = 0u, const int* kflag = nullptr,
+                                            const double* DK = nullptr, SubsetKnownBest* kb = nullptr) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    const bool smea = rule == RCMARL_SUBSET_SMEA;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (int k = warp; k < nin; k += NW) {
-        bool inf = false;
-        for (int p = lane; p < n; p += 32) inf |= isinf(row.at(k, p));
-        inf = __any_sync(0xffffffffu, inf);
+        if ((known >> k) & 1u) {
+            if (lane == 0) S.flagged[k] = kflag[k];
+            continue;
+        }
+        const bool inf = warp_has_inf(row(k), n, lane);
         if (lane == 0) S.flagged[k] = inf ? 1 : 0;
     }
     __syncthreads();
@@ -837,28 +908,33 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
             int a = 0, r = t;
             while (r >= m - 1 - a) { r -= m - 1 - a; ++a; }
             const int b = a + 1 + r;
-            const float* xa = row(S.ulist[a]);
-            const float* xb = row(S.ulist[b]);
-            double s = 0.0;
-            for (int p = lane; p < n; p += 32) {
-                const double d = (double)xa[p] - (double)xb[p];
-                s = fma(d, d, s);
-            }
-            s = warp_sum_f64(s);
+            const int ia = S.ulist[a], ib = S.ulist[b];
+            const double s = ((known >> ia) & (known >> ib) & 1u) ? DK[ia * MAXN + ib]
+                                                                   : warp_sqdist_f64(row(ia), row(ib), n, lane);
             if (lane == 0) { S.D[a * MAXN + b] = s; S.D[b * MAXN + a] = s; }
         }
         if (tid < m) S.D[tid * MAXN + tid] = 0.0;
         __syncthreads();
         const int sz = nin - max(nin - m, H);                        // >= 1
         const int total = S.binom[m][sz];
-        double bc = INFINITY;
-        int br = 0x7fffffff;
+        double bc = INFINITY, kc = INFINITY;
+        int br = 0x7fffffff, kr = 0x7fffffff;
+        unsigned urows = 0u, kpos = 0u;                               // kb: U as a row mask, the known U positions
+        if (kb)
+            for (int a = 0; a < m; ++a) {
+                urows |= 1u << S.ulist[a];
+                kpos |= ((known >> S.ulist[a]) & 1u) << a;
+            }
+        const bool use = kb && sz > 1 && kb->urows == urows;          // skip the known-only candidates, merge kb's
+        const bool take = kb && sz > 1 && kb->urows == 0u;            // and take kb in this call
         if (sz == 1) {                                                // every criterion is 0: rank 0
             bc = 0.0;
             br = 0;
         } else if (!smea) {
             for (int r = tid; r < total; r += VEC_THREADS) {
                 const unsigned mask = subset_unrank(r, m, sz, S.binom);
+                const bool konly = (mask & ~kpos) == 0u;
+                if (use && konly) continue;
                 double c = 0.0;
                 for (unsigned ma = mask; ma; ma &= ma - 1) {
                     const int a = __ffs(ma) - 1;
@@ -868,11 +944,14 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
                     }
                 }
                 if (c < bc) { bc = c; br = r; }
+                if (take && konly && c < kc) { kc = c; kr = r; }
             }
         } else {
             double* B = S.B[warp];
             for (int r = warp; r < total; r += NW) {
                 const unsigned mask = subset_unrank(r, m, sz, S.binom);
+                const bool konly = (mask & ~kpos) == 0u;              // the same in every lane
+                if (use && konly) continue;
                 int pa = 0;                                           // lane a < sz: the a-th position of the subset
                 unsigned mm = mask;
                 for (int i = 0; i < lane && mm; ++i) mm &= mm - 1;
@@ -901,26 +980,29 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
                 for (int a = 1; a < sz; ++a) c = fmax(c, B[a * MAXN + a]);
                 __syncwarp();                                         // every lane has read the diagonal
                 if (c < bc) { bc = c; br = r; }
+                if (take && konly && c < kc) { kc = c; kr = r; }
             }
         }
         S.best_c[tid] = bc;
         S.best_r[tid] = br;
         __syncthreads();
-        if (warp == 0) {                                              // argmin over (c, rank): a total order
-            for (int q = lane + 32; q < VEC_THREADS; q += 32) {
-                const double c = S.best_c[q];
-                const int r = S.best_r[q];
-                if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
-            }
-            for (int o = 16; o > 0; o >>= 1) {
-                const double c = __shfl_xor_sync(0xffffffffu, bc, o);
-                const int r = __shfl_xor_sync(0xffffffffu, br, o);
-                if (c < bc || (c == bc && r < br)) { bc = c; br = r; }
-            }
+        if (warp == 0) {
+            subset_argmin(S, bc, br, lane);
+            if (use && (kb->c < bc || (kb->c == bc && kb->r < br))) { bc = kb->c; br = kb->r; }
             const unsigned mask = subset_unrank(br, m, sz, S.binom);
             if (lane < nin) S.wt[lane] = 0.f;
             __syncwarp();
             if (lane < m && ((mask >> lane) & 1u)) S.wt[S.ulist[lane]] = 1.f / (float)sz;
+        }
+        if (take) {                                                   // the same in every thread
+            __syncthreads();                                          // warp 0 has read every best
+            S.best_c[tid] = kc;
+            S.best_r[tid] = kr;
+            __syncthreads();
+            if (warp == 0) {
+                subset_argmin(S, kc, kr, lane);
+                if (lane == 0) { kb->c = kc; kb->r = kr; kb->urows = urows; }
+            }
         }
     } else if (tid < nin) {
         S.wt[tid] = tid == 0 ? 1.f : 0.f;                            // every row flagged: out = x_0
@@ -930,8 +1012,24 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
         float s = 0.f, cnt = 0.f;
         for (int k = 0; k < nin; ++k)
             if (S.wt[k] != 0.f) { s += row.at(k, p); cnt += 1.f; }
-        job.dst[p] = s / cnt;
+        out[p] = s / cnt;
     }
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_constant__ VectorParams P) {
+    extern __shared__ __align__(16) float smem[];
+    __shared__ SubsetShared S;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x;
+    float* xs = smem;                              // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    subset_binom(S);
+    __syncthreads();
+    subset_rule(StagedRows{xs, n}, n, nin, job.H, job.rule, job.dst, S);
     if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
 }
 
@@ -1499,7 +1597,17 @@ __device__ __forceinline__ void arc_rows(float* xs, const int* off, int n, int n
     __syncthreads();
 }
 
-template <bool ARC>
+// The receiver's MDA / SMEA rule inside the subset forms of the pipeline and history searches
+// (rcmarl_subset_pipeline_attack, rcmarl_subset_history_attack): subset_rule's scratch, and the flags and pairwise
+// distances of the rows that do not depend on the candidate (subset_known), taken once per job.
+struct SubsetAttackShared {
+    SubsetShared S;
+    double DK[RCMARL_MAX_NEIGHBOURS * RCMARL_MAX_NEIGHBOURS];
+    int flag[RCMARL_MAX_NEIGHBOURS];
+    SubsetKnownBest KB;
+};
+
+template <bool ARC, bool SUBSET>
 __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const __grid_constant__ PipelineParams P) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
     extern __shared__ __align__(16) float smem[];
@@ -1555,6 +1663,19 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
         if (pj.mixing == RCMARL_PIPE_NONE) ooff = A.off;
     }
     const SlotRows slots{xs, soff}, rows{xs, ooff};
+    SubsetAttackShared* U = nullptr;              // SUBSET: the rule's scratch
+    unsigned known = 0u;                          // SUBSET: the rule's rows that do not depend on the candidate
+    if constexpr (SUBSET) {
+        __shared__ SubsetAttackShared SU;
+        U = &SU;
+        subset_binom(SU.S);
+        if (!ARC && pj.mixing == RCMARL_PIPE_NONE) {   // the real slots: their flags and distances once per job
+            for (int k = 0; k < nin; ++k) known |= job.slots[k] >= 0 ? 1u << k : 0u;
+            subset_known(rows, n, nin, known, SU.flag, SU.DK);
+        }
+        if (tid == 0) SU.KB.urows = 0u;
+        __syncthreads();
+    }
     const auto eval = [&](int q) {
         if constexpr (ARC)                        // once per candidate: every crafted slot holds it, one d_k for all
             if (q == 0)
@@ -1567,7 +1688,9 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
             bucket_means(slots, n, nin, nb, members + q * MAXN, [&](int b) { return mixed + b * n; });
             __syncthreads();
         }
-        if (job.family == RCMARL_TAILOR_COORD)
+        if constexpr (SUBSET)
+            subset_rule(rows, n, nrows, job.H, job.rule, z, U->S, known, U->flag, U->DK, known ? &U->KB : nullptr);
+        else if (job.family == RCMARL_TAILOR_COORD)
             coord_rule(rows, n, nrows, job.H, job.rule, z);
         else if (job.family == RCMARL_TAILOR_VECTOR)
             vector_rule(rows, n, nrows, job.H, job.rule, z, z, S.dist, S.wt, S.score, S.total);
@@ -1648,7 +1771,7 @@ __device__ __forceinline__ float momentum_invert(float t, float c, const float* 
     return __fadd_rn(c, __fdiv_rn(__fsub_rn(__fsub_rn(t, c), __fmul_rn(beta, old)), __fsub_rn(1.f, beta)));
 }
 
-template <bool ARC>
+template <bool ARC, bool SUBSET>
 __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __grid_constant__ HistoryParams P) {
     extern __shared__ __align__(16) float smem[];
     __shared__ TailoredShared S;
@@ -1695,6 +1818,19 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
     }
     const float range = tailored_range(job, nh, xs, mu, d, S);
     const SlotRows rows{xs, ARC ? A.off : S.off};
+    SubsetAttackShared* U = nullptr;               // SUBSET: the rule's scratch
+    unsigned known = 0u;                           // SUBSET: the rule's rows that do not depend on the candidate
+    if constexpr (SUBSET) {
+        __shared__ SubsetAttackShared SU;
+        U = &SU;
+        subset_binom(SU.S);
+        if (!ARC) {                                // the real slots' rows r_k: their flags and distances once per job
+            for (int k = 0; k < nin; ++k) known |= job.slots[k] >= 0 ? 1u << k : 0u;
+            subset_known(rows, n, nin, known, SU.flag, SU.DK);
+        }
+        if (tid == 0) SU.KB.urows = 0u;
+        __syncthreads();
+    }
     // a_k of every crafted slot for the target in cand, then the rule into z; returns whether every crafted message is
     // finite (the same in every thread).  An infeasible candidate skips the rule unless `always`: its objective is -inf
     // whatever the rule gives.
@@ -1717,7 +1853,9 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
         if (!ok && !always) return false;
         if constexpr (ARC)                         // one d_k per crafted slot: colluders' rows differ
             arc_rows(xs, S.off, n, nin, job.H, ~real & ((1u << nin) - 1u), 0u, 0, clip, A);
-        if (job.family == RCMARL_TAILOR_COORD)
+        if constexpr (SUBSET)
+            subset_rule(rows, n, nin, job.H, job.rule, z, U->S, known, U->flag, U->DK, known ? &U->KB : nullptr);
+        else if (job.family == RCMARL_TAILOR_COORD)
             coord_rule(rows, n, nin, job.H, job.rule, z);
         else if (job.family == RCMARL_TAILOR_VECTOR)
             vector_rule(rows, n, nin, job.H, job.rule, z, z, S.dist, S.wt, S.score, S.total);
@@ -2704,8 +2842,15 @@ static bool arc_staging(const rcmarl_tailored_attack_job& q, bool arc, int64_t& 
     return q.slots[0] < 0;
 }
 
-template <bool ARC>
+// the receiver's rule in a subset form of the pipeline or history search: family SUBSET, MDA or SMEA, 0 <= H < n_rows
+static bool bad_subset_receiver(int family, int rule, int H, int n_rows) {
+    return family != RCMARL_TAILOR_SUBSET || (rule != RCMARL_SUBSET_MDA && rule != RCMARL_SUBSET_SMEA) || H < 0 ||
+           H >= n_rows;
+}
+
+template <bool ARC, bool SUBSET>
 static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
+    constexpr int bound = SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_PIPELINE_MAX_FLOATS;
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     PipelineParams P;
     RangeSet S;
@@ -2726,9 +2871,10 @@ static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         } else if (pj.mixing != RCMARL_PIPE_NONE) {
             return RCMARL_ERR_ARG;
         }
-        if (bad_receiver_rule(q.family, q.rule, q.H, n_rows)) return RCMARL_ERR_ARG;
+        if (SUBSET ? bad_subset_receiver(q.family, q.rule, q.H, n_rows) : bad_receiver_rule(q.family, q.rule, q.H, n_rows))
+            return RCMARL_ERR_ARG;
         int64_t floats = (int64_t)(n_real + n_mixed + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
-        if (arc_staging(q, ARC, floats) || floats > RCMARL_PIPELINE_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (arc_staging(q, ARC, floats) || floats > bound) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = pj;
         // writes dst, gamma_out and model_out, reads the real slots' rows
@@ -2738,12 +2884,12 @@ static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<pipeline_attack_kernel<ARC>>(P, n_jobs, RCMARL_PIPELINE_MAX_FLOATS, max_floats, ADA_THREADS,
-                                                      stream);
+    return launch_staged<pipeline_attack_kernel<ARC, SUBSET>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
 }
 
-template <bool ARC>
+template <bool ARC, bool SUBSET>
 static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
+    constexpr int bound = SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_HISTORY_MAX_FLOATS;
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     HistoryParams P;
     RangeSet S;
@@ -2752,7 +2898,9 @@ static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         const rcmarl_history_attack_job& hj = jobs[j];
         const rcmarl_tailored_attack_job& q = hj.attack;
         int n_real = 0;
-        if (bad_tailored_slots(q, n_real) || bad_receiver_rule(q.family, q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
+        if (bad_tailored_slots(q, n_real)) return RCMARL_ERR_ARG;
+        if (SUBSET ? bad_subset_receiver(q.family, q.rule, q.H, q.n_in) : bad_receiver_rule(q.family, q.rule, q.H, q.n_in))
+            return RCMARL_ERR_ARG;
         if (!hj.ref || !hj.momentum) return RCMARL_ERR_ARG;
         if (!std::isfinite(hj.beta) || hj.beta < 0.f || hj.beta >= 1.f || (hj.first != 0 && hj.first != 1))
             return RCMARL_ERR_ARG;
@@ -2760,7 +2908,7 @@ static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         for (int k = 0; k < q.n_in; ++k)
             if (((hj.own_mask >> k) & 1u) && q.slots[k] >= 0) return RCMARL_ERR_ARG;   // an own bit on a real slot
         int64_t floats = (int64_t)(q.n_in + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
-        if (arc_staging(q, ARC, floats) || floats > RCMARL_HISTORY_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (arc_staging(q, ARC, floats) || floats > bound) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = hj;
         // writes dst, gamma_out and model_out, reads the real slots' rows, the ref and the n_in M rows
@@ -2772,26 +2920,35 @@ static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         S.r.rows(hj.momentum, q.n_in, hj.momentum_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<history_attack_kernel<ARC>>(P, n_jobs, RCMARL_HISTORY_MAX_FLOATS, max_floats, ADA_THREADS,
-                                                     stream);
+    return launch_staged<history_attack_kernel<ARC, SUBSET>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
 }
 
 extern "C" {
 
 int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
-    return pipeline_attack<false>(jobs, n_jobs, stream);
+    return pipeline_attack<false, false>(jobs, n_jobs, stream);
 }
 
 int rcmarl_pipeline_arc_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
-    return pipeline_attack<true>(jobs, n_jobs, stream);
+    return pipeline_attack<true, false>(jobs, n_jobs, stream);
 }
 
 int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
-    return history_attack<false>(jobs, n_jobs, stream);
+    return history_attack<false, false>(jobs, n_jobs, stream);
 }
 
 int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
-    return history_attack<true>(jobs, n_jobs, stream);
+    return history_attack<true, false>(jobs, n_jobs, stream);
+}
+
+int rcmarl_subset_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, int arc, void* stream) {
+    if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
+    return arc ? pipeline_attack<true, true>(jobs, n_jobs, stream) : pipeline_attack<false, true>(jobs, n_jobs, stream);
+}
+
+int rcmarl_subset_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, int arc, void* stream) {
+    if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
+    return arc ? history_attack<true, true>(jobs, n_jobs, stream) : history_attack<false, true>(jobs, n_jobs, stream);
 }
 
 int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* stream) {

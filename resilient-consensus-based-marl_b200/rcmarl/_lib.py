@@ -38,7 +38,7 @@ DEV_UV, DEV_STD, DEV_SGN = 0, 1, 2                # rcmarl_adaptive_dev
 ADAPTIVE_ATTACKS = {f"{k}_{d}": (kind, dev) for k, kind in (("minmax", ADAPT_MINMAX), ("minsum", ADAPT_MINSUM))
                     for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
 ADAPTIVE_MAX_FLOATS = 18 * 1536
-TAILOR_COORD, TAILOR_VECTOR, TAILOR_SPECTRAL = 0, 1, 2   # rcmarl_tailored_family
+TAILOR_COORD, TAILOR_VECTOR, TAILOR_SPECTRAL, TAILOR_SUBSET = 0, 1, 2, 3   # rcmarl_tailored_family
 # rule-aware attacks (rcmarl_tailored_attack): candidate steps K and the staging bound; the names are TAILORED_ATTACKS
 TAILORED_STEPS = 32
 TAILORED_MAX_FLOATS = 19 * 1536
@@ -65,6 +65,9 @@ PIPELINE_MAX_PERMS = 16
 PIPELINE_PERMS = 4
 # momentum-aware attacks (rcmarl_history_attack): the staging bound; the names are HISTORY_ATTACKS
 HISTORY_MAX_FLOATS = 22 * 1421
+# subset-aware attacks (rcmarl_subset_pipeline_attack / rcmarl_subset_history_attack): the staging bound; the names
+# are SUBSET_ATTACKS
+SUBSET_ATTACK_MAX_FLOATS = 35 * 1421
 MIMIC_MAX_FLOATS = 19 * 1536                      # rcmarl_mimic_attack's staging bound
 MIMIC_MAX_T0 = 2 ** 31 - 1                        # the mimic attack's power steps T0: an integer in 0 .. 2^31 - 1
 
@@ -206,6 +209,8 @@ SYMBOLS = [
     ("rcmarl_history_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, c_fp]),
     ("rcmarl_pipeline_arc_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, c_fp]),
     ("rcmarl_history_arc_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, c_fp]),
+    ("rcmarl_subset_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, C.c_int, c_fp]),
+    ("rcmarl_subset_history_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, C.c_int, c_fp]),
     ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
     ("rcmarl_mimic_attack", C.c_int, [C.POINTER(MimicJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -467,6 +472,23 @@ def is_arc_attack(name):
     return isinstance(name, str) and name in ARC_ATTACKS
 
 
+class SubsetAttackKind(int):
+    """The kind check_attack gives a subset-aware attack (rcmarl_subset_pipeline_attack / rcmarl_subset_history_attack):
+    its rcmarl_adaptive_dev, as a type of its own so that it is told apart from the attacks that do not model the
+    receiver's MDA / SMEA selection."""
+
+    def __repr__(self):
+        return f"SubsetAttackKind({int(self)})"
+
+
+SUBSET_ATTACKS = {f"subset_{d}": SubsetAttackKind(dev) for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+
+
+def is_subset_attack(name):
+    """True for the name of a subset-aware attack: "subset_uv", "subset_std", "subset_sgn"."""
+    return isinstance(name, str) and name in SUBSET_ATTACKS
+
+
 class DissensusKind(int):
     """The kind check_attack gives the dissensus attack (rcmarl_dissensus_attack), a type of its own so that it is told
     apart from the other attacks' kinds; its parameter is eps >= 0."""
@@ -488,15 +510,16 @@ STATE_ATTACKS = {"dissensus": DissensusKind(0), "mimic": MimicKind(0)}
 
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss", the adaptive, the tailored, the pipeline, the history and the ARC attacks and "dissensus" also >= 0; for
-    "mimic" an integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack / rcmarl_tailored_attack /
-    rcmarl_pipeline_attack / rcmarl_history_attack / rcmarl_pipeline_arc_attack / rcmarl_history_arc_attack /
+    "gauss", the adaptive, the tailored, the pipeline, the history, the ARC and the subset attacks and "dissensus" also
+    >= 0; for "mimic" an integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack /
+    rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / rcmarl_pipeline_arc_attack /
+    rcmarl_history_arc_attack / rcmarl_subset_pipeline_attack / rcmarl_subset_history_attack /
     rcmarl_dissensus_attack / rcmarl_mimic_attack require
     (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
     the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the
     paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, the PipelineKind of a pipeline
-    attack, the HistoryKind of a history attack and the ArcAttackKind of an ARC attack, whose parameter is the range
-    multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
+    attack, the HistoryKind of a history attack, the ArcAttackKind of an ARC attack and the SubsetAttackKind of a
+    subset attack, whose parameter is the range multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
     and MimicKind for "mimic", whose parameter is T0 (the power steps each pair takes before its direction freezes)."""
     try:
         name, param = attack
@@ -504,17 +527,17 @@ def check_attack(attack):
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
     known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **PIPELINE_ATTACKS, **HISTORY_ATTACKS, **ARC_ATTACKS,
-             **STATE_ATTACKS}
+             **SUBSET_ATTACKS, **STATE_ATTACKS}
     if not isinstance(name, str) or name not in known:
         names = sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(PIPELINE_ATTACKS) \
-            + sorted(HISTORY_ATTACKS) + sorted(ARC_ATTACKS) + sorted(STATE_ATTACKS)
+            + sorted(HISTORY_ATTACKS) + sorted(ARC_ATTACKS) + sorted(SUBSET_ATTACKS) + sorted(STATE_ATTACKS)
         raise RcmarlError(f"unknown attack {name!r}: expected one of {names}")
     if name == "mimic":
         if not (math.isfinite(param) and param == int(param) and 0 <= param <= MIMIC_MAX_T0):
             raise RcmarlError(f"attack 'mimic' needs an integer T0 in 0 .. {MIMIC_MAX_T0}, got {param}")
         return known[name], param
     nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS \
-        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS or name in ARC_ATTACKS
+        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS or name in ARC_ATTACKS or name in SUBSET_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
     return known[name], param

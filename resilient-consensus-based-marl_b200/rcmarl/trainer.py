@@ -11,6 +11,7 @@ Data-parallel (SURVEY 8e): each rank owns n_envs environments and their buffer
 rows for ever; parameters are replicated; the only exchange is one all-reduce
 of the packed UNSCALED gradient sums per SGD / Adam / projection step.
 """
+import functools
 import os
 
 import numpy as np
@@ -158,14 +159,17 @@ class Trainer:
                         else 'history' if e in self.hist_pairs else 'ARC')
                 raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose rule "
                                     f"{agg[j]!r} the attack does not model")
-        for e in self.arc_pairs:                   # an ARC job stages k_clip clipped rows on top of its base job's
+        for e in self.arc_pairs + self.subset_pairs:   # an ARC job stages k_clip clipped rows on top of its base job's
             b, j, _ = self.byz_pairs[e]
             n_real = sum(k >= 0 for k in self._tailored_slots(j)[0])
             kc = L.arc_count(self.H[j], len(self.in_nodes[j])) if self.clipping[j] is not None else 0
             floats, bound = self._arc_staging(j, n_real, kc)
+            if self.subset_rule[j] is not None:    # a subset job stages as its ARC form, under a bound of its own
+                bound = L.SUBSET_ATTACK_MAX_FLOATS
             if floats > bound:
-                raise L.RcmarlError(f"Byzantine agent {b} runs an ARC attack against agent {j}, whose job stages "
-                                    f"{floats} floats, more than the {bound} the library admits")
+                raise L.RcmarlError(f"Byzantine agent {b} runs {'an ARC' if e in self.arc_pairs else 'a subset'} "
+                                    f"attack against agent {j}, whose job stages {floats} floats, more than the "
+                                    f"{bound} the library admits")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
         # that of each cooperative agent on dnc, then that of each on mda / smea
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
@@ -245,8 +249,8 @@ class Trainer:
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
         # clipping factors c of each agent that clips: row 2q critic, 2q + 1 TR of arc_agents[q]
         self.arc_weights = torch.zeros(2 * len(self.arc_agents), L.MAX_NEIGHBOURS, **f32) if self.arc_agents else None
-        # gamma of each adaptive, tailored, pipeline, history or ARC attack of the last epoch: row q = gamma_pairs[q],
-        # columns critic, TR
+        # gamma of each adaptive, tailored, pipeline, history, ARC or subset attack of the last epoch: row q =
+        # gamma_pairs[q], columns critic, TR
         self.att_gamma = torch.zeros(len(self.gamma_pairs), 2, **f32) if self.gamma_pairs else None
         # the mimic attack's direction state z of each mimic pair (row q = mimic_pairs[q]; [q, 0, :PC] critic, [q, 1] TR),
         # the index into S_j each copied in the last epoch, and the power steps each has taken (host)
@@ -356,7 +360,14 @@ class Trainer:
         # rcmarl_pipeline_arc_attack); launches of their own, after the history ones (_arc_job_groups)
         self.arc_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                           if isinstance(self.attack[b][0], L.ArcAttackKind)]
-        self.gamma_pairs = self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs
+        # the pairs whose attacker runs a subset-aware attack (kind L.SubsetAttackKind): against an mda / smea receiver
+        # the history or pipeline search through its whole chain and its subset selection
+        # (rcmarl_subset_history_attack / rcmarl_subset_pipeline_attack), against any other exactly an ARC pair's job;
+        # launches of their own, after the ARC ones (_subset_job_groups)
+        self.subset_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                             if isinstance(self.attack[b][0], L.SubsetAttackKind)]
+        self.gamma_pairs = (self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs
+                            + self.subset_pairs)
         # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
         # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
         # tailored one
@@ -448,11 +459,11 @@ class Trainer:
         return out
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline, a history or an ARC
-        attack: float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
-        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline, history or ARC attack gamma_i*,
-        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / their ARC forms); entry 0 for the
-        critic, 1 for the team-reward net."""
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline, a history, an ARC or a
+        subset attack: float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
+        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline, history, ARC or subset attack gamma_i*,
+        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / their ARC and subset forms); entry 0
+        for the critic, 1 for the team-reward net."""
         if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
@@ -499,19 +510,35 @@ class Trainer:
         `epoch` is set per epoch).  Per pair one critic and one TR job: against a receiver that clips, the history form
         (momentum) or the pipeline form (with the receiver's mixing) through its clipping step; against one that does
         not, exactly the job a history pair gets."""
+        n_before = len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs) + len(self.hist_pairs)
+        return self._chain_job_groups(self.arc_pairs, n_before)
+
+    def _subset_job_groups(self):
+        """_arc_job_groups for the subset pairs, launched after the ARC groups: against an mda / smea receiver the
+        history form (momentum) or the pipeline form (with the receiver's mixing) of rcmarl_subset_history_attack /
+        rcmarl_subset_pipeline_attack, with arc = whether the receiver clips (the launch is functools.partial of
+        ops.subset_history_attack / ops.subset_pipeline_attack with that arc); against any other receiver exactly the
+        job, and the launch, an ARC pair gets."""
+        n_before = (len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs) + len(self.hist_pairs)
+                    + len(self.arc_pairs))
+        return self._chain_job_groups(self.subset_pairs, n_before)
+
+    def _chain_job_groups(self, pairs, n_before):
+        """The groups of _arc_job_groups / _subset_job_groups for `pairs`, whose gamma rows start at n_before."""
         NA = self.NA
         mom_index = {i: q for q, i in enumerate(self.mom_agents)}
-        n_before = len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs) + len(self.hist_pairs)
-        tables = {}                                    # (history form, clips) -> ([jobs], [mom])
-        for q_pair, e in enumerate(self.arc_pairs):
+        tables = {}                                    # (subset rule, history form, clips) -> ([jobs], [mom])
+        for q_pair, e in enumerate(pairs):
             b, j, _ = self.byz_pairs[e]
             kind, param = self.attack[b]
             slots, hon = self._tailored_slots(j)
-            rule = ((L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
+            subset = self.subset_rule[j] is not None
+            rule = ((L.TAILOR_SUBSET, self.subset_rule[j]) if subset
+                    else (L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
                     else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
                     else (L.TAILOR_COORD, self.aggregation[j]))
             hist = self.momentum[j] is not None
-            jobs, moms = tables.setdefault((hist, self.clipping[j] is not None), ([], []))
+            jobs, moms = tables.setdefault((subset, hist, self.clipping[j] is not None), ([], []))
             for t, (msgs, P, ref) in enumerate(((self.msg_c, self.PC, self.critic[j]), (self.msg_t, self.PT, self.tr[j]))):
                 gamma_out = self.att_gamma[n_before + q_pair, t:t + 1]
                 if hist:
@@ -530,10 +557,11 @@ class Trainer:
                   (False, True): ops.pipeline_arc_attack, (False, False): ops.pipeline_attack}
         cls = {True: L.HistoryAttackJob, False: L.PipelineAttackJob}
         out = []
-        for (hist, clips), (jobs, moms) in sorted(tables.items(), reverse=True):
+        for (subset, hist, clips), (jobs, moms) in sorted(tables.items(), reverse=True):
+            fn = (functools.partial(ops.subset_history_attack if hist else ops.subset_pipeline_attack, arc=clips)
+                  if subset else launch[(hist, clips)])
             for g in range(0, len(jobs), L.MAX_JOBS):
-                out.append((launch[(hist, clips)], ops.job_array(cls[hist], jobs[g:g + L.MAX_JOBS]),
-                            moms[g:g + L.MAX_JOBS] if hist else None))
+                out.append((fn, ops.job_array(cls[hist], jobs[g:g + L.MAX_JOBS]), moms[g:g + L.MAX_JOBS] if hist else None))
         return out
 
     def _attack_job_groups(self):
@@ -561,7 +589,7 @@ class Trainer:
         mom_index = {i: q for q, i in enumerate(self.mom_agents)}
         diss_set = set(self.diss_pairs)
         mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
-        arc_set = set(self.arc_pairs)                  # their jobs are _arc_job_groups'
+        arc_set = set(self.arc_pairs + self.subset_pairs)   # their jobs are _arc_job_groups' / _subset_job_groups'
         for e, (b, j, honest) in enumerate(self.byz_pairs):
             if e in arc_set:
                 continue
@@ -838,7 +866,7 @@ class Trainer:
         # the Byzantine messages' job tables (_attack_job_groups)
         (att_groups, ada_groups, tail_groups, pipe_groups, hist_groups, hist_mom, diss_groups, mimic_t0,
          mimic_groups) = self._attack_job_groups()
-        arc_groups = self._arc_job_groups()
+        arc_groups = self._arc_job_groups() + self._subset_job_groups()
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
         # 16 cooperative agents x 2 nets, so one nnm launch and one bucketing launch per epoch.  A bucketing job draws
