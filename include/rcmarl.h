@@ -468,6 +468,40 @@ int rcmarl_dnc_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* s
 typedef enum { RCMARL_SUBSET_MDA = 0, RCMARL_SUBSET_SMEA = 1 } rcmarl_subset_rule;
 int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
 
+/* Iterative outlier scissor (rcmarl_ios_aggregate): the IOS rule of Wu, Chen & Ling, "Byzantine-Resilient
+ * Decentralized Stochastic Optimization With Robust Aggregation Rules" (IEEE Trans. Signal Processing, 2023), with
+ * uniform weights (so FABA, Xia et al., IJCAI 2019, over one neighbourhood).  The receiver drops the message furthest
+ * from the mean of those it still holds, re-centres, and repeats H times; the output is the mean of the rest.  It takes
+ * rcmarl_vector_job with rule = RCMARL_FILTER_IOS; its n = n_in slots x_0 .. x_{n-1}, x_k = msgs + in_nodes[k] *
+ * msg_stride (x_0 the receiver's own; repeats in in_nodes count) each hold P = job.n floats.
+ *   Flagged  F = the rows holding +-inf (DnC's convention); U = every other row, in index order.  If U is empty:
+ *            out = x_0, w = e_0.  A row of 1e30 is finite and not flagged: fp64 holds the square of any finite fp32
+ *            value, so it is removed by its distance.
+ *   Iterate  max(0, H - |F|) times: the centre c_p = (sum_{k in U, index order} (double)x_k,p) / (double)|U| in fp64,
+ *            from scratch; d_k = sum_p ((double)x_k,p - c_p)^2 for k in U (each d_k summed by one warp: lane-strided
+ *            fma partials, then the fixed xor butterfly); remove k* = argmax_{k in U} d_k (equal d: the higher index
+ *            first) from U.
+ *   Output   I = the rows left in U; out = (sum_{k in I, index order} x_k) / (float)|I|, an fp32 sum from 0
+ *            (multi-Krum's, DnC's and MDA's arithmetic); w_k = 1/(float)|I| on I, 0 elsewhere, written to weights_out
+ *            when it is not NULL.
+ * The receiver's own message is a candidate for removal, as under DnC and MDA: this is the library's definition.  It
+ * differs from the paper's Algorithm 1, where the receiver removes only received messages and always keeps its own.  Two rows
+ * left lie equally far from their mean: where their fp64 sums are exact (coordinate exponents less than 29 apart), the
+ * two d are equal and the higher index is removed.  H = 0
+ * with no flagged row gives the plain mean, bitwise rcmarl_dnc_aggregate's and rcmarl_subset_aggregate's at H = 0 and,
+ * where n_in >= 3, multi-Krum's at H = 0.  Rows of +-inf are never kept while fewer than n_in rows hold them, and rows
+ * of 1e30, at most H - |F| of them, get weight 0 while the other rows lie far closer together.  NaN inputs are not
+ * supported.  One CTA per job, fixed summation orders, no atomics: bitwise reproducible, independent of the job order
+ * and of how jobs are split over launches.  dst[0:n] = out.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst and weights_out untouched): n_jobs outside 1..RCMARL_MAX_JOBS, a null
+ * dst or msgs, n < 1, n_in outside 1..RCMARL_MAX_NEIGHBOURS, a negative in-node, a rule other than RCMARL_FILTER_IOS,
+ * H outside [0, n_in), (n_in + 2) * n > RCMARL_IOS_MAX_FLOATS (the staging bound: the fp32 messages and the fp64 centre
+ * are staged in shared memory), a dst or weights_out that overlaps an in-node row of any job of the launch, and two
+ * written ranges (dsts, weights_outs) of the launch that overlap. */
+#define RCMARL_IOS_MAX_FLOATS (48 * 1024)
+typedef enum { RCMARL_FILTER_IOS = 0 } rcmarl_filter_rule;
+int rcmarl_ios_aggregate(const rcmarl_vector_job* jobs_host, int n_jobs, void* stream);
+
 /* Nearest-neighbour mixing (rcmarl_nnm_mix): the pre-aggregation step of Allouah, Farhadkhani, Guerraoui, Gupta, Pinot
  * & Stephan, "Fixing by Mixing: A Recipe for Optimal Byzantine ML under Heterogeneity" (AISTATS 2023).  It replaces each
  * message a receiver hears by the mean of its n - H nearest received messages (itself among them); the receiver's own

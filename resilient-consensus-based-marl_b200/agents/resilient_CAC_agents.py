@@ -6,7 +6,8 @@ Same constructor and method names, argument meaning and mutation conventions as 
   resilient_consensus_*_hidden   overwrite the hidden layers with the clipped mean of the neighbours' (:142-166), or
                                  their trimmed / W-MSR mean with aggregation="trim" / "wmsr", or the hidden layers
                                  of a distance-based ("krum", "mkrum", "scclip", "gmed"), divide-and-conquer
-                                 ("dnc") or exact subset-selection ("mda", "smea") aggregate of whole messages
+                                 ("dnc"), exact subset-selection ("mda", "smea") or iterative outlier scissor ("ios")
+                                 aggregate of whole messages
   resilient_consensus_critic/_TR return the aggregated estimates (B,1), output layer unchanged (:168-206)
                                  With mixing="nnm", every consensus step first replaces each received message by the
                                  mean of its n - H nearest (nearest-neighbour mixing, rcmarl_nnm_mix); with
@@ -41,8 +42,10 @@ class RPBCAC_agent():
         # resilient aggregation rule of every consensus step: "clip" (the reference's), "trim" or "wmsr"
         # (include/rcmarl.h, rcmarl_agg_rule), or a distance-based rule over whole messages: "krum", "mkrum", "scclip"
         # or "gmed" (rcmarl_vector_rule), the spectral rule "dnc" (divide-and-conquer, rcmarl_dnc_aggregate), or the
-        # exact subset-selection rules "mda" and "smea" (rcmarl_subset_aggregate)
-        if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation) or L.is_subset_rule(aggregation)):
+        # exact subset-selection rules "mda" and "smea" (rcmarl_subset_aggregate), or the iterative outlier scissor "ios"
+        # (rcmarl_ios_aggregate)
+        if not (L.is_vector_rule(aggregation) or L.is_spectral_rule(aggregation) or L.is_subset_rule(aggregation)
+                or L.is_filter_rule(aggregation)):
             L.agg_rule(aggregation)
         self.aggregation = aggregation
         # pre-aggregation mixing of the received messages: None, "nnm", "bucket" or ("bucket", s) (rcmarl_mixing_rule)
@@ -136,13 +139,13 @@ class RPBCAC_agent():
         return out
 
     def _whole_messages(self):
-        """True if the rule aggregates whole messages (a distance-based rule, dnc, mda or smea)."""
+        """True if the rule aggregates whole messages (a distance-based rule, dnc, mda, smea or ios)."""
         return (L.is_vector_rule(self.aggregation) or L.is_spectral_rule(self.aggregation)
-                or L.is_subset_rule(self.aggregation))
+                or L.is_subset_rule(self.aggregation) or L.is_filter_rule(self.aggregation))
 
     def _with_aggregate(self, stack):
         """[n, P] device stack (own = row 0) -> [n + 1, P] whose last row is the aggregate of the distance-based, dnc,
-        mda or smea rule."""
+        mda, smea or ios rule."""
         n, P = stack.shape
         out = torch.cat([stack, torch.empty(1, P, dtype=stack.dtype, device=stack.device)])
         if L.is_spectral_rule(self.aggregation):
@@ -152,6 +155,9 @@ class RPBCAC_agent():
             L.check_subset_rule(self.H, n)
             ops.subset_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H,
                                                  L.SUBSET_RULES[self.aggregation])])
+        elif L.is_filter_rule(self.aggregation):
+            L.check_filter_rule(self.H, n)
+            ops.ios_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, L.FILTER_IOS)])
         else:
             L.check_vector_rule(self.aggregation, self.H, n)
             ops.vector_aggregate([ops.vector_job(out[n], out, P, P, list(range(n)), self.H, self.aggregation)])
@@ -159,8 +165,8 @@ class RPBCAC_agent():
 
     def _consensus_inputs(self, stack, net, round):
         """(message stack, in_nodes, H, rule) of the hidden and estimate consensus over the stacked messages.  A
-        distance-based, dnc, mda or smea rule's aggregate becomes the single in-node under clip, which returns it exactly, as in
-        Trainer.  An agent that clips does so first, then an agent that mixes does so (a bucketing agent with the draws
+        distance-based, dnc, mda, smea or ios rule's aggregate becomes the single in-node under clip, which returns it
+        exactly, as in Trainer.  An agent that clips does so first, then an agent that mixes does so (a bucketing agent with the draws
         of (net, round))."""
         stack = self._mixed(self._clipped(stack), net, round)
         if self._whole_messages():

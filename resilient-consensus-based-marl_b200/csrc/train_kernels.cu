@@ -15,6 +15,8 @@
 //                   (rcmarl_dnc_aggregate)
 //   subset_agg_kernel  exact subset selection (MDA, SMEA): averages the n - H messages that agree most as a set
 //                   (rcmarl_subset_aggregate)
+//   ios_agg_kernel  iterative outlier scissor: drops the message furthest from the re-centred mean H times
+//                   (rcmarl_ios_aggregate)
 //   nnm_mix_kernel  nearest-neighbour mixing: each message becomes the mean of its n - H nearest (rcmarl_nnm_mix)
 //   arc_clip_kernel  adaptive robust clipping: the k_clip messages furthest from the receiver's own are pulled in to
 //                   the distance of the next (rcmarl_arc_clip)
@@ -1031,6 +1033,93 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
     __syncthreads();
     subset_rule(StagedRows{xs, n}, n, nin, job.H, job.rule, job.dst, S);
     if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
+}
+
+// Iterative outlier scissor (rcmarl_ios_aggregate, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The
+// fp32 messages and the fp64 centre are staged in shared memory, rows holding +-inf are flagged as in dnc_rule, and the
+// rows still held are a bit mask.  Each iteration recomputes the centre from scratch (one thread per coordinate, rows
+// in index order) and sums each d_k on ONE warp (lane-strided fma partials, then the fixed xor butterfly), so no value
+// depends on which warp takes a row; thread 0 then removes the argmax, scanning upwards with >= so that equal
+// distances remove the higher index.  The output takes one thread per coordinate, as in dnc_rule.
+__global__ void __launch_bounds__(VEC_THREADS) ios_agg_kernel(const __grid_constant__ VectorParams P) {
+    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr int NW = VEC_THREADS / 32;
+    extern __shared__ __align__(16) float smem[];
+    __shared__ double d[MAXN];
+    __shared__ int flagged[MAXN];
+    __shared__ float wt[MAXN];
+    __shared__ unsigned held;
+    __shared__ int iters;
+    const rcmarl_vector_job& job = P.jobs[blockIdx.x];
+    const int n = job.n, nin = job.n_in;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    double* c = reinterpret_cast<double*>(smem);   // [n]
+    float* xs = smem + 2 * (int64_t)n;             // [n_in][n]
+    for (int k = 0; k < nin; ++k) {
+        const float* src = job.msgs + (int64_t)job.in_nodes[k] * job.msg_stride;
+        for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
+    }
+    __syncthreads();
+    for (int k = warp; k < nin; k += NW) {
+        const bool inf = warp_has_inf(xs + (int64_t)k * n, n, lane);
+        if (lane == 0) flagged[k] = inf ? 1 : 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        unsigned u = 0u;
+        int nf = 0;
+        for (int k = 0; k < nin; ++k) {
+            if (flagged[k]) ++nf;
+            else u |= 1u << k;
+        }
+        held = u;
+        iters = u ? max(0, job.H - nf) : 0;
+    }
+    __syncthreads();
+    const int n_iter = iters;
+    for (int it = 0; it < n_iter; ++it) {
+        const unsigned u = held;
+        const double m = (double)__popc(u);
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            double s = 0.0;
+            for (unsigned r = u; r; r &= r - 1) s += (double)xs[(__ffs(r) - 1) * n + p];
+            c[p] = s / m;
+        }
+        __syncthreads();
+        for (int k = warp; k < nin; k += NW) {
+            if (!((u >> k) & 1u)) continue;
+            const float* xk = xs + (int64_t)k * n;
+            double s = 0.0;
+            for (int p = lane; p < n; p += 32) {
+                const double e = (double)xk[p] - c[p];
+                s = fma(e, e, s);
+            }
+            s = warp_sum_f64(s);
+            if (lane == 0) d[k] = s;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int top = -1;
+            for (unsigned r = u; r; r &= r - 1) {
+                const int k = __ffs(r) - 1;
+                if (top < 0 || d[k] >= d[top]) top = k;
+            }
+            held = u & ~(1u << top);
+        }
+        __syncthreads();
+    }
+    if (tid < nin) {
+        const unsigned u = held ? held : 1u;                         // every row flagged: out = x_0
+        wt[tid] = ((u >> tid) & 1u) ? 1.f / (float)__popc(u) : 0.f;
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = |I| (1 when every row is flagged)
+        float s = 0.f, cnt = 0.f;
+        for (int k = 0; k < nin; ++k)
+            if (wt[k] != 0.f) { s += xs[k * n + p]; cnt += 1.f; }
+        job.dst[p] = s / cnt;
+    }
+    if (job.weights_out && tid < nin) job.weights_out[tid] = wt[tid];
 }
 
 // Nearest-neighbour mixing (rcmarl_nnm_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The n_in
@@ -2669,6 +2758,28 @@ int rcmarl_subset_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* str
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
     return launch_staged<subset_agg_kernel>(P, n_jobs, RCMARL_SUBSET_MAX_FLOATS, max_floats, VEC_THREADS, stream);
+}
+
+int rcmarl_ios_aggregate(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {
+    if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
+    VectorParams P;
+    RangeSet S;
+    int64_t max_floats = 0;
+    for (int j = 0; j < n_jobs; ++j) {
+        const rcmarl_vector_job& q = jobs[j];
+        if (!q.dst || !q.msgs || q.n < 1 || q.n_in < 1 || q.n_in > RCMARL_MAX_NEIGHBOURS) return RCMARL_ERR_ARG;
+        if (q.rule != RCMARL_FILTER_IOS || q.H < 0 || q.H >= q.n_in || bad_nodes(q.in_nodes, q.n_in)) return RCMARL_ERR_ARG;
+        const int64_t floats = (int64_t)(q.n_in + 2) * q.n;
+        if (floats > RCMARL_IOS_MAX_FLOATS) return RCMARL_ERR_ARG;
+        if (floats > max_floats) max_floats = floats;
+        P.jobs[j] = q;
+        // writes dst and weights_out, reads the in-node rows
+        S.w.floats(q.dst, q.n);
+        if (q.weights_out) S.w.floats(q.weights_out, q.n_in);
+        S.r.nodes(q.msgs, q.in_nodes, q.n_in, q.msg_stride, q.n);
+    }
+    if (S.overlaps()) return RCMARL_ERR_ARG;
+    return launch_staged<ios_agg_kernel>(P, n_jobs, RCMARL_IOS_MAX_FLOATS, max_floats, VEC_THREADS, stream);
 }
 
 int rcmarl_nnm_mix(const rcmarl_vector_job* jobs, int n_jobs, void* stream) {

@@ -49,6 +49,9 @@ DNC_MAX_FLOATS = 48 * 1024
 SUBSET_MDA, SUBSET_SMEA = 0, 1                    # rcmarl_subset_rule
 SUBSET_RULES = {"mda": SUBSET_MDA, "smea": SUBSET_SMEA}
 SUBSET_MAX_FLOATS = 48 * 1024
+FILTER_IOS = 0                                    # rcmarl_filter_rule
+FILTER_RULES = {"ios": FILTER_IOS}
+IOS_MAX_FLOATS = 48 * 1024
 MIX_NNM = 0                                       # rcmarl_mixing_rule
 MIXING_RULES = {"nnm": MIX_NNM}
 NNM_MAX_FLOATS = 48 * 1024
@@ -199,6 +202,7 @@ SYMBOLS = [
     ("rcmarl_vector_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_dnc_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_subset_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
+    ("rcmarl_ios_aggregate", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_nnm_mix", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_arc_clip", C.c_int, [C.POINTER(VectorJob), C.c_int, c_fp]),
     ("rcmarl_bucket_mix", C.c_int, [C.POINTER(BucketJob), C.c_int, c_fp]),
@@ -330,6 +334,19 @@ def check_subset_rule(H, n_in):
     if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
         raise RcmarlError(f"aggregation 'mda' / 'smea' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most "
                           f"{MAX_NEIGHBOURS})")
+
+
+def is_filter_rule(rule):
+    """True for the name of an iterative filtering rule (rcmarl_filter_rule): "ios"."""
+    return isinstance(rule, str) and rule in FILTER_RULES
+
+
+def check_filter_rule(H, n_in):
+    """Raise RcmarlError unless the iterative outlier scissor (rcmarl_ios_aggregate, include/rcmarl.h) allows H out of
+    n_in messages: 1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in.  Returns the rcmarl_filter_rule id."""
+    if not (1 <= n_in <= MAX_NEIGHBOURS and 0 <= H < n_in):
+        raise RcmarlError(f"aggregation 'ios' with H={H} needs 0 <= H < n_in (n_in={n_in}, at most {MAX_NEIGHBOURS})")
+    return FILTER_IOS
 
 
 def mixing_entry(mixing):

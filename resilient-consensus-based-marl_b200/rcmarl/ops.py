@@ -534,6 +534,12 @@ def subset_aggregate(jobs):
     L.check(L.lib().rcmarl_subset_aggregate(a, len(a), _stream()), "rcmarl_subset_aggregate")
 
 
+def ios_aggregate(jobs):
+    """rcmarl_ios_aggregate over rcmarl_vector_job jobs (vector_job(..., rule=L.FILTER_IOS, ...))."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.VectorJob, jobs)
+    L.check(L.lib().rcmarl_ios_aggregate(a, len(a), _stream()), "rcmarl_ios_aggregate")
+
+
 def nnm_mix(jobs):
     """rcmarl_nnm_mix over rcmarl_vector_job jobs (vector_job(dst, ..., rule=L.MIX_NNM, weights_out=[n_in * n_in])):
     mixed row k goes to dst + k * msg_stride."""

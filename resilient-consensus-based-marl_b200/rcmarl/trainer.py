@@ -63,12 +63,14 @@ class Trainer:
         # per such agent; its consensus and team jobs then read that row as their only in-node under clip, which returns
         # it exactly (the projection target phi.W3 + b3 is linear in the head).
         # The spectral rule "dnc" (divide-and-conquer) does the same through a launch of its own, and so do the exact
-        # subset-selection rules "mda" and "smea" (rcmarl_subset_rule).
+        # subset-selection rules "mda" and "smea" (rcmarl_subset_rule), and the iterative outlier scissor "ios"
+        # (rcmarl_filter_rule).
         self.vector_rule = [L.VECTOR_RULES[a] if L.is_vector_rule(a) else None for a in agg] + [None] * (NA - n_real)
         self.dnc = [L.is_spectral_rule(a) for a in agg] + [False] * (NA - n_real)
         self.subset_rule = [L.SUBSET_RULES[a] if L.is_subset_rule(a) else None for a in agg] + [None] * (NA - n_real)
+        self.ios = [L.is_filter_rule(a) for a in agg] + [False] * (NA - n_real)
         self.aggregation = [L.AGG_CLIP if L.is_vector_rule(a) or L.is_spectral_rule(a) or L.is_subset_rule(a)
-                            else L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
+                            or L.is_filter_rule(a) else L.agg_rule(a) for a in agg] + [L.AGG_CLIP] * (NA - n_real)
 
         def check_rule(i, n):
             if self.vector_rule[i] is not None:
@@ -77,6 +79,8 @@ class Trainer:
                 L.check_spectral_rule(self.H[i], n)
             elif self.subset_rule[i] is not None:
                 L.check_subset_rule(self.H[i], n)
+            elif self.ios[i]:
+                L.check_filter_rule(self.H[i], n)
             else:
                 L.check_aggregation(agg[i], self.H[i], n)
         for i in self.coop:
@@ -133,6 +137,13 @@ class Trainer:
             if i in self.coop:                     # only cooperative agents aggregate: the name alone is checked
                 self.clipping[i] = clip[i]
         self._init_attacks(attack)
+        for e in self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs + self.subset_pairs:
+            b, j, _ = self.byz_pairs[e]            # no rule-aware attack models the iterative outlier scissor
+            if self.ios[j]:
+                name = ('tailored' if e in self.tailor_pairs else 'pipeline' if e in self.pipe_pairs
+                        else 'history' if e in self.hist_pairs else 'ARC' if e in self.arc_pairs else 'subset')
+                raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose rule "
+                                    f"{agg[j]!r} the attack does not model")
         for e in self.tailor_pairs + self.pipe_pairs:   # neither attack models the receiver's history
             b, j, _ = self.byz_pairs[e]
             if self.momentum[j] is not None:
@@ -171,7 +182,7 @@ class Trainer:
                                     f"attack against agent {j}, whose job stages {floats} floats, more than the "
                                     f"{bound} the library admits")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
-        # that of each cooperative agent on dnc, then that of each on mda / smea
+        # that of each cooperative agent on dnc, then that of each on mda / smea, then that of each on ios
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
         self.vec_row = {i: NA + len(self.byz_pairs) + q for q, i in enumerate(self.vec_agents)}
         self.dnc_agents = [i for i in self.coop if self.dnc[i]]
@@ -179,11 +190,14 @@ class Trainer:
         self.subset_agents = [i for i in self.coop if self.subset_rule[i] is not None]
         self.subset_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + q
                            for q, i in enumerate(self.subset_agents)}
+        self.ios_agents = [i for i in self.coop if self.ios[i]]
+        self.ios_row = {i: NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents)
+                        + len(self.subset_agents) + q for q, i in enumerate(self.ios_agents)}
         # then the mixed rows of each cooperative agent that mixes (n_in for nnm, n_out for bucketing): mixed row k at
         # mix_row[i] + k
         self.mix_agents = [i for i in self.coop if self.mixing[i] is not None]
         self.mix_row, row = {}, NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) \
-            + len(self.subset_agents)
+            + len(self.subset_agents) + len(self.ios_agents)
         for i in self.mix_agents:
             self.mix_row[i] = row
             row += L.mixed_rows(self.mixing[i], len(self.in_nodes[i]))
@@ -229,10 +243,11 @@ class Trainer:
             self.tr[i].copy_(torch.as_tensor(nets.pack_padded(w[2], 3 * NA)))
             self.critic_local[i].copy_(torch.as_tensor(nets.pack_padded(w[3] if len(w) > 3 else w[1], 2 * NA)))
         # transmitted messages: row i is agent i's; row NA + e is the message crafted for Byzantine pair e; row
-        # vec_row[i] / dnc_row[i] / subset_row[i] the aggregate of cooperative agent i's distance-based / dnc / mda or
-        # smea rule; mix_row[i] + k its mixed message k; mom_row[i] + k its momentum row of slot k; arc_row[i] + k its
-        # clipped row of slot k
+        # vec_row[i] / dnc_row[i] / subset_row[i] / ios_row[i] the aggregate of cooperative agent i's distance-based /
+        # dnc / mda or smea / ios rule; mix_row[i] + k its mixed message k; mom_row[i] + k its momentum row of slot k;
+        # arc_row[i] + k its clipped row of slot k
         n_rows = NA + len(self.byz_pairs) + len(self.vec_agents) + len(self.dnc_agents) + len(self.subset_agents) \
+            + len(self.ios_agents) \
             + sum(L.mixed_rows(self.mixing[i], len(self.in_nodes[i])) for i in self.mix_agents) \
             + sum(len(self.in_nodes[i]) for i in self.mom_agents) + sum(len(self.in_nodes[i]) for i in self.arc_agents)
         self.msg_c = torch.zeros(n_rows, self.PC, **f32)
@@ -244,6 +259,8 @@ class Trainer:
         # ... and of each mda / smea aggregate: row 2q critic, 2q + 1 TR of subset_agents[q]
         self.subset_weights = (torch.zeros(2 * len(self.subset_agents), L.MAX_NEIGHBOURS, **f32)
                                if self.subset_agents else None)
+        # ... and of each ios aggregate: row 2q critic, 2q + 1 TR of ios_agents[q]
+        self.ios_weights = torch.zeros(2 * len(self.ios_agents), L.MAX_NEIGHBOURS, **f32) if self.ios_agents else None
         # mixing matrix M (row-major [n_rows][n_in], n_rows = len(_rule_nodes(i))) of each agent that mixes: row 2q
         # critic, 2q + 1 TR of mix_agents[q]
         self.mix_weights = torch.zeros(2 * len(self.mix_agents), L.MAX_NEIGHBOURS ** 2, **f32) if self.mix_agents else None
@@ -402,16 +419,16 @@ class Trainer:
         return list(range(self.mix_row[j], self.mix_row[j] + L.mixed_rows(self.mixing[j], len(self.in_nodes[j]))))
 
     def neighbour_weights(self):
-        """{cooperative agent i with a distance-based, the dnc or an mda / smea rule: float32 [2, n_in]}: the weight w_k
-        its rule gave each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the message
-        crafted for i) in the last epoch of the last update round; row 0 for the critic, row 1 for the team-reward net.
-        For an agent that mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry
+        """{cooperative agent i with a distance-based, the dnc, an mda / smea or the ios rule: float32 [2, n_in]}: the
+        weight w_k its rule gave each in-neighbour (in_nodes[i] order, a Byzantine neighbour's entry standing for the
+        message crafted for i) in the last epoch of the last update round; row 0 for the critic, row 1 for the
+        team-reward net.  For an agent that mixes, the rule weighs the mixed messages (the n_out rows of a bucketing agent), and the entry
         is the effective weight w M of each in-neighbour.  For an agent with momentum, entry k is the weight of slot k's
         momentum row.  For an agent that clips, with w' that weight and c its clipping factors (clipping_factors), entry
         k >= 1 is w'_k c_k and entry 0 is w'_0 + sum_{k >= 1} w'_k (1 - c_k): a clipped row is x_0 + c_k (x_k - x_0)."""
         out = {}
         for agents, weights in ((self.vec_agents, self.vec_weights), (self.dnc_agents, self.dnc_weights),
-                                (self.subset_agents, self.subset_weights)):
+                                (self.subset_agents, self.subset_weights), (self.ios_agents, self.ios_weights)):
             if not agents:
                 continue
             w = weights.cpu().numpy()
@@ -849,7 +866,7 @@ class Trainer:
 
         cons_jobs, team_jobs, team_apply = [], [], []
         for n, i in enumerate(coop):
-            agg_row = self.vec_row.get(i, self.dnc_row.get(i, self.subset_row.get(i)))
+            agg_row = self.vec_row.get(i, self.dnc_row.get(i, self.subset_row.get(i, self.ios_row.get(i))))
             if agg_row is not None:                        # the aggregate as the single in-node: clip returns it exactly
                 nodes, H, rule = [agg_row], 0, L.AGG_CLIP
             else:
@@ -935,6 +952,14 @@ class Trainer:
                 subset_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], self.subset_rule[i],
                                                   weights_out=self.subset_weights[2 * q + t]))
         subset_jobs = ops.job_array(L.VectorJob, subset_jobs) if subset_jobs else None
+        # the ios aggregates likewise, in one launch of their own
+        ios_jobs = []
+        for q, i in enumerate(self.ios_agents):
+            nodes, row = self._rule_nodes(i), self.ios_row[i]
+            for t, (msgs, P) in enumerate(((self.msg_c, self.PC), (self.msg_t, self.PT))):
+                ios_jobs.append(ops.vector_job(msgs[row], msgs, P, P, nodes, self.H[i], L.FILTER_IOS,
+                                               weights_out=self.ios_weights[2 * q + t]))
+        ios_jobs = ops.job_array(L.VectorJob, ios_jobs) if ios_jobs else None
 
         for epoch in range(self.n_epochs):                                 # :100
             # ---------------- I) local updates (:105-121)
@@ -1017,6 +1042,9 @@ class Trainer:
                 self.launches += 1
             if subset_jobs is not None:
                 ops.subset_aggregate(subset_jobs)
+                self.launches += 1
+            if ios_jobs is not None:
+                ops.ios_aggregate(ios_jobs)
                 self.launches += 1
             # ---------------- II) resilient consensus (:125-145)
             if coop:

@@ -1,10 +1,11 @@
 """Byzantine attacks against each resilient aggregation rule on the C2 team: 4 cooperative agents (H = 1) and agent 4
 Byzantine (include/rcmarl.h, rcmarl_attack), for every rule (by default clip, trim, wmsr; any of the coordinate rules,
-the distance-based krum, mkrum, scclip, gmed, the divide-and-conquer dnc and the exact subset-selection mda and smea)
+the distance-based krum, mkrum, scclip, gmed, the divide-and-conquer dnc, the exact subset-selection mda and smea, and
+the iterative outlier scissor ios)
 x attack (alie, ipm, gauss) over the learning harness's seeds
 (tests/golden/ref_learning.npz, scenario malicious/H1: the start weights and task of each seed; agent 4 keeps its weights
 and learns like a Faulty agent).  Reported per cell: the cooperative team's return and the cooperative critics' estimate
-of it, means of the last 500 episodes, over the seeds; for a distance-based rule, dnc, mda or smea also the mean weight the receivers of
+of it, means of the last 500 episodes, over the seeds; for a distance-based rule, dnc, mda, smea or ios also the mean weight the receivers of
 agent 4 gave its crafted message in the last epoch of the last round (Trainer.neighbour_weights, both nets), over the
 seeds.  The attack list (by default alie 1.0, ipm 0.5, gauss 0.3) may also name the min-max / min-sum attacks
 (rcmarl_adaptive_attack: minmax_uv, minmax_std, minmax_sgn, minsum_uv, minsum_std, minsum_sgn, scale 1 = the paper's
@@ -35,7 +36,8 @@ pipeline search through the receiver's clipping step as well (rcmarl_history_arc
 against a receiver that does not clip they are the history attacks, and mda or smea cells are marked refused.  The
 subset-aware attacks (subset_uv, subset_std, subset_sgn, range multiplier 2 by default) run that search through an mda or
 smea receiver's exact subset selection as well (rcmarl_subset_history_attack / rcmarl_subset_pipeline_attack); against
-any other rule they are the ARC-aware attacks.
+any other rule they are the ARC-aware attacks.  No rule-aware attack (tailored, pipeline, history, ARC-aware or
+subset-aware) models ios: those cells are marked refused.
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -44,7 +46,7 @@ agent 4 copied in the last epoch of the last round (Trainer.mimic_targets, criti
 Before the sweep it times one C2 update round at the benchmark's size with agent 4 Byzantine against the same round with
 agent 4 Faulty, alternating the two trainers round by round (CUDA events around update_round).  When the rule list names
 a distance-based rule it also times the round (agent 4 Byzantine) with every cooperative agent on clip, gmed and mkrum,
-and when it names dnc, mda or smea, on clip and each of those it names (all of them when it names several),
+and when it names dnc, mda, smea or ios, on clip and each of those it names (all of them when it names several),
 alternated the same way.  When the attack list names an adaptive attack it also times the round with agent 4 on
 minmax_std against the same round on gauss, alternated the same way, and when it names a tailored attack, the round on
 tailored_std (every cooperative agent on clip) against gauss, when it names a pipeline attack, the round on
@@ -113,7 +115,7 @@ def split_rule(rule):
 BASES = tuple(split_rule(r)[1] for r in RULES)
 VECTOR = ("krum", "mkrum", "scclip", "gmed")
 SUBSET = ("mda", "smea")
-WHOLE = VECTOR + ("dnc",) + SUBSET              # the rules that report neighbour weights
+WHOLE = VECTOR + ("dnc",) + SUBSET + ("ios",)   # the rules that report neighbour weights
 ADAPTIVE = ("minmax_uv", "minmax_std", "minmax_sgn", "minsum_uv", "minsum_std", "minsum_sgn")
 TAILORED = ("tailored_uv", "tailored_std", "tailored_sgn")
 PIPELINE = ("pipeline_uv", "pipeline_std", "pipeline_sgn")
@@ -161,10 +163,10 @@ def timing():
 
 
 def timed_rules():
-    """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc, mda and
-    smea where listed."""
+    """The rules rule_timing compares: clip, then gmed and mkrum if a distance-based rule is listed, and dnc, mda,
+    smea and ios where listed."""
     return (("clip",) + (("gmed", "mkrum") if any(r in VECTOR for r in BASES) else ())
-            + tuple(r for r in ("dnc",) + SUBSET if r in BASES))
+            + tuple(r for r in ("dnc",) + SUBSET if r in BASES) + (("ios",) if "ios" in BASES else ()))
 
 
 def rule_timing():

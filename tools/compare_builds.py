@@ -1,9 +1,9 @@
 """Compare the outputs of the distance-based rules (rcmarl_vector_aggregate), the min-max / min-sum attacks
 (rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
 (rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack), the subset-selection rules MDA / SMEA
-(rcmarl_subset_aggregate), per-neighbour momentum (rcmarl_momentum_mix), the pipeline attacks
-(rcmarl_pipeline_attack) and the history attacks (rcmarl_history_attack) between two builds of librcmarl.so, bit for
-bit.  Their kernels share their bodies with tailored_attack_kernel, pipeline_attack_kernel and history_attack_kernel
+(rcmarl_subset_aggregate), per-neighbour momentum (rcmarl_momentum_mix), the iterative outlier scissor
+(rcmarl_ios_aggregate), the pipeline attacks (rcmarl_pipeline_attack) and the history attacks (rcmarl_history_attack)
+between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with tailored_attack_kernel, pipeline_attack_kernel and history_attack_kernel
 (vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows, bucket_draw / bucket_means, tailored_stage /
 tailored_range, the candidate search and the momentum step in csrc/train_kernels.cu), so a change there may change
 their register allocation and SASS; this shows whether it changed anything they compute.
@@ -13,7 +13,8 @@ around a common centre, four of them 1e3 times larger and one holding 1e30; ever
 per job, repeated in-nodes) with the weights, every min-max / min-sum attack at n_honest 1 .. 16 (scale 1.5, with
 gamma), DnC, nnm and bucketing (s = 1, 2, 3) at n_in 1 .. 16 with their weights or mixing matrices, and every tailored
 attack x rule at n_in 2 .. 16 (scale 2, with gamma), MDA and SMEA at n_in 1 .. 16 (H drawn per job, with the
-weights), momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), every pipeline
+weights), momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), IOS at n_in
+1 .. 16 (H drawn per job, with the weights), every pipeline
 attack x rule (DnC included) x mixing (none, nnm, bucketing at s = 2 with 3 samples) at n_in 2 .. 16 with gamma and
 model_out, and history_std x rule at n_in 2 .. 16 for (beta, first) = (0.9, 0), (0.99, 0), (0.5, 1), at the trainer's
 parameter counts.  Entry points a build does not export are skipped when loading it, so a
@@ -132,6 +133,17 @@ if hasattr(lib, "rcmarl_momentum_mix"):
                                            int(step == 0)) for q in range(16)])
         named.update({f"momentum_{step}_{q}": np.concatenate([dsts[q].cpu().numpy().ravel(), Ms[q].cpu().numpy().ravel()])
                       for q in range(16)})
+if hasattr(lib, "rcmarl_ios_aggregate"):
+    jobs, dsts = [], []
+    rs_ios = np.random.RandomState(78)                             # its own draws: the later inputs stay the same
+    for n_in in range(1, 17):
+        d = torch.full((P + 16,), float("nan"), device="cuda")
+        nodes = [int(x) for x in rs_ios.choice(24, size=n_in)]
+        jobs.append(ops.vector_job(d[:P], msgs, P, PC[n_in % 4], nodes, int(rs_ios.randint(0, n_in)), L.FILTER_IOS,
+                                   weights_out=d[P:]))
+        dsts.append(d)
+    ops.ios_aggregate(jobs)
+    named.update({f"ios_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
 
 
 def attack_cases(rule):
@@ -205,7 +217,8 @@ def main():
     only = sorted(set(a.files) ^ set(b.files))
     diff = [k for k in common if a[k].tobytes() != b[k].tobytes()]
     print(f"{len(common)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix, "
-          "tailored_attack, subset_aggregate, momentum_mix, pipeline_attack and history_attack outputs): "
+          "tailored_attack, subset_aggregate, momentum_mix, ios_aggregate, pipeline_attack and history_attack "
+          "outputs): "
           + ("bitwise equal" if not diff else f"{len(diff)} differ: {diff[:8]}")
           + (f"; {len(only)} from an entry point only one build exports, not compared" if only else ""))
     sys.exit(1 if diff or not common else 0)
