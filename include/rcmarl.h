@@ -258,7 +258,8 @@ int rcmarl_adaptive_attack(const rcmarl_adaptive_attack_job* jobs_host, int n_jo
 #define RCMARL_TAILORED_MAX_FLOATS (19 * 1536)
 typedef enum {
     RCMARL_TAILOR_COORD = 0, RCMARL_TAILOR_VECTOR = 1, RCMARL_TAILOR_SPECTRAL = 2,
-    RCMARL_TAILOR_SUBSET = 3    /* rule: rcmarl_subset_rule; only the subset forms (rcmarl_subset_pipeline_attack) */
+    RCMARL_TAILOR_SUBSET = 3,   /* rule: rcmarl_subset_rule; only the subset forms (rcmarl_subset_pipeline_attack) */
+    RCMARL_TAILOR_FILTER = 4    /* rule: rcmarl_filter_rule; only the IOS forms (rcmarl_ios_pipeline_attack) */
 } rcmarl_tailored_family;
 typedef struct {
     float* dst;                 /* the crafted message (packed network) */
@@ -827,6 +828,48 @@ int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs_host, int n_
 #define RCMARL_SUBSET_ATTACK_MAX_FLOATS (35 * 1421)
 int rcmarl_subset_pipeline_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, int arc, void* stream);
 int rcmarl_subset_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, int arc, void* stream);
+
+/* IOS-aware Byzantine messages (rcmarl_ios_pipeline_attack, rcmarl_ios_history_attack): the pipeline and history
+ * attacks, with or without ARC, against a receiver j whose rule is the iterative outlier scissor (rcmarl_ios_aggregate).
+ * Threat model: that of the base attack, plus j's rule.  The jobs are rcmarl_pipeline_attack_job and
+ * rcmarl_history_attack_job with every field's meaning unchanged, except that the family is RCMARL_TAILOR_FILTER and the
+ * rule an rcmarl_filter_rule:
+ *   rcmarl_ios_pipeline_attack   received -> [ARC] -> [nnm | bucket] -> IOS (the pipeline form; arc = 1:
+ *                                rcmarl_pipeline_arc_attack's clipping step);
+ *   rcmarl_ios_history_attack    received -> momentum -> [ARC] -> IOS (the history form; arc = 1:
+ *                                rcmarl_history_arc_attack's clipping step).
+ *   Rule.    For each candidate gamma_i (and each shuffle sample q under bucketing), rcmarl_ios_aggregate's arithmetic
+ *            bit for bit over the n_rows rows the base attack's rule reads, at H (the same device code): the flagged
+ *            set F, max(0, H - |F|) removals, each with the fp64 centre from scratch (staged, as DnC's mean, in front of
+ *            the real slots), the fp64 d_k (one warp per row, the fixed xor butterfly) and the argmax removed (equal d:
+ *            the higher index first, so of colluding crafted slots, whose rows are bitwise equal, the highest goes
+ *            first), then the fp32 mean of the rows left, summed from 0.  Every candidate runs the full loop.
+ *   Everything else is the base attack's: mu, d, Gamma, the K + 1 candidates, O_i, the pick, dst, gamma_out and
+ *   model_out = R(gamma_i*) (under bucketing R_0, with the attacker's sample 0), with ARC (arc = 1) exactly where the ARC
+ *   forms put it.
+ * At H = 0 with finite rows, the rule is the plain mean, bitwise rcmarl_dnc_aggregate's at H = 0, so dst, gamma_out and
+ * model_out are bitwise those of the base entry point with family SPECTRAL (DnC) at H = 0 (rcmarl_pipeline_attack,
+ * rcmarl_history_attack, or their ARC forms when arc = 1).  Exactness: under the base attack's conditions, model_out is
+ * bitwise what j computes from the messages actually sent -- [rcmarl_momentum_mix] -> [rcmarl_arc_clip] ->
+ * [rcmarl_nnm_mix] -> rcmarl_ios_aggregate; under bucketing, with the attacker's sample 0 in place of j's secret
+ * shuffle.  NaN inputs are not supported.  One CTA per job, exactly the staging of the DnC form (the real slots, mu, d,
+ * the candidate, the output row, the mixed or crafted rows, the clipped rows and the fp64 centre) in shared memory;
+ * fixed summation orders, no atomics -- bitwise reproducible, independent of the job order and of how jobs are split
+ * over launches.
+ * Refused (RCMARL_ERR_ARG, nothing launched, dst, gamma_out and model_out untouched): everything the base entry point
+ * (arc = 1: its ARC form) refuses except the family -- a family other than RCMARL_TAILOR_FILTER, a rule other than
+ * RCMARL_FILTER_IOS, H outside [0, n_rows) -- arc other than 0 or 1, with arc = 1 a crafted slot 0, and a staging size
+ * (n_real + n_mixed + 6 + k_clip) * n above RCMARL_PIPELINE_MAX_FLOATS in the pipeline form and (n_in + 6 + k_clip) * n
+ * above RCMARL_HISTORY_MAX_FLOATS in the history form (n_real, n_mixed as for rcmarl_pipeline_attack; k_clip =
+ * (2 * H * (n_in - H)) / n_in with arc = 1, else 0): the DnC form's staging under the base bounds, so the IOS forms
+ * admit exactly the shapes the DnC forms admit.  At the 16-agent team-reward net (1421 parameters) with n_in = 16 and
+ * 15 real slots: the pipeline form without mixing, and under bucketing with s >= 2, at every H with or without ARC;
+ * under bucketing with s = 1 without ARC, and with ARC k_clip <= 1 (H = 1); under nnm without ARC, and with ARC no
+ * H >= 1; the history form without ARC, and with ARC no H >= 1.  Every shape of the 5-agent team (n_in <= 5, at most
+ * 761 parameters) is admitted in all four forms.  Static shared memory plus the bound stays under the 227 KB a CTA may
+ * opt in to. */
+int rcmarl_ios_pipeline_attack(const rcmarl_pipeline_attack_job* jobs_host, int n_jobs, int arc, void* stream);
+int rcmarl_ios_history_attack(const rcmarl_history_attack_job* jobs_host, int n_jobs, int arc, void* stream);
 
 /* ---------------------------------------------------------------------------
  * K1 / K3.  Batched forward values:  out[row] = add_scale * add[row*add_stride + add_off]

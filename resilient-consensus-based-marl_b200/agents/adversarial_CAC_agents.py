@@ -88,7 +88,9 @@ class Byzantine_CAC_agent(Faulty_CAC_agent):
     rcmarl_pipeline_arc_attack (against a receiver that does not clip it is the history attack); or that search through
     an mda / smea receiver's exact subset selection as well, ("subset_uv" | "subset_std" | "subset_sgn", s), at
     rcmarl_subset_history_attack / rcmarl_subset_pipeline_attack (against a receiver on any other rule it is the ARC
-    attack); or the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
+    attack); or that search through an ios receiver's iterative outlier scissor as well, ("ios_uv" | "ios_std" |
+    "ios_sgn", s), at rcmarl_ios_history_attack / rcmarl_ios_pipeline_attack (against a receiver on any other rule it
+    is the subset attack); or the dissensus attack that cancels (eps = 1) or reverses (eps > 1) the receiver's honest pull, ("dissensus", eps)
     with eps >= 0, at rcmarl_dissensus_attack; or the mimic attack that copies the honest neighbour furthest along the
     honest messages' principal direction, ("mimic", T0) with T0 the number of power steps, an integer in 0 .. 2^31 - 1,
     after which the direction is frozen, at rcmarl_mimic_attack).

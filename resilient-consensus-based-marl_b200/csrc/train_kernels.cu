@@ -1041,18 +1041,89 @@ __global__ void __launch_bounds__(VEC_THREADS) subset_agg_kernel(const __grid_co
 // in index order) and sums each d_k on ONE warp (lane-strided fma partials, then the fixed xor butterfly), so no value
 // depends on which warp takes a row; thread 0 then removes the argmax, scanning upwards with >= so that equal
 // distances remove the higher index.  The output takes one thread per coordinate, as in dnc_rule.
-__global__ void __launch_bounds__(VEC_THREADS) ios_agg_kernel(const __grid_constant__ VectorParams P) {
-    constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+struct IosShared {
+    double d[RCMARL_MAX_NEIGHBOURS];
+    int flagged[RCMARL_MAX_NEIGHBOURS];
+    float wt[RCMARL_MAX_NEIGHBOURS];
+    unsigned held;
+    int iters;
+};
+
+// The body of rcmarl_ios_aggregate over nin rows row(0) .. row(nin - 1) of n floats in shared memory: writes the
+// aggregate to out[0:n] and leaves w_k in S.wt (the caller synchronises before reading either).  c is a shared work
+// row of n doubles (the centre).  Called by the whole CTA of VEC_THREADS threads; Row maps a row index to its staged
+// row.
+template <class Row>
+__device__ __forceinline__ void ios_rule(const Row& row, int n, int nin, int H, double* c, float* out, IosShared& S) {
     constexpr int NW = VEC_THREADS / 32;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (int k = warp; k < nin; k += NW) {
+        const bool inf = warp_has_inf(row(k), n, lane);
+        if (lane == 0) S.flagged[k] = inf ? 1 : 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        unsigned u = 0u;
+        int nf = 0;
+        for (int k = 0; k < nin; ++k) {
+            if (S.flagged[k]) ++nf;
+            else u |= 1u << k;
+        }
+        S.held = u;
+        S.iters = u ? max(0, H - nf) : 0;
+    }
+    __syncthreads();
+    const int n_iter = S.iters;
+    for (int it = 0; it < n_iter; ++it) {
+        const unsigned u = S.held;
+        const double m = (double)__popc(u);
+        for (int p = tid; p < n; p += VEC_THREADS) {
+            double s = 0.0;
+            for (unsigned r = u; r; r &= r - 1) s += (double)row.at(__ffs(r) - 1, p);
+            c[p] = s / m;
+        }
+        __syncthreads();
+        for (int k = warp; k < nin; k += NW) {
+            if (!((u >> k) & 1u)) continue;
+            const float* xk = row(k);
+            double s = 0.0;
+            for (int p = lane; p < n; p += 32) {
+                const double e = (double)xk[p] - c[p];
+                s = fma(e, e, s);
+            }
+            s = warp_sum_f64(s);
+            if (lane == 0) S.d[k] = s;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int top = -1;
+            for (unsigned r = u; r; r &= r - 1) {
+                const int k = __ffs(r) - 1;
+                if (top < 0 || S.d[k] >= S.d[top]) top = k;
+            }
+            S.held = u & ~(1u << top);
+        }
+        __syncthreads();
+    }
+    if (tid < nin) {
+        const unsigned u = S.held ? S.held : 1u;                     // every row flagged: out = x_0
+        S.wt[tid] = ((u >> tid) & 1u) ? 1.f / (float)__popc(u) : 0.f;
+    }
+    __syncthreads();
+    for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = |I| (1 when every row is flagged)
+        float s = 0.f, cnt = 0.f;
+        for (int k = 0; k < nin; ++k)
+            if (S.wt[k] != 0.f) { s += row.at(k, p); cnt += 1.f; }
+        out[p] = s / cnt;
+    }
+}
+
+__global__ void __launch_bounds__(VEC_THREADS) ios_agg_kernel(const __grid_constant__ VectorParams P) {
     extern __shared__ __align__(16) float smem[];
-    __shared__ double d[MAXN];
-    __shared__ int flagged[MAXN];
-    __shared__ float wt[MAXN];
-    __shared__ unsigned held;
-    __shared__ int iters;
+    __shared__ IosShared S;
     const rcmarl_vector_job& job = P.jobs[blockIdx.x];
     const int n = job.n, nin = job.n_in;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     double* c = reinterpret_cast<double*>(smem);   // [n]
     float* xs = smem + 2 * (int64_t)n;             // [n_in][n]
     for (int k = 0; k < nin; ++k) {
@@ -1060,66 +1131,8 @@ __global__ void __launch_bounds__(VEC_THREADS) ios_agg_kernel(const __grid_const
         for (int p = tid; p < n; p += VEC_THREADS) xs[k * n + p] = __ldg(src + p);
     }
     __syncthreads();
-    for (int k = warp; k < nin; k += NW) {
-        const bool inf = warp_has_inf(xs + (int64_t)k * n, n, lane);
-        if (lane == 0) flagged[k] = inf ? 1 : 0;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        unsigned u = 0u;
-        int nf = 0;
-        for (int k = 0; k < nin; ++k) {
-            if (flagged[k]) ++nf;
-            else u |= 1u << k;
-        }
-        held = u;
-        iters = u ? max(0, job.H - nf) : 0;
-    }
-    __syncthreads();
-    const int n_iter = iters;
-    for (int it = 0; it < n_iter; ++it) {
-        const unsigned u = held;
-        const double m = (double)__popc(u);
-        for (int p = tid; p < n; p += VEC_THREADS) {
-            double s = 0.0;
-            for (unsigned r = u; r; r &= r - 1) s += (double)xs[(__ffs(r) - 1) * n + p];
-            c[p] = s / m;
-        }
-        __syncthreads();
-        for (int k = warp; k < nin; k += NW) {
-            if (!((u >> k) & 1u)) continue;
-            const float* xk = xs + (int64_t)k * n;
-            double s = 0.0;
-            for (int p = lane; p < n; p += 32) {
-                const double e = (double)xk[p] - c[p];
-                s = fma(e, e, s);
-            }
-            s = warp_sum_f64(s);
-            if (lane == 0) d[k] = s;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            int top = -1;
-            for (unsigned r = u; r; r &= r - 1) {
-                const int k = __ffs(r) - 1;
-                if (top < 0 || d[k] >= d[top]) top = k;
-            }
-            held = u & ~(1u << top);
-        }
-        __syncthreads();
-    }
-    if (tid < nin) {
-        const unsigned u = held ? held : 1u;                         // every row flagged: out = x_0
-        wt[tid] = ((u >> tid) & 1u) ? 1.f / (float)__popc(u) : 0.f;
-    }
-    __syncthreads();
-    for (int p = tid; p < n; p += VEC_THREADS) {                     // cnt = |I| (1 when every row is flagged)
-        float s = 0.f, cnt = 0.f;
-        for (int k = 0; k < nin; ++k)
-            if (wt[k] != 0.f) { s += xs[k * n + p]; cnt += 1.f; }
-        job.dst[p] = s / cnt;
-    }
-    if (job.weights_out && tid < nin) job.weights_out[tid] = wt[tid];
+    ios_rule(StagedRows{xs, n}, n, nin, job.H, c, job.dst, S);
+    if (job.weights_out && tid < nin) job.weights_out[tid] = S.wt[tid];
 }
 
 // Nearest-neighbour mixing (rcmarl_nnm_mix, include/rcmarl.h): one CTA of VEC_THREADS threads per job.  The n_in
@@ -1696,9 +1709,15 @@ struct SubsetAttackShared {
     SubsetKnownBest KB;
 };
 
-template <bool ARC, bool SUBSET>
+// The receiver's rule stage in the pipeline and history searches: the base rules (families COORD, VECTOR and
+// SPECTRAL), MDA / SMEA (the subset forms, subset_rule) or IOS (the IOS forms, ios_rule, whose fp64 centre takes the
+// region in front of the real slots that DnC's mean takes).
+enum RuleStage { STAGE_BASE = 0, STAGE_SUBSET = 1, STAGE_IOS = 2 };
+
+template <bool ARC, int STAGE>
 __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const __grid_constant__ PipelineParams P) {
     constexpr int MAXN = RCMARL_MAX_NEIGHBOURS;
+    constexpr bool SUBSET = STAGE == STAGE_SUBSET, IOS = STAGE == STAGE_IOS;
     extern __shared__ __align__(16) float smem[];
     __shared__ TailoredShared S;
     __shared__ DncShared D;
@@ -1719,8 +1738,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
         nh += (job.honest_mask >> k) & 1u;
         nr += job.slots[k] >= 0 ? 1 : 0;
     }
-    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC: [n]
-    float* xs = smem + (job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
+    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC, IOS: [n]
+    float* xs = smem + (IOS || job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
     float* mu = xs + (int64_t)nr * n;              // [n]
     float* d = mu + n;                             // [n]
     float* cand = d + n;                           // [n]: m(gamma_i), every crafted slot
@@ -1765,6 +1784,11 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
         if (tid == 0) SU.KB.urows = 0u;
         __syncthreads();
     }
+    IosShared* I = nullptr;                       // IOS: the rule's scratch
+    if constexpr (IOS) {
+        __shared__ IosShared IS;
+        I = &IS;
+    }
     const auto eval = [&](int q) {
         if constexpr (ARC)                        // once per candidate: every crafted slot holds it, one d_k for all
             if (q == 0)
@@ -1779,6 +1803,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) pipeline_attack_kernel(const _
         }
         if constexpr (SUBSET)
             subset_rule(rows, n, nrows, job.H, job.rule, z, U->S, known, U->flag, U->DK, known ? &U->KB : nullptr);
+        else if constexpr (IOS)
+            ios_rule(rows, n, nrows, job.H, mu64, z, *I);
         else if (job.family == RCMARL_TAILOR_COORD)
             coord_rule(rows, n, nrows, job.H, job.rule, z);
         else if (job.family == RCMARL_TAILOR_VECTOR)
@@ -1860,8 +1886,9 @@ __device__ __forceinline__ float momentum_invert(float t, float c, const float* 
     return __fadd_rn(c, __fdiv_rn(__fsub_rn(__fsub_rn(t, c), __fmul_rn(beta, old)), __fsub_rn(1.f, beta)));
 }
 
-template <bool ARC, bool SUBSET>
+template <bool ARC, int STAGE>
 __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __grid_constant__ HistoryParams P) {
+    constexpr bool SUBSET = STAGE == STAGE_SUBSET, IOS = STAGE == STAGE_IOS;
     extern __shared__ __align__(16) float smem[];
     __shared__ TailoredShared S;
     __shared__ DncShared D;
@@ -1876,8 +1903,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
         nr += job.slots[k] >= 0 ? 1 : 0;
     }
     const int k0 = __ffs(hj.own_mask) - 1;         // the lowest own slot
-    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC: [n]
-    float* xs = smem + (job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
+    double* mu64 = reinterpret_cast<double*>(smem);                 // DnC, IOS: [n]
+    float* xs = smem + (IOS || job.family == RCMARL_TAILOR_SPECTRAL ? 2 * (int64_t)n : 0);   // [nr][n]
     float* mu = xs + (int64_t)nr * n;              // [n]
     float* d = mu + n;                             // [n]
     float* cand = d + n;                           // [n]: the target t(gamma_i)
@@ -1920,6 +1947,11 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
         if (tid == 0) SU.KB.urows = 0u;
         __syncthreads();
     }
+    IosShared* I = nullptr;                        // IOS: the rule's scratch
+    if constexpr (IOS) {
+        __shared__ IosShared IS;
+        I = &IS;
+    }
     // a_k of every crafted slot for the target in cand, then the rule into z; returns whether every crafted message is
     // finite (the same in every thread).  An infeasible candidate skips the rule unless `always`: its objective is -inf
     // whatever the rule gives.
@@ -1944,6 +1976,8 @@ __global__ void __launch_bounds__(ADA_THREADS, 1) history_attack_kernel(const __
             arc_rows(xs, S.off, n, nin, job.H, ~real & ((1u << nin) - 1u), 0u, 0, clip, A);
         if constexpr (SUBSET)
             subset_rule(rows, n, nin, job.H, job.rule, z, U->S, known, U->flag, U->DK, known ? &U->KB : nullptr);
+        else if constexpr (IOS)
+            ios_rule(rows, n, nin, job.H, mu64, z, *I);
         else if (job.family == RCMARL_TAILOR_COORD)
             coord_rule(rows, n, nin, job.H, job.rule, z);
         else if (job.family == RCMARL_TAILOR_VECTOR)
@@ -2959,9 +2993,22 @@ static bool bad_subset_receiver(int family, int rule, int H, int n_rows) {
            H >= n_rows;
 }
 
-template <bool ARC, bool SUBSET>
+// the receiver's rule in an IOS form of the pipeline or history search: family FILTER, IOS, 0 <= H < n_rows
+static bool bad_ios_receiver(int family, int rule, int H, int n_rows) {
+    return family != RCMARL_TAILOR_FILTER || rule != RCMARL_FILTER_IOS || H < 0 || H >= n_rows;
+}
+
+// the receiver's rule for the rule stage STAGE of the pipeline or history search
+template <int STAGE>
+static bool bad_stage_receiver(int family, int rule, int H, int n_rows) {
+    if (STAGE == STAGE_SUBSET) return bad_subset_receiver(family, rule, H, n_rows);
+    if (STAGE == STAGE_IOS) return bad_ios_receiver(family, rule, H, n_rows);
+    return bad_receiver_rule(family, rule, H, n_rows);
+}
+
+template <bool ARC, int STAGE>
 static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
-    constexpr int bound = SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_PIPELINE_MAX_FLOATS;
+    constexpr int bound = STAGE == STAGE_SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_PIPELINE_MAX_FLOATS;
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     PipelineParams P;
     RangeSet S;
@@ -2982,9 +3029,10 @@ static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         } else if (pj.mixing != RCMARL_PIPE_NONE) {
             return RCMARL_ERR_ARG;
         }
-        if (SUBSET ? bad_subset_receiver(q.family, q.rule, q.H, n_rows) : bad_receiver_rule(q.family, q.rule, q.H, n_rows))
-            return RCMARL_ERR_ARG;
-        int64_t floats = (int64_t)(n_real + n_mixed + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        if (bad_stage_receiver<STAGE>(q.family, q.rule, q.H, n_rows)) return RCMARL_ERR_ARG;
+        // DnC's mean and IOS's centre: n doubles in front of the real slots
+        const bool f64 = q.family == RCMARL_TAILOR_SPECTRAL || q.family == RCMARL_TAILOR_FILTER;
+        int64_t floats = (int64_t)(n_real + n_mixed + 4 + (f64 ? 2 : 0)) * q.n;
         if (arc_staging(q, ARC, floats) || floats > bound) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = pj;
@@ -2995,12 +3043,12 @@ static int pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, v
         S.r.nodes(q.msgs, q.slots, q.n_in, q.msg_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<pipeline_attack_kernel<ARC, SUBSET>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
+    return launch_staged<pipeline_attack_kernel<ARC, STAGE>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
 }
 
-template <bool ARC, bool SUBSET>
+template <bool ARC, int STAGE>
 static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
-    constexpr int bound = SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_HISTORY_MAX_FLOATS;
+    constexpr int bound = STAGE == STAGE_SUBSET ? RCMARL_SUBSET_ATTACK_MAX_FLOATS : RCMARL_HISTORY_MAX_FLOATS;
     if (!jobs || n_jobs < 1 || n_jobs > RCMARL_MAX_JOBS) return RCMARL_ERR_ARG;
     HistoryParams P;
     RangeSet S;
@@ -3010,15 +3058,15 @@ static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         const rcmarl_tailored_attack_job& q = hj.attack;
         int n_real = 0;
         if (bad_tailored_slots(q, n_real)) return RCMARL_ERR_ARG;
-        if (SUBSET ? bad_subset_receiver(q.family, q.rule, q.H, q.n_in) : bad_receiver_rule(q.family, q.rule, q.H, q.n_in))
-            return RCMARL_ERR_ARG;
+        if (bad_stage_receiver<STAGE>(q.family, q.rule, q.H, q.n_in)) return RCMARL_ERR_ARG;
         if (!hj.ref || !hj.momentum) return RCMARL_ERR_ARG;
         if (!std::isfinite(hj.beta) || hj.beta < 0.f || hj.beta >= 1.f || (hj.first != 0 && hj.first != 1))
             return RCMARL_ERR_ARG;
         if (hj.own_mask == 0u || (hj.own_mask >> q.n_in)) return RCMARL_ERR_ARG;
         for (int k = 0; k < q.n_in; ++k)
             if (((hj.own_mask >> k) & 1u) && q.slots[k] >= 0) return RCMARL_ERR_ARG;   // an own bit on a real slot
-        int64_t floats = (int64_t)(q.n_in + 4 + (q.family == RCMARL_TAILOR_SPECTRAL ? 2 : 0)) * q.n;
+        const bool f64 = q.family == RCMARL_TAILOR_SPECTRAL || q.family == RCMARL_TAILOR_FILTER;
+        int64_t floats = (int64_t)(q.n_in + 4 + (f64 ? 2 : 0)) * q.n;
         if (arc_staging(q, ARC, floats) || floats > bound) return RCMARL_ERR_ARG;
         if (floats > max_floats) max_floats = floats;
         P.jobs[j] = hj;
@@ -3031,35 +3079,49 @@ static int history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, voi
         S.r.rows(hj.momentum, q.n_in, hj.momentum_stride, q.n);
     }
     if (S.overlaps()) return RCMARL_ERR_ARG;
-    return launch_staged<history_attack_kernel<ARC, SUBSET>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
+    return launch_staged<history_attack_kernel<ARC, STAGE>>(P, n_jobs, bound, max_floats, ADA_THREADS, stream);
 }
 
 extern "C" {
 
 int rcmarl_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
-    return pipeline_attack<false, false>(jobs, n_jobs, stream);
+    return pipeline_attack<false, STAGE_BASE>(jobs, n_jobs, stream);
 }
 
 int rcmarl_pipeline_arc_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, void* stream) {
-    return pipeline_attack<true, false>(jobs, n_jobs, stream);
+    return pipeline_attack<true, STAGE_BASE>(jobs, n_jobs, stream);
 }
 
 int rcmarl_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
-    return history_attack<false, false>(jobs, n_jobs, stream);
+    return history_attack<false, STAGE_BASE>(jobs, n_jobs, stream);
 }
 
 int rcmarl_history_arc_attack(const rcmarl_history_attack_job* jobs, int n_jobs, void* stream) {
-    return history_attack<true, false>(jobs, n_jobs, stream);
+    return history_attack<true, STAGE_BASE>(jobs, n_jobs, stream);
 }
 
 int rcmarl_subset_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, int arc, void* stream) {
     if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
-    return arc ? pipeline_attack<true, true>(jobs, n_jobs, stream) : pipeline_attack<false, true>(jobs, n_jobs, stream);
+    return arc ? pipeline_attack<true, STAGE_SUBSET>(jobs, n_jobs, stream)
+               : pipeline_attack<false, STAGE_SUBSET>(jobs, n_jobs, stream);
 }
 
 int rcmarl_subset_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, int arc, void* stream) {
     if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
-    return arc ? history_attack<true, true>(jobs, n_jobs, stream) : history_attack<false, true>(jobs, n_jobs, stream);
+    return arc ? history_attack<true, STAGE_SUBSET>(jobs, n_jobs, stream)
+               : history_attack<false, STAGE_SUBSET>(jobs, n_jobs, stream);
+}
+
+int rcmarl_ios_pipeline_attack(const rcmarl_pipeline_attack_job* jobs, int n_jobs, int arc, void* stream) {
+    if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
+    return arc ? pipeline_attack<true, STAGE_IOS>(jobs, n_jobs, stream)
+               : pipeline_attack<false, STAGE_IOS>(jobs, n_jobs, stream);
+}
+
+int rcmarl_ios_history_attack(const rcmarl_history_attack_job* jobs, int n_jobs, int arc, void* stream) {
+    if (arc != 0 && arc != 1) return RCMARL_ERR_ARG;
+    return arc ? history_attack<true, STAGE_IOS>(jobs, n_jobs, stream)
+               : history_attack<false, STAGE_IOS>(jobs, n_jobs, stream);
 }
 
 int rcmarl_dissensus_attack(const rcmarl_dissensus_job* jobs, int n_jobs, void* stream) {

@@ -38,7 +38,7 @@ DEV_UV, DEV_STD, DEV_SGN = 0, 1, 2                # rcmarl_adaptive_dev
 ADAPTIVE_ATTACKS = {f"{k}_{d}": (kind, dev) for k, kind in (("minmax", ADAPT_MINMAX), ("minsum", ADAPT_MINSUM))
                     for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
 ADAPTIVE_MAX_FLOATS = 18 * 1536
-TAILOR_COORD, TAILOR_VECTOR, TAILOR_SPECTRAL, TAILOR_SUBSET = 0, 1, 2, 3   # rcmarl_tailored_family
+TAILOR_COORD, TAILOR_VECTOR, TAILOR_SPECTRAL, TAILOR_SUBSET, TAILOR_FILTER = 0, 1, 2, 3, 4   # rcmarl_tailored_family
 # rule-aware attacks (rcmarl_tailored_attack): candidate steps K and the staging bound; the names are TAILORED_ATTACKS
 TAILORED_STEPS = 32
 TAILORED_MAX_FLOATS = 19 * 1536
@@ -215,6 +215,8 @@ SYMBOLS = [
     ("rcmarl_history_arc_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, c_fp]),
     ("rcmarl_subset_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, C.c_int, c_fp]),
     ("rcmarl_subset_history_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, C.c_int, c_fp]),
+    ("rcmarl_ios_pipeline_attack", C.c_int, [C.POINTER(PipelineAttackJob), C.c_int, C.c_int, c_fp]),
+    ("rcmarl_ios_history_attack", C.c_int, [C.POINTER(HistoryAttackJob), C.c_int, C.c_int, c_fp]),
     ("rcmarl_dissensus_attack", C.c_int, [C.POINTER(DissensusJob), C.c_int, c_fp]),
     ("rcmarl_mimic_attack", C.c_int, [C.POINTER(MimicJob), C.c_int, c_fp]),
     ("rcmarl_values", C.c_int, [C.POINTER(Rows), C.POINTER(ValueJob), C.c_int, c_fp]),
@@ -506,6 +508,23 @@ def is_subset_attack(name):
     return isinstance(name, str) and name in SUBSET_ATTACKS
 
 
+class IosAttackKind(int):
+    """The kind check_attack gives an IOS-aware attack (rcmarl_ios_pipeline_attack / rcmarl_ios_history_attack): its
+    rcmarl_adaptive_dev, as a type of its own so that it is told apart from the attacks that do not model the
+    receiver's iterative outlier scissor."""
+
+    def __repr__(self):
+        return f"IosAttackKind({int(self)})"
+
+
+IOS_ATTACKS = {f"ios_{d}": IosAttackKind(dev) for d, dev in (("uv", DEV_UV), ("std", DEV_STD), ("sgn", DEV_SGN))}
+
+
+def is_ios_attack(name):
+    """True for the name of an IOS-aware attack: "ios_uv", "ios_std", "ios_sgn"."""
+    return isinstance(name, str) and name in IOS_ATTACKS
+
+
 class DissensusKind(int):
     """The kind check_attack gives the dissensus attack (rcmarl_dissensus_attack), a type of its own so that it is told
     apart from the other attacks' kinds; its parameter is eps >= 0."""
@@ -527,16 +546,16 @@ STATE_ATTACKS = {"dissensus": DissensusKind(0), "mimic": MimicKind(0)}
 
 def check_attack(attack):
     """(name, param) -> (kind, float param); raise RcmarlError unless the name is known and the parameter finite (for
-    "gauss", the adaptive, the tailored, the pipeline, the history, the ARC and the subset attacks and "dissensus" also
-    >= 0; for "mimic" an integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack /
+    "gauss", the adaptive, the tailored, the pipeline, the history, the ARC, the subset and the IOS attacks and
+    "dissensus" also >= 0; for "mimic" an integer in 0 .. MIMIC_MAX_T0), as rcmarl_attack / rcmarl_adaptive_attack /
     rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / rcmarl_pipeline_arc_attack /
     rcmarl_history_arc_attack / rcmarl_subset_pipeline_attack / rcmarl_subset_history_attack /
-    rcmarl_dissensus_attack / rcmarl_mimic_attack require
+    rcmarl_ios_pipeline_attack / rcmarl_ios_history_attack / rcmarl_dissensus_attack / rcmarl_mimic_attack require
     (include/rcmarl.h).  kind is the rcmarl_attack_kind id of "alie", "ipm" and "gauss",
     the pair (rcmarl_adaptive_kind, rcmarl_adaptive_dev) of an adaptive attack, whose parameter is the scale s (1 is the
     paper's attack), the TailoredKind (its rcmarl_adaptive_dev) of a tailored attack, the PipelineKind of a pipeline
-    attack, the HistoryKind of a history attack, the ArcAttackKind of an ARC attack and the SubsetAttackKind of a
-    subset attack, whose parameter is the range multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
+    attack, the HistoryKind of a history attack, the ArcAttackKind of an ARC attack, the SubsetAttackKind of a
+    subset attack and the IosAttackKind of an IOS attack, whose parameter is the range multiplier s, DissensusKind for "dissensus", whose parameter is eps (1 cancels the honest pull under a plain mean),
     and MimicKind for "mimic", whose parameter is T0 (the power steps each pair takes before its direction freezes)."""
     try:
         name, param = attack
@@ -544,17 +563,19 @@ def check_attack(attack):
     except (TypeError, ValueError):
         raise RcmarlError(f"an attack is a (name, param) pair, got {attack!r}")
     known = {**ATTACKS, **ADAPTIVE_ATTACKS, **TAILORED_ATTACKS, **PIPELINE_ATTACKS, **HISTORY_ATTACKS, **ARC_ATTACKS,
-             **SUBSET_ATTACKS, **STATE_ATTACKS}
+             **SUBSET_ATTACKS, **IOS_ATTACKS, **STATE_ATTACKS}
     if not isinstance(name, str) or name not in known:
         names = sorted(ATTACKS) + sorted(ADAPTIVE_ATTACKS) + sorted(TAILORED_ATTACKS) + sorted(PIPELINE_ATTACKS) \
-            + sorted(HISTORY_ATTACKS) + sorted(ARC_ATTACKS) + sorted(SUBSET_ATTACKS) + sorted(STATE_ATTACKS)
+            + sorted(HISTORY_ATTACKS) + sorted(ARC_ATTACKS) + sorted(SUBSET_ATTACKS) + sorted(IOS_ATTACKS) \
+            + sorted(STATE_ATTACKS)
         raise RcmarlError(f"unknown attack {name!r}: expected one of {names}")
     if name == "mimic":
         if not (math.isfinite(param) and param == int(param) and 0 <= param <= MIMIC_MAX_T0):
             raise RcmarlError(f"attack 'mimic' needs an integer T0 in 0 .. {MIMIC_MAX_T0}, got {param}")
         return known[name], param
     nonneg = name in ("gauss", "dissensus") or name in ADAPTIVE_ATTACKS or name in TAILORED_ATTACKS \
-        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS or name in ARC_ATTACKS or name in SUBSET_ATTACKS
+        or name in PIPELINE_ATTACKS or name in HISTORY_ATTACKS or name in ARC_ATTACKS or name in SUBSET_ATTACKS \
+        or name in IOS_ATTACKS
     if not math.isfinite(param) or (nonneg and param < 0):
         raise RcmarlError(f"attack {name!r} needs a finite parameter" + (" >= 0" if nonneg else "") + f", got {param}")
     return known[name], param

@@ -361,17 +361,19 @@ def pipeline_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack
     (those of tailored_attack_job, or "dnc") or a (rcmarl_tailored_family, rule id) pair; attack: "pipeline_uv",
     "pipeline_std", "pipeline_sgn", an ARC attack's name ("arc_uv", "arc_std", "arc_sgn": the same job for
     pipeline_arc_attack), a subset attack's name ("subset_uv", "subset_std", "subset_sgn": with rule "mda" or "smea"
-    the job for subset_pipeline_attack, else the same job as the ARC attack's) or an rcmarl_adaptive_dev id; mixing:
-    the receiver's mixing entry (None, "nnm",
-    "bucket" or ("bucket", s), see _lib.mixing_entry); n_perms: the attacker's shuffle samples under bucketing; (seed,
+    the job for subset_pipeline_attack, else the same job as the ARC attack's), an IOS attack's name ("ios_uv",
+    "ios_std", "ios_sgn": with rule "ios" the job for ios_pipeline_attack, else the same job as the subset attack's)
+    or an rcmarl_adaptive_dev id; mixing: the receiver's mixing entry (None, "nnm", "bucket" or ("bucket", s), see
+    _lib.mixing_entry); n_perms: the attacker's shuffle samples under bucketing; (seed,
     attacker, receiver, net, round, epoch): the Philox key and counter words of those samples; model_out [n]: R_0 of the
     pick.  Names are checked here, ids and limits by the library."""
     if isinstance(attack, str):
-        if not (L.is_pipeline_attack(attack) or L.is_arc_attack(attack) or L.is_subset_attack(attack)):
-            raise L.RcmarlError(f"unknown pipeline attack {attack!r}: expected one of "
-                                f"{sorted(L.PIPELINE_ATTACKS) + sorted(L.ARC_ATTACKS) + sorted(L.SUBSET_ATTACKS)}")
-        rule = _subset_family(attack, rule)
-        attack = {**L.PIPELINE_ATTACKS, **L.ARC_ATTACKS, **L.SUBSET_ATTACKS}[attack]
+        if not (L.is_pipeline_attack(attack) or L.is_arc_attack(attack) or L.is_subset_attack(attack)
+                or L.is_ios_attack(attack)):
+            names = sorted(L.PIPELINE_ATTACKS) + sorted(L.ARC_ATTACKS) + sorted(L.SUBSET_ATTACKS) + sorted(L.IOS_ATTACKS)
+            raise L.RcmarlError(f"unknown pipeline attack {attack!r}: expected one of {names}")
+        rule = _chain_family(attack, rule)
+        attack = {**L.PIPELINE_ATTACKS, **L.ARC_ATTACKS, **L.SUBSET_ATTACKS, **L.IOS_ATTACKS}[attack]
     if L.is_spectral_rule(rule):
         rule = (L.TAILOR_SPECTRAL, L.SPECTRAL_RULES[rule])
     mixing = L.mixing_entry(mixing)
@@ -386,9 +388,14 @@ def pipeline_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack
     return j
 
 
-def _subset_family(attack, rule):
-    """(TAILOR_SUBSET, rule id) for a subset attack's name against "mda" / "smea", else rule unchanged."""
-    return (L.TAILOR_SUBSET, L.SUBSET_RULES[rule]) if L.is_subset_attack(attack) and L.is_subset_rule(rule) else rule
+def _chain_family(attack, rule):
+    """(TAILOR_SUBSET, rule id) for a subset or IOS attack's name against "mda" / "smea", (TAILOR_FILTER, FILTER_IOS)
+    for an IOS attack's name against "ios", else rule unchanged."""
+    if (L.is_subset_attack(attack) or L.is_ios_attack(attack)) and L.is_subset_rule(rule):
+        return L.TAILOR_SUBSET, L.SUBSET_RULES[rule]
+    if L.is_ios_attack(attack) and L.is_filter_rule(rule):
+        return L.TAILOR_FILTER, L.FILTER_RULES[rule]
+    return rule
 
 
 def pipeline_attack(jobs):
@@ -406,17 +413,19 @@ def history_attack_job(dst, msgs, msg_stride, n, slots, honest, rule, H, attack,
                        beta, first, own, gamma_out=None, model_out=None):
     """rcmarl_history_attack_job: slots, honest, rule, H and scale as pipeline_attack_job; attack: "history_uv",
     "history_std", "history_sgn", an ARC attack's name (the same job for history_arc_attack), a subset attack's name
-    (with rule "mda" or "smea" the job for subset_history_attack, else the same job as the ARC attack's) or an
+    (with rule "mda" or "smea" the job for subset_history_attack, else the same job as the ARC attack's), an IOS
+    attack's name (with rule "ios" the job for ios_history_attack, else the same job as the subset attack's) or an
     rcmarl_adaptive_dev id; ref the receiver's reference c [>= n]; momentum its state
     M, row k at momentum + k * momentum_stride (read only); beta in [0, 1); first 1 for the receiver's first step; own:
     the crafted slot indices that receive dst; model_out [n]: R of the pick.  Names and own slots are checked here, ids
     and limits by the library."""
     if isinstance(attack, str):
-        if not (L.is_history_attack(attack) or L.is_arc_attack(attack) or L.is_subset_attack(attack)):
-            raise L.RcmarlError(f"unknown history attack {attack!r}: expected one of "
-                                f"{sorted(L.HISTORY_ATTACKS) + sorted(L.ARC_ATTACKS) + sorted(L.SUBSET_ATTACKS)}")
-        rule = _subset_family(attack, rule)
-        attack = {**L.HISTORY_ATTACKS, **L.ARC_ATTACKS, **L.SUBSET_ATTACKS}[attack]
+        if not (L.is_history_attack(attack) or L.is_arc_attack(attack) or L.is_subset_attack(attack)
+                or L.is_ios_attack(attack)):
+            names = sorted(L.HISTORY_ATTACKS) + sorted(L.ARC_ATTACKS) + sorted(L.SUBSET_ATTACKS) + sorted(L.IOS_ATTACKS)
+            raise L.RcmarlError(f"unknown history attack {attack!r}: expected one of {names}")
+        rule = _chain_family(attack, rule)
+        attack = {**L.HISTORY_ATTACKS, **L.ARC_ATTACKS, **L.SUBSET_ATTACKS, **L.IOS_ATTACKS}[attack]
     if L.is_spectral_rule(rule):
         rule = (L.TAILOR_SPECTRAL, L.SPECTRAL_RULES[rule])
     bad = [k for k in own if not (isinstance(k, (int, np.integer)) and 0 <= k < len(slots))]
@@ -449,6 +458,20 @@ def subset_history_attack(jobs, arc):
     TAILOR_SUBSET), through the receiver's clipping step when arc is true."""
     a = jobs if isinstance(jobs, C.Array) else job_array(L.HistoryAttackJob, jobs)
     L.check(L.lib().rcmarl_subset_history_attack(a, len(a), int(arc), _stream()), "rcmarl_subset_history_attack")
+
+
+def ios_pipeline_attack(jobs, arc):
+    """rcmarl_ios_pipeline_attack: pipeline_attack_job's jobs against IOS receivers (family TAILOR_FILTER), through the
+    receiver's clipping step when arc is true."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.PipelineAttackJob, jobs)
+    L.check(L.lib().rcmarl_ios_pipeline_attack(a, len(a), int(arc), _stream()), "rcmarl_ios_pipeline_attack")
+
+
+def ios_history_attack(jobs, arc):
+    """rcmarl_ios_history_attack: history_attack_job's jobs against IOS receivers with momentum (family TAILOR_FILTER),
+    through the receiver's clipping step when arc is true."""
+    a = jobs if isinstance(jobs, C.Array) else job_array(L.HistoryAttackJob, jobs)
+    L.check(L.lib().rcmarl_ios_history_attack(a, len(a), int(arc), _stream()), "rcmarl_ios_history_attack")
 
 
 def history_arc_attack(jobs):

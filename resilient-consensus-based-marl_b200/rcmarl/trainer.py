@@ -170,7 +170,8 @@ class Trainer:
                         else 'history' if e in self.hist_pairs else 'ARC')
                 raise L.RcmarlError(f"Byzantine agent {b} runs a {name} attack against agent {j}, whose rule "
                                     f"{agg[j]!r} the attack does not model")
-        for e in self.arc_pairs + self.subset_pairs:   # an ARC job stages k_clip clipped rows on top of its base job's
+        # an ARC job stages k_clip clipped rows on top of its base job's
+        for e in self.arc_pairs + self.subset_pairs + self.ios_pairs:
             b, j, _ = self.byz_pairs[e]
             n_real = sum(k >= 0 for k in self._tailored_slots(j)[0])
             kc = L.arc_count(self.H[j], len(self.in_nodes[j])) if self.clipping[j] is not None else 0
@@ -178,9 +179,9 @@ class Trainer:
             if self.subset_rule[j] is not None:    # a subset job stages as its ARC form, under a bound of its own
                 bound = L.SUBSET_ATTACK_MAX_FLOATS
             if floats > bound:
-                raise L.RcmarlError(f"Byzantine agent {b} runs {'an ARC' if e in self.arc_pairs else 'a subset'} "
-                                    f"attack against agent {j}, whose job stages {floats} floats, more than the "
-                                    f"{bound} the library admits")
+                name = 'an ARC' if e in self.arc_pairs else 'a subset' if e in self.subset_pairs else 'an IOS'
+                raise L.RcmarlError(f"Byzantine agent {b} runs {name} attack against agent {j}, whose job stages "
+                                    f"{floats} floats, more than the {bound} the library admits")
         # row of the aggregate of each cooperative agent with a distance-based rule, after the Byzantine pair rows, then
         # that of each cooperative agent on dnc, then that of each on mda / smea, then that of each on ios
         self.vec_agents = [i for i in self.coop if self.vector_rule[i] is not None]
@@ -383,8 +384,14 @@ class Trainer:
         # launches of their own, after the ARC ones (_subset_job_groups)
         self.subset_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
                              if isinstance(self.attack[b][0], L.SubsetAttackKind)]
+        # the pairs whose attacker runs an IOS-aware attack (kind L.IosAttackKind): against an ios receiver the history
+        # or pipeline search through its whole chain and its iterative outlier scissor (rcmarl_ios_history_attack /
+        # rcmarl_ios_pipeline_attack), against any other exactly a subset pair's job; launches of their own, after the
+        # subset ones (_ios_job_groups)
+        self.ios_pairs = [e for e, (b, _, _) in enumerate(self.byz_pairs)
+                          if isinstance(self.attack[b][0], L.IosAttackKind)]
         self.gamma_pairs = (self.adapt_pairs + self.tailor_pairs + self.pipe_pairs + self.hist_pairs + self.arc_pairs
-                            + self.subset_pairs)
+                            + self.subset_pairs + self.ios_pairs)
         # the pairs whose attacker runs the dissensus attack (rcmarl_dissensus_attack) and those that run the mimic attack
         # (rcmarl_mimic_attack, whose direction state carries over between epochs and rounds): a launch each, after the
         # tailored one
@@ -476,11 +483,11 @@ class Trainer:
         return out
 
     def attack_gammas(self):
-        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline, a history, an ARC or a
-        subset attack: float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last update round
-        (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline, history, ARC or subset attack gamma_i*,
-        rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / their ARC and subset forms); entry 0
-        for the critic, 1 for the team-reward net."""
+        """{(attacker b, cooperative receiver j) of a min-max / min-sum, a tailored, a pipeline, a history, an ARC, a
+        subset or an IOS attack: float32 [2]}: the gamma of the message b crafted for j in the last epoch of the last
+        update round (include/rcmarl.h, rcmarl_adaptive_attack; for a tailored, pipeline, history, ARC, subset or IOS
+        attack gamma_i*, rcmarl_tailored_attack / rcmarl_pipeline_attack / rcmarl_history_attack / their ARC, subset and
+        IOS forms); entry 0 for the critic, 1 for the team-reward net."""
         if not self.gamma_pairs:
             return {}
         g = self.att_gamma.cpu().numpy()
@@ -510,9 +517,9 @@ class Trainer:
 
     def _arc_staging(self, j, n_real, kc):
         """(floats, bound) of the job an ARC pair against receiver j gets (include/rcmarl.h): the history form's
-        (n_in + 4 + (DnC ? 2 : 0) + k_clip) * PT if j has momentum, else the pipeline form's (n_real + n_mixed + 4 +
-        (DnC ? 2 : 0) + k_clip) * PT, with k_clip = kc (0 when j does not clip)."""
-        n_in, extra = len(self.in_nodes[j]), (2 if self.dnc[j] else 0) + 4 + kc
+        (n_in + 4 + (DnC or IOS ? 2 : 0) + k_clip) * PT if j has momentum, else the pipeline form's (n_real + n_mixed +
+        4 + (DnC or IOS ? 2 : 0) + k_clip) * PT, with k_clip = kc (0 when j does not clip)."""
+        n_in, extra = len(self.in_nodes[j]), (2 if self.dnc[j] or self.ios[j] else 0) + 4 + kc
         PT = L.param_count(3 * self.NA, 1)             # the TR net, the larger of the two
         if self.momentum[j] is not None:
             return (n_in + extra) * PT, L.HISTORY_MAX_FLOATS
@@ -540,22 +547,34 @@ class Trainer:
                     + len(self.arc_pairs))
         return self._chain_job_groups(self.subset_pairs, n_before)
 
+    def _ios_job_groups(self):
+        """_arc_job_groups for the IOS pairs, launched after the subset groups: against an ios receiver the history form
+        (momentum) or the pipeline form (with the receiver's mixing) of rcmarl_ios_history_attack /
+        rcmarl_ios_pipeline_attack, with arc = whether the receiver clips (the launch is functools.partial of
+        ops.ios_history_attack / ops.ios_pipeline_attack with that arc); against an mda / smea receiver exactly the job,
+        and the launch, a subset pair gets; against any other exactly those an ARC pair gets."""
+        n_before = (len(self.adapt_pairs) + len(self.tailor_pairs) + len(self.pipe_pairs) + len(self.hist_pairs)
+                    + len(self.arc_pairs) + len(self.subset_pairs))
+        return self._chain_job_groups(self.ios_pairs, n_before)
+
     def _chain_job_groups(self, pairs, n_before):
-        """The groups of _arc_job_groups / _subset_job_groups for `pairs`, whose gamma rows start at n_before."""
+        """The groups of _arc_job_groups / _subset_job_groups / _ios_job_groups for `pairs`, whose gamma rows start at
+        n_before."""
         NA = self.NA
         mom_index = {i: q for q, i in enumerate(self.mom_agents)}
-        tables = {}                                    # (subset rule, history form, clips) -> ([jobs], [mom])
+        tables = {}                                    # (ios rule, subset rule, history form, clips) -> ([jobs], [mom])
         for q_pair, e in enumerate(pairs):
             b, j, _ = self.byz_pairs[e]
             kind, param = self.attack[b]
             slots, hon = self._tailored_slots(j)
-            subset = self.subset_rule[j] is not None
+            subset, ios = self.subset_rule[j] is not None, self.ios[j]
             rule = ((L.TAILOR_SUBSET, self.subset_rule[j]) if subset
+                    else (L.TAILOR_FILTER, L.FILTER_IOS) if ios
                     else (L.TAILOR_VECTOR, self.vector_rule[j]) if self.vector_rule[j] is not None
                     else (L.TAILOR_SPECTRAL, L.SPECTRAL_DNC) if self.dnc[j]
                     else (L.TAILOR_COORD, self.aggregation[j]))
             hist = self.momentum[j] is not None
-            jobs, moms = tables.setdefault((subset, hist, self.clipping[j] is not None), ([], []))
+            jobs, moms = tables.setdefault((ios, subset, hist, self.clipping[j] is not None), ([], []))
             for t, (msgs, P, ref) in enumerate(((self.msg_c, self.PC, self.critic[j]), (self.msg_t, self.PT, self.tr[j]))):
                 gamma_out = self.att_gamma[n_before + q_pair, t:t + 1]
                 if hist:
@@ -574,8 +593,9 @@ class Trainer:
                   (False, True): ops.pipeline_arc_attack, (False, False): ops.pipeline_attack}
         cls = {True: L.HistoryAttackJob, False: L.PipelineAttackJob}
         out = []
-        for (subset, hist, clips), (jobs, moms) in sorted(tables.items(), reverse=True):
-            fn = (functools.partial(ops.subset_history_attack if hist else ops.subset_pipeline_attack, arc=clips)
+        for (ios, subset, hist, clips), (jobs, moms) in sorted(tables.items(), reverse=True):
+            fn = (functools.partial(ops.ios_history_attack if hist else ops.ios_pipeline_attack, arc=clips) if ios
+                  else functools.partial(ops.subset_history_attack if hist else ops.subset_pipeline_attack, arc=clips)
                   if subset else launch[(hist, clips)])
             for g in range(0, len(jobs), L.MAX_JOBS):
                 out.append((fn, ops.job_array(cls[hist], jobs[g:g + L.MAX_JOBS]), moms[g:g + L.MAX_JOBS] if hist else None))
@@ -606,7 +626,8 @@ class Trainer:
         mom_index = {i: q for q, i in enumerate(self.mom_agents)}
         diss_set = set(self.diss_pairs)
         mimic_row = {e: q for q, e in enumerate(self.mimic_pairs)}
-        arc_set = set(self.arc_pairs + self.subset_pairs)   # their jobs are _arc_job_groups' / _subset_job_groups'
+        # their jobs are _arc_job_groups' / _subset_job_groups' / _ios_job_groups'
+        arc_set = set(self.arc_pairs + self.subset_pairs + self.ios_pairs)
         for e, (b, j, honest) in enumerate(self.byz_pairs):
             if e in arc_set:
                 continue
@@ -883,7 +904,7 @@ class Trainer:
         # the Byzantine messages' job tables (_attack_job_groups)
         (att_groups, ada_groups, tail_groups, pipe_groups, hist_groups, hist_mom, diss_groups, mimic_t0,
          mimic_groups) = self._attack_job_groups()
-        arc_groups = self._arc_job_groups() + self._subset_job_groups()
+        arc_groups = self._arc_job_groups() + self._subset_job_groups() + self._ios_job_groups()
 
         # the mixed rows of the agents that mix, from the messages each hears (crafted Byzantine ones included): at most
         # 16 cooperative agents x 2 nets, so one nnm launch and one bucketing launch per epoch.  A bucketing job draws

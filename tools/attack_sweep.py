@@ -36,8 +36,10 @@ pipeline search through the receiver's clipping step as well (rcmarl_history_arc
 against a receiver that does not clip they are the history attacks, and mda or smea cells are marked refused.  The
 subset-aware attacks (subset_uv, subset_std, subset_sgn, range multiplier 2 by default) run that search through an mda or
 smea receiver's exact subset selection as well (rcmarl_subset_history_attack / rcmarl_subset_pipeline_attack); against
-any other rule they are the ARC-aware attacks.  No rule-aware attack (tailored, pipeline, history, ARC-aware or
-subset-aware) models ios: those cells are marked refused.
+any other rule they are the ARC-aware attacks.  The IOS-aware attacks (ios_uv, ios_std, ios_sgn, range multiplier 2 by
+default) run that search through an ios receiver's iterative outlier scissor as well (rcmarl_ios_history_attack /
+rcmarl_ios_pipeline_attack); against any other rule they are the subset-aware attacks.  No other rule-aware attack
+(tailored, pipeline, history, ARC-aware or subset-aware) models ios: those cells are marked refused.
 The list may also name the dissensus attack (rcmarl_dissensus_attack, dissensus[:eps], eps = 1 by default: it cancels
 the receiver's honest pull under a plain mean) and the mimic attack (rcmarl_mimic_attack, mimic[:T0], T0 = 50 power steps
 by default, after which the direction is frozen); for mimic the table reports, per receiver, the agent whose message
@@ -75,7 +77,8 @@ from rcmarl.trainer import Trainer             # noqa: E402
 PARAMS = {"alie": 1.0, "ipm": 0.5, "gauss": 0.3, "tailored_uv": 2.0, "tailored_std": 2.0, "tailored_sgn": 2.0,
           "pipeline_uv": 2.0, "pipeline_std": 2.0, "pipeline_sgn": 2.0, "history_uv": 2.0, "history_std": 2.0,
           "history_sgn": 2.0, "arc_uv": 2.0, "arc_std": 2.0, "arc_sgn": 2.0,
-          "subset_uv": 2.0, "subset_std": 2.0, "subset_sgn": 2.0, "dissensus": 1.0, "mimic": 50.0}
+          "subset_uv": 2.0, "subset_std": 2.0, "subset_sgn": 2.0, "ios_uv": 2.0, "ios_std": 2.0, "ios_sgn": 2.0,
+          "dissensus": 1.0, "mimic": 50.0}
 n_blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 40
 n_envs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 timed_rounds = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -122,6 +125,7 @@ PIPELINE = ("pipeline_uv", "pipeline_std", "pipeline_sgn")
 HISTORY = ("history_uv", "history_std", "history_sgn")
 ARC = ("arc_uv", "arc_std", "arc_sgn")
 SUBSET = ("subset_uv", "subset_std", "subset_sgn")
+IOS = ("ios_uv", "ios_std", "ios_sgn")
 ATTACKS = tuple((a.split(":")[0], float(a.split(":")[1]) if ":" in a else PARAMS.get(a, 1.0))
                 for a in (sys.argv[6] if len(sys.argv) > 6 else "alie,ipm,gauss").split(","))
 tail = 10                                       # 10 blocks x 50 episodes = the last 500 episodes
@@ -247,7 +251,7 @@ def timing_line(rt):
                                                                for k in timed_rules()[1:]])
 
 
-adaptive = any(a in ADAPTIVE + TAILORED + PIPELINE + HISTORY + ARC + SUBSET for a, _ in ATTACKS)
+adaptive = any(a in ADAPTIVE + TAILORED + PIPELINE + HISTORY + ARC + SUBSET + IOS for a, _ in ATTACKS)
 tailored = any(a in TAILORED for a, _ in ATTACKS)
 pipeline = any(a in PIPELINE for a, _ in ATTACKS)
 history = any(a in HISTORY for a, _ in ATTACKS)
@@ -327,8 +331,8 @@ for rule in RULES:
         if vector:
             cell["byz_weight"] = float(np.mean(byz)) if split_rule(rule)[1] in WHOLE else None
         if adaptive:
-            cell["gamma"] = float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED + PIPELINE + HISTORY + ARC + SUBSET \
-                else None
+            cell["gamma"] = (float(np.mean(gam)) if attack[0] in ADAPTIVE + TAILORED + PIPELINE + HISTORY + ARC + SUBSET
+                             + IOS else None)
         if mimic:
             cell["copied"] = {str(j): ks for j, ks in copied.items()} if copied else None
         result["cells"].append(cell)

@@ -2,8 +2,9 @@
 (rcmarl_adaptive_attack), DnC (rcmarl_dnc_aggregate), nearest-neighbour mixing (rcmarl_nnm_mix), bucketing
 (rcmarl_bucket_mix), the tailored attacks (rcmarl_tailored_attack), the subset-selection rules MDA / SMEA
 (rcmarl_subset_aggregate), per-neighbour momentum (rcmarl_momentum_mix), the iterative outlier scissor
-(rcmarl_ios_aggregate), the pipeline attacks (rcmarl_pipeline_attack) and the history attacks (rcmarl_history_attack)
-between two builds of librcmarl.so, bit for bit.  Their kernels share their bodies with tailored_attack_kernel, pipeline_attack_kernel and history_attack_kernel
+(rcmarl_ios_aggregate), the pipeline attacks (rcmarl_pipeline_attack), the history attacks (rcmarl_history_attack)
+and the IOS-aware attacks (rcmarl_ios_pipeline_attack, rcmarl_ios_history_attack) between two builds of librcmarl.so,
+bit for bit.  Their kernels share their bodies with tailored_attack_kernel, pipeline_attack_kernel and history_attack_kernel
 (vector_rule, adaptive_gamma, dnc_rule, warp_jacobi, nnm_rows, bucket_draw / bucket_means, tailored_stage /
 tailored_range, the candidate search and the momentum step in csrc/train_kernels.cu), so a change there may change
 their register allocation and SASS; this shows whether it changed anything they compute.
@@ -16,8 +17,9 @@ attack x rule at n_in 2 .. 16 (scale 2, with gamma), MDA and SMEA at n_in 1 .. 1
 weights), momentum at n_in 1 .. 16 over three steps (beta 0.9, the rows and the state after each), IOS at n_in
 1 .. 16 (H drawn per job, with the weights), every pipeline
 attack x rule (DnC included) x mixing (none, nnm, bucketing at s = 2 with 3 samples) at n_in 2 .. 16 with gamma and
-model_out, and history_std x rule at n_in 2 .. 16 for (beta, first) = (0.9, 0), (0.99, 0), (0.5, 1), at the trainer's
-parameter counts.  Entry points a build does not export are skipped when loading it, so a
+model_out, history_std x rule at n_in 2 .. 16 for (beta, first) = (0.9, 0), (0.99, 0), (0.5, 1), and ios_std in the
+pipeline form (mixing none, nnm, bucketing at s = 2) and ios_uv in the history form (beta 0.9) at n_in 2 .. 16 with and
+without ARC (H drawn per job), at the trainer's parameter counts.  Entry points a build does not export are skipped when loading it, so a
 build from before rcmarl_tailored_attack existed loads too; the outputs of an entry point only one build exports are
 listed and not compared.
 
@@ -196,6 +198,46 @@ if hasattr(lib, "rcmarl_history_attack"):
                 dsts.append(d)
             ops.history_attack(jobs)
             named.update({f"history_{rule}_{beta}_{first}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
+if hasattr(lib, "rcmarl_ios_pipeline_attack"):
+    rs_att = np.random.RandomState(79)                             # its own draws: the later inputs stay the same
+    ref = msgs[0] * 0.5
+    M = (torch.randn(16, P, generator=torch.Generator().manual_seed(6)) * 0.3).cuda()
+    for arc in (0, 1):
+        for mixing in (None, "nnm", ("bucket", 2)):
+            jobs, dsts = [], []
+            for n_in in range(2, 17):
+                n_cr = 1 + n_in % 3 if n_in > 3 else 1
+                real = [int(x) for x in rs_att.choice(20, size=n_in - n_cr, replace=False)]
+                slots = real[:1] + [-1] * n_cr + real[1:]
+                honest = [k for k, s in enumerate(slots) if 0 <= s < 16] or [0]
+                n_rows = 1 + (n_in - 2) // 2 + 1 if isinstance(mixing, tuple) else n_in
+                n_mixed = n_in if mixing == "nnm" else n_rows - 1 if isinstance(mixing, tuple) else 0
+                H, n = int(rs_att.randint(0, n_rows)), PC[n_in % 4]
+                if (len(real) + n_mixed + 6 + arc * L.arc_count(H, n_in)) * n > L.PIPELINE_MAX_FLOATS:
+                    continue                                      # past the staging bound
+                d = torch.full((2 * P + 1,), float("nan"), device="cuda")
+                jobs.append(ops.pipeline_attack_job(d[:P], msgs, P, n, slots, honest, "ios", H, "ios_std", 2.0,
+                                                    mixing=mixing, n_perms=3, seed=11, attacker=n_in, receiver=2,
+                                                    net=1, round=5, epoch=1, gamma_out=d[2 * P:],
+                                                    model_out=d[P:2 * P]))
+                dsts.append(d)
+            ops.ios_pipeline_attack(jobs, arc)
+            named.update({f"ios_pipeline_{arc}_{mixing}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
+        jobs, dsts = [], []
+        for n_in in range(2, 17):
+            n_cr = 1 + n_in % 3 if n_in > 3 else 1
+            real = [int(x) for x in rs_att.choice(20, size=n_in - n_cr, replace=False)]
+            slots = real[:1] + [-1] * n_cr + real[1:]
+            honest = [k for k, s in enumerate(slots) if 0 <= s < 16] or [0]
+            H, n = int(rs_att.randint(0, n_in)), PC[n_in % 4]
+            if (n_in + 6 + arc * L.arc_count(H, n_in)) * n > L.HISTORY_MAX_FLOATS:
+                continue                                          # past the staging bound
+            d = torch.full((2 * P + 1,), float("nan"), device="cuda")
+            jobs.append(ops.history_attack_job(d[:P], msgs, P, n, slots, honest, "ios", H, "ios_uv", 2.0, ref, M, P,
+                                               0.9, 0, [slots.index(-1)], gamma_out=d[2 * P:], model_out=d[P:2 * P]))
+            dsts.append(d)
+        ops.ios_history_attack(jobs, arc)
+        named.update({f"ios_history_{arc}_{k}": d.cpu().numpy() for k, d in enumerate(dsts)})
 np.savez(sys.argv[1], *outs, **named)
 '''
 
@@ -217,8 +259,8 @@ def main():
     only = sorted(set(a.files) ^ set(b.files))
     diff = [k for k in common if a[k].tobytes() != b[k].tobytes()]
     print(f"{len(common)} output arrays (vector_aggregate, adaptive_attack, dnc_aggregate, nnm_mix, bucket_mix, "
-          "tailored_attack, subset_aggregate, momentum_mix, ios_aggregate, pipeline_attack and history_attack "
-          "outputs): "
+          "tailored_attack, subset_aggregate, momentum_mix, ios_aggregate, pipeline_attack, history_attack, "
+          "ios_pipeline_attack and ios_history_attack outputs): "
           + ("bitwise equal" if not diff else f"{len(diff)} differ: {diff[:8]}")
           + (f"; {len(only)} from an entry point only one build exports, not compared" if only else ""))
     sys.exit(1 if diff or not common else 0)
